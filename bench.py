@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Benchmark of the hot path: images/sec of the full training step (BASELINE.json `metric`).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a (H100) path
+    python bench.py ... --dump-outputs DIR                    # also write the last timed step's outputs as .npy
     python bench.py --impl reference --gpus N --steps K ...   # the reference arithmetic on the box's host cores
 
 Workload (BASELINE.json configs[1]): FLUX-VAE config ch=128, ch_mult=1,2,4,4, z=16, 256x256 synthetic images,
@@ -13,7 +14,12 @@ Printed JSON (one line, rank 0): see the contract in the task statement. `value`
 timed, max over ranks; `e2e` = the same step through the public Trainer API with pinned host batches (H2D inside the timed
 region) and a device->host read of the loss every step; `roofline` = achieved tensor throughput of the dominant kernel
 (vqb::conv_gemm_kernel, fwd + dgrad launches) from CUDA events around every launch of an extra profiled step;
-`cpu_baseline` = the CPU oracle (port of the reference arithmetic) on this box's host cores, bounded sample.
+`cpu_baseline` = the CPU oracle (port of the reference arithmetic) on this machine's host cores, bounded sample.
+
+--dump-outputs DIR writes what the timed path computed in its last timed step: every tensor the step returns (losses,
+z, the reconstruction) and a fixed, seeded sample of the VAE parameters after that step's optimizer update, as float32
+DIR/<name>.npy (arrays above 4M elements as a fixed, seeded sample, <name>_sample.npy). Inputs and initialisation are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -59,8 +65,49 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
-    return 1400.0, "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md; MEASURED_PEAKS.json absent)"
+        return d.get("bf16_tflops_sustained", 989.0), "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
+    return 989.0, "H100 SXM data-sheet dense BF16 rate at 700 W (not a measured peak; MEASURED_PEAKS.json absent)"
+
+
+DUMP_MAX_ELEMS = 4 << 20  # per array: 16 MB of float32
+DUMP_BUDGET_BYTES = 64 << 20  # all arrays of one dump together
+
+
+def _dump_array(d, name, t, max_elems):
+    """Writes t as float32 DIR/<name>.npy, or a fixed, seeded sample of max_elems elements as <name>_sample.npy.
+    Returns the bytes written."""
+    import numpy as np
+
+    a = t.detach().float().cpu().numpy().reshape(-1) if t.dim() else t.detach().float().cpu().numpy()
+    if a.size > max_elems:
+        idx = np.sort(np.random.default_rng(0).choice(a.size, max_elems, replace=False))
+        a, name = a[idx], name + "_sample"
+    elif t.dim():
+        a = a.reshape(tuple(t.shape))
+    a = a.astype(np.float32)
+    np.save(os.path.join(d, name + ".npy"), a)
+    return a.nbytes
+
+
+def dump_outputs(d, out, vae):
+    """The last timed step's returned tensors + a seeded 1M-element sample of the updated VAE parameters, at most
+    DUMP_BUDGET_BYTES in all: an array that would overflow what is left is written as a seeded sample that fits."""
+    os.makedirs(d, exist_ok=True)
+    flat = torch.cat([p.detach().float().reshape(-1) for _, p in sorted(vae.named_parameters())])
+    gen = torch.Generator(device=flat.device).manual_seed(0)
+    idx = torch.randperm(flat.numel(), generator=gen, device=flat.device)[:1 << 20].sort().values
+    left = DUMP_BUDGET_BYTES - _dump_array(d, "vae_params_sample", flat[idx], DUMP_MAX_ELEMS)
+    arrays = []
+    for k, v in sorted(out.items()):
+        if isinstance(v, dict):
+            arrays += [(f"{k}.{kk}", vv) for kk, vv in sorted(v.items()) if torch.is_tensor(vv)]
+        elif torch.is_tensor(v):
+            arrays.append((k, v))
+    for name, t in arrays:
+        cap = min(DUMP_MAX_ELEMS, left // 4)
+        if cap < 1:
+            raise RuntimeError(f"--dump-outputs: no room left for {name} within {DUMP_BUDGET_BYTES >> 20} MB")
+        left -= _dump_array(d, name, t, cap)
 
 
 class ClockSampler:
@@ -261,9 +308,9 @@ def emit_json(line):
     out.flush()
 
 
-def eager_b200_leg(cfg, B, world, rank, device, steps, warmup):
+def eager_leg(cfg, B, world, rank, device, steps, warmup):
     """The kernel-for-kernel bar (SURVEY.md §8d "Reference beside it (2)"): the reference's arithmetic executed by stock
-    PyTorch eager (cuDNN / ATen) on this same B200, with the reference's own precision mix — TF32 encoder / LPIPS / D
+    PyTorch eager (cuDNN / ATen) on this same GPU, with the reference's own precision mix — TF32 encoder / LPIPS / D
     (vae_trainer.py:18-19), bf16-autocast decoder (:453,623), fp32 GroupNorm — fused AdamW, and the gradient all-reduce
     the reference intends for N > 1. The reference tree is plain Python without packaging (`pip install /root/reference`
     fails: no setup.py / pyproject.toml) and may not be copied, so its modules are represented by the oracle
@@ -402,30 +449,20 @@ def _eager_generator_step_hr(SO, VO, LP, vsd, lsd, dsd, real_hr, real_enc, vcfg,
     return {"loss": loss.detach()}
 
 
-def load_traffic_table():
-    """Measured DRAM traffic of the dominant conv shapes (ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum per
-    launch) next to their algorithmic bytes: profiles/r02_ncu_traffic.json when present, else the round-1 capture."""
-    for name in ("r02_ncu_traffic.json", "r01_ncu_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return name, json.load(f)
-        except Exception:
-            continue
-    return None, None
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", type=str, default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", type=str, default="native", choices=["native", "reference"])
     ap.add_argument("--config", type=str, default=os.environ.get("VQB_BENCH_CONFIG", "lpips"), choices=sorted(CONFIGS),
                     help="lpips = BASELINE configs[1] (the metric's config), gan = [2], vq = [3], hr512 = [4]")
     ap.add_argument("--batch", type=int, default=int(os.environ.get("VQB_BENCH_BATCH", "0")), help="per-GPU batch")
     ap.add_argument("--gan", action="store_true", help="alias of --config gan")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--no-eager", action="store_true", help="skip the PyTorch-eager-on-B200 peer leg")
+    ap.add_argument("--no-eager", action="store_true", help="skip the PyTorch-eager peer leg on the same GPU")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32, <= 64 MB)")
     ap.add_argument("--no-graph", action="store_true", help="run the step eagerly instead of as one CUDA-graph replay")
     args = ap.parse_args()
     if args.gan and args.config == "lpips":
@@ -450,7 +487,7 @@ def main():
     import native
     import vae_trainer as vt
 
-    assert torch.cuda.is_available(), "bench.py needs a CUDA (sm_100a) device: there is no CPU path"
+    assert torch.cuda.is_available(), "bench.py needs a CUDA (sm_90a) device: there is no CPU path"
     torch.cuda.set_device(local_rank)
     device = f"cuda:{local_rank}"
     if world > 1:
@@ -496,6 +533,8 @@ def main():
     if graphed:  # replays do not pass through the C entry points: kernels per replay (counted at capture) x replays
         launches = tr.graph_launches_per_step * K
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, tr.vae)
 
     # ---------------- timed: end to end (pinned host batch -> H2D inside, loss read back every step)
     barrier()
@@ -520,7 +559,7 @@ def main():
     prof = profile_conv_kernels(tr, dev_batches[0])
     peak_mem = torch.cuda.max_memory_allocated() / 2 ** 30
 
-    # ---------------- the PyTorch-eager-on-B200 peer (same step, same batch, same GPUs), after freeing our own state
+    # ---------------- the PyTorch-eager peer (same step, same batch, same GPUs), after freeing our own state
     eager = None
     if not args.no_eager:
         tr._graph = None
@@ -531,7 +570,7 @@ def main():
         torch.cuda.empty_cache()
         torch.cuda.reset_peak_memory_stats()
         try:
-            eager = eager_b200_leg(cfg, B, world, rank, device, K, W)
+            eager = eager_leg(cfg, B, world, rank, device, K, W)
         except Exception as e:  # the peer must never take the product line down
             eager = {"unavailable": f"{type(e).__name__}: {str(e)[:200]}"}
 
@@ -539,10 +578,6 @@ def main():
         peak, peak_src = load_peaks()
         value = world * B / (ms * 1e-3)
         e2e = world * B / (ms_e2e * 1e-3)
-        tname, ttab = load_traffic_table()
-        conv_traffic = None
-        if ttab is not None:
-            conv_traffic = ttab.get("conv_gemm_bytes_per_launch", ttab.get("conv_gemm"))
         tflop = cfg["tflop"]
         line = {
             "metric": "images/sec", "value": value, "unit": "images/s", "n_gpus": world, "steps": K, "warmup": W,
@@ -553,7 +588,7 @@ def main():
                                    "(the reference trains with its Dropout(0.5) live; `Trainer(lpips_eval=False)` "
                                    "reproduces that)",
                        "name": args.config, "cuda_graph": graphed, "graph_prep_steps": PREP, "per_gpu_batch": B, "global_batch": world * B, "parallelism": f"dp{world}",
-                       "l2": "no explicit flush: per-step working set (activations ~0.9 GB/image) >> 126 MB L2",
+                       "l2": "no explicit flush: per-step working set (activations ~0.9 GB/image) >> 50 MB L2",
                        "tflop_per_image": tflop},
             "e2e": {"value": e2e, "unit": "images/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": B * 3 * R * R * 4,
                     "d2h_bytes_per_step": 4, "last_loss": last_loss},
@@ -562,10 +597,9 @@ def main():
             "peak_mem_gib": peak_mem,
             "achieved_step_tflops_per_gpu": tflop * B / (ms * 1e-3),
             "step_frac_of_peak": tflop * B / (ms * 1e-3) / peak,
-            "roofline": {"kernel": "vqb::conv_gemm_kernel (tcgen05 implicit-GEMM conv, fwd+dgrad launches of one step)",
+            "roofline": {"kernel": "vqb::conv_gemm_kernel (wgmma implicit-GEMM conv, fwd+dgrad launches of one step)",
                          "bound": "tensor", "achieved": prof["conv"]["tflops"], "peak": peak, "unit": "TFLOP/s",
-                         "frac": prof["conv"]["tflops"] / peak, "traffic": conv_traffic, "traffic_source": tname,
-                         "traffic_per_shape": (ttab or {}).get("per_shape"), "peak_source": peak_src,
+                         "frac": prof["conv"]["tflops"] / peak, "peak_source": peak_src,
                          "launches_per_step": prof["conv"]["launches"], "ms_per_step": prof["conv"]["ms"],
                          "alg_flops_per_launch": prof["conv"]["flops_per_launch"],
                          "avg_launch_ms": prof["conv"]["ms_per_launch"]},
@@ -575,9 +609,9 @@ def main():
                                "ms_per_step": prof["wgrad"]["ms"]},
         }
         if eager is not None:
-            line["eager_b200"] = eager
+            line["eager"] = eager
             if "value" in eager:
-                line["vs_eager_b200"] = value / eager["value"]
+                line["vs_eager"] = value / eager["value"]
         if world == 1 and not args.no_cpu_baseline:
             threads = cpu_threads()
             step, b = cpu_step_runner(batch=1, threads=threads)

@@ -1,5 +1,5 @@
 /*
- * vqb200.h — C ABI of libvqb200.so, the B200 (sm_100a) native layer under the
+ * vqb200.h — C ABI of libvqb200.so, the H100 (sm_90a) native layer under the
  * vqgan-training hot path (Encoder -> reg -> Decoder fwd/bwd + LPIPS/VGG + PatchD + losses).
  *
  * The reference (cloneofsimo/vqgan-training) has NO native layer: its boundary is the Python
@@ -13,7 +13,7 @@
  *   - activations are NHWC bf16 with C a multiple of 8 ("internal layout"); master weights,
  *     gradients and module-boundary tensors are fp32 NCHW / OIHW (the reference's layout).
  *   - every function returns 0 on success or a negative VQB_E* code; vqb_last_error() gives a
- *     message. There is no CPU fallback: on a machine without an sm_100 device the compute entry
+ *     message. There is no CPU fallback: on a machine without an sm_90 device the compute entry
  *     points fail with VQB_ENODEVICE.
  */
 #ifndef VQB200_H_
@@ -28,7 +28,7 @@ extern "C" {
 
 #define VQB_OK 0
 #define VQB_EINVAL (-1)    /* bad shape / alignment / flag combination */
-#define VQB_ENODEVICE (-2) /* no sm_100 device or driver entry point missing */
+#define VQB_ENODEVICE (-2) /* no sm_90 device or driver entry point missing */
 #define VQB_ECUDA (-3)     /* a CUDA runtime / driver call failed */
 
 #define VQB_MAX_VIEWS 16
@@ -81,7 +81,7 @@ int vqb_conv_gemm(const VqbConvDesc* d, const void* a, const void* w_packed /* b
 
 /*
  * Weight gradient  dWp[co][t][c] = sum_{n,h,w} dy[n,h,w,co] * X_view(t)[n, h+dh_t, w+dw_t, c]
- * as a split-K tcgen05 GEMM with MN-major operands. `partial` is fp32 [ksplit][Cout][ntaps*C];
+ * as a split-K wgmma GEMM with MN-major operands. `partial` is fp32 [ksplit][Cout][ntaps*C];
  * vqb_wgrad_reduce sums the splits and writes the OIHW fp32 gradient.
  * Replaces: the wgrad half of convolution_backward for every trainable conv (autograd of the
  * call sites listed at vqb_conv_gemm).
@@ -186,13 +186,6 @@ int vqb_gn_silu_bwd_pre(const void* x, const void* dy, const void* add, void* dx
                         const float* mr, const float* cs, float* dgamma, float* dbeta, float* ws, int N, int HW, int C,
                         int G, int silu, float* dx_colsum, void* stream);
 
-#ifdef VQB_DEBUG
-/* bring-up experiment only (csrc/dbg_shift.cu, libvqb200_dbg.so): one M=128,N=64,K=64 MMA whose A descriptor starts
- * shift_rows rows into a TMA-written 128B-swizzled tile with 8-row groups sbo_bytes apart */
-int vqb_dbg_shift_mma(const void* X, int R, const void* B, float* out, int shift_rows, int sbo_bytes, int base_offset,
-                      void* stream);
-#endif
-
 /*
  * Wavelet front-end of the encoder (--use_wavelet; utils.py:229-247): F.pad(x, 2) + grouped 6x6 stride-2 conv with the
  * four fixed analysis filters filt[4][6][6] (device, fp32), fused with the NCHW fp32 -> NHWC bf16 conversion:
@@ -295,9 +288,8 @@ int vqb_pack_weights_multi(const VqbPackJob* jobs_dev, int njobs, int total_bloc
 /* library / device info */
 const char* vqb_last_error(void);
 int vqb_version(void);
-int vqb_device_ok(void); /* 1 if the current device is sm_100 and the TMA driver entry point resolved */
+int vqb_device_ok(void); /* 1 if the current device is sm_90 and the TMA driver entry point resolved */
 int vqb_kernel_launch_count(void); /* number of kernels this library launched in this process */
-int vqb_set_debug_mode(int mode);   /* perf-experiment switches: only the -DVQB_DEBUG build accepts mode != 0 */
 
 #ifdef __cplusplus
 }

@@ -388,11 +388,30 @@ def flux_hr_case(name="vae_flux_hr", R=256):
     save(name, **res)
 
 
+def init_case(name="ref_init_seed123"):
+    """Initial weights of the reference VAE under torch.manual_seed(123) (tests/test_host_logic.py
+    ::test_seeded_init_matches_reference_bit_for_bit): a SHA-256 digest of every tensor's bytes, its shape (padded with
+    -1) and its first 8 values — bit-exact comparison in a few KB."""
+    import hashlib
+
+    torch.manual_seed(123)
+    sd = ref_ae.VAE(64, 3, 32, 3, [1, 2], 2, 4, False, True, False).state_dict()
+    keys = sorted(sd)
+    shapes = np.full((len(keys), 4), -1, dtype=np.int64)
+    head = np.zeros((len(keys), 8), dtype=np.float32)
+    for i, k in enumerate(keys):
+        shapes[i, :sd[k].dim()] = list(sd[k].shape)
+        v = sd[k].detach().float().reshape(-1)[:8].numpy()
+        head[i, :len(v)] = v
+    sha = [hashlib.sha256(sd[k].detach().contiguous().cpu().numpy().tobytes()).hexdigest() for k in keys]
+    save(name, keys=np.array(keys), sha256=np.array(sha), shapes=shapes, head=head)
+
+
 if __name__ == "__main__":
     only = sys.argv[1:]
     if only:  # e.g. `python oracle/make_golden.py flux_step flux_hr` (the ch=128 cases take minutes of CPU time)
         for c in only:
-            {"flux_step": flux_step_case, "flux_hr": flux_hr_case, "ckpt": ckpt_case}[c]()
+            {"flux_step": flux_step_case, "flux_hr": flux_hr_case, "ckpt": ckpt_case, "init": init_case}[c]()
         dist.destroy_process_group()
         sys.exit(0)
     vae_case("vae_small", VO.VAEConfig(resolution=32, ch=32, ch_mult=(1, 2), num_res_blocks=2, z_channels=4), 2, 32)
@@ -407,5 +426,6 @@ if __name__ == "__main__":
     flux_step_case()
     flux_hr_case()
     ckpt_case()
+    init_case()
     dist.destroy_process_group()
     print("all golden fixtures written to", OUT)

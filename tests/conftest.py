@@ -13,7 +13,7 @@ os.environ.setdefault("VQB_OFFLINE", "1")  # do not try to download torchvision 
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100) device; run with -m gpu on the B200 box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90, H100) device; select with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):

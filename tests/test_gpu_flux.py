@@ -1,8 +1,8 @@
 """GPU (-m gpu): parity at the BASELINE.json configurations (ch=128, ch_mult 1,2,4,4, z=16, 256x256 — the shapes bench.py
 times), against goldens produced by the UNMODIFIED reference on CPU fp32 (oracle/make_golden.py flux_step / flux_hr).
 
-These are the shapes where the halo-tile conv path (C % 64 == 0, Cout >= 128), the N = 256 tiles, the 256-pixel double
-accumulator, one-wave split-K at realistic K and GroupNorm with 4/8/16 channels per group are live.
+These are the shapes where the 128-column conv tiles, the fused GroupNorm statistics in the conv epilogue, split-K
+weight gradients at realistic K and GroupNorm with 4/8/16 channels per group are live.
 
 Every tolerance is tied to a PEER: the reference's own arithmetic (oracle restatement = plain PyTorch/cuDNN) executed on
 this GPU in reduced precision, measured against the same fp32 CPU golden. Two peers are run and printed:
@@ -11,8 +11,8 @@ this GPU in reduced precision, measured against the same fp32 CPU golden. Two pe
   * "bf16" — the same arithmetic with bf16 autocast around the encoder too: BASELINE.json's configs name bf16 as the
              compute dtype of this path and this implementation stores every activation in bf16 (DESIGN.md deviation 2),
              so the encoder output z and the encoder gradients are bounded by the all-bf16 peer: a TF32 encoder keeps
-             fp32 activation storage, which bf16 storage cannot match by construction (measured z rel-L2: TF32 ~1e-3,
-             bf16 eager and this implementation ~1e-2).
+             fp32 activation storage, which bf16 storage cannot match by construction (measured on an H100: z rel-L2
+             TF32 ~1e-3, bf16 eager and this implementation ~1e-2).
 For every quantity q:  err_ours(q) <= max(1.5 * err_peer(q), floor)  with `floor` stated next to each assert; where the
 peer reaches cosine >= 0.999 we must too.
 """
@@ -208,21 +208,21 @@ def test_flux_generator_step_vs_reference_golden(flux_models, gan, batch):
     assert _bound(ez, Bf["ez"], 5e-3), "z"
     assert _bound(er, M["er"], 1e-2), "recon"
     # the GAN term is a mean over 256 patch logits whose bf16 errors are spatially coherent (weight rounding acts on
-    # positive post-ReLU features): the mean inherits the per-logit error level, 1.5e-2 for this implementation AND for
-    # eager bf16 D (test_flux_discriminator_step...; measured here 1.35e-2 .. 1.5e-2 over runs), hence the 3e-2 floor with
-    # the GAN term, 5e-3 without
+    # positive post-ReLU features): the mean inherits the per-logit error level (this implementation on an H100: loss rel
+    # 1.0e-2 .. 1.7e-2 over eleven runs of this case), hence the 3e-2 floor with the GAN term, 5e-3 without
     assert _bound(ep, M["ep"], 5e-3) and _bound(el, max(M["el"], Bf["el"]), 3e-2 if gan else 5e-3), "losses"
     # with the GAN term every gradient first crosses the 13 bf16 layers of the discriminator, which the "mix" peer runs
     # in TF32: the decoder quantities are then bounded by the all-bf16 peer as well
     D = Bf if gan else M
     # (floors: this implementation's own run-to-run spread — atomics reorder the fused GroupNorm statistics and bf16
-    #  rounding amplifies that — measured mean |ratio-1| 0.005 .. 0.012 with the GAN term over repeated runs)
+    #  rounding amplifies that — on an H100 five runs with the GAN term gave mean |ratio-1| 0.008 .. 0.018)
     assert _bound(nr_dec.max(), D["nr_dec"].max(), 0.04 if gan else 0.02) and \
         _bound(nr_dec.mean(), D["nr_dec"].mean(), 0.02 if gan else 0.01), "dec norms"
     if batch == 1:
         # run-to-run spread of this implementation (fp32 atomics in the fused GroupNorm statistics reorder sums, and bf16
-        # rounding amplifies that through ~60 layers): measured mean |ratio-1| 0.002-0.011 (gan) over repeated runs, so
-        # the floors are 0.05 (max) / 0.02 (mean) with the GAN term, 0.02 / 0.01 without
+        # rounding amplifies that through ~60 layers); floors 0.05 (max) / 0.02 (mean) with the GAN term, 0.02 / 0.01
+        # without. On an H100 nine runs with the GAN term gave mean |ratio-1| 0.004 .. 0.027: the GroupNorm / LPIPS
+        # reductions that use fp32 atomics make this case exceed its floor in some runs.
         assert _bound(nr_enc.max(), Bf["nr_enc"].max(), 0.05 if gan else 0.02) and \
             _bound(nr_enc.mean(), Bf["nr_enc"].mean(), 0.02 if gan else 0.01), "enc norms"
     bad = [k for k in picks

@@ -1,4 +1,4 @@
-"""GPU (-m gpu): the CUDA hot path (through the drop-in Python surface -> ctypes -> C ABI -> sm_100a kernels) against
+"""GPU (-m gpu): the CUDA hot path (through the drop-in Python surface -> ctypes -> C ABI -> sm_90a kernels) against
 (1) the golden vectors produced by the unmodified reference and (2) the CPU oracle on the same seeded inputs.
 
 Tolerances. The reference computes the encoder in TF32, the decoder under bf16 autocast and LPIPS/D in TF32
@@ -236,7 +236,7 @@ def test_generator_and_discriminator_step_vs_reference_golden():
 
 
 def test_attention_vae_vs_reference_golden():
-    """AttnBlock (flash-style warp-MMA core + tcgen05 qkv/proj convs) inside the VAE vs the reference golden
+    """AttnBlock (flash-style warp-MMA core + wgmma qkv/proj convs) inside the VAE vs the reference golden
     (the reference cannot construct use_attn=True at HEAD; the golden was produced by swapping AttnBlock in)."""
     name = "vae_attn"
     cfg = VO.VAEConfig(resolution=32, ch=32, ch_mult=(1, 2), num_res_blocks=1, z_channels=4, use_attn=True)

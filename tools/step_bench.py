@@ -21,8 +21,6 @@ if WORLD > 1:  # torchrun: one process per GPU, NCCL
     dist.init_process_group("nccl")
     if RANK != 0:
         sys.stdout = open(os.devnull, "w")
-if os.environ.get("VQB_DEBUG_MODE"):
-    native.load().vqb_set_debug_mode(int(os.environ["VQB_DEBUG_MODE"]))  # perf experiments only
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 8
 ch = int(sys.argv[2]) if len(sys.argv) > 2 else 128
 gan = len(sys.argv) > 3 and sys.argv[3] == "gan"

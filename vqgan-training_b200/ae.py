@@ -1,9 +1,9 @@
-"""B200-native drop-in for the reference `ae.py` (cloneofsimo/vqgan-training): same classes, constructor signatures,
+"""H100-native drop-in for the reference `ae.py` (cloneofsimo/vqgan-training): same classes, constructor signatures,
 attribute names, parameter creation order (so `torch.manual_seed(s); VAE(...)` yields the reference's init) and
-state_dict keys / fp32 OIHW shapes — but every forward/backward runs hand-written sm_100a kernels (libvqb200.so):
+state_dict keys / fp32 OIHW shapes — but every forward/backward runs hand-written sm_90a kernels (libvqb200.so):
 
-  conv 3x3/1x1 s1, Downsample (pad(0,1,0,1)+s2), dgrad, wgrad  -> tcgen05 implicit-GEMM kernels (csrc/conv_gemm.cu,
-                                                                  csrc/wgrad_gemm.cu), TMA-staged, TMEM accumulators
+  conv 3x3/1x1 s1, Downsample (pad(0,1,0,1)+s2), dgrad, wgrad  -> wgmma implicit-GEMM kernels (csrc/conv_gemm.cu,
+                                                                  csrc/wgrad_gemm.cu), TMA-staged, register accumulators
   FP32GroupNorm + swish                                          -> fused stats/apply kernels (csrc/elementwise.cu)
   Upsample (nearest x2)                                          -> vector copy kernel + conv
   AttnBlock                                                      -> GN kernel + 1x1 conv kernels + flash-style core
@@ -75,7 +75,7 @@ def swish(x):
 
 
 class StandardizedC2d(nn.Conv2d):
-    """nn.Conv2d parameters/initialisation (ae.py:38: StandardizedC2d = nn.Conv2d) with a tcgen05 forward/backward."""
+    """nn.Conv2d parameters/initialisation (ae.py:38: StandardizedC2d = nn.Conv2d) with a wgmma forward/backward."""
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)

@@ -1,8 +1,8 @@
 // Multi-head self-attention core of AttnBlock (ae.py:74-93): softmax(q k^T / sqrt(64)) v per head of 64 channels,
 // flash-attention style (online softmax, no T x T matrix in HBM), warp-level tensor-core MMA
 // (mma.sync.m16n8k16 bf16 -> fp32). The 1x1 qkv / proj_out convolutions and the GroupNorm around it run on the
-// tcgen05 conv / GN kernels; this file is only the [T x T] part: T = (H/8)(W/8) = 1024 tokens at 256^2, 8 heads at
-// C = 512, 4.3 GFLOP per image and block (SURVEY.md a6) — latency/occupancy bound, not worth a TMEM pipeline.
+// wgmma conv / GN kernels; this file is only the [T x T] part: T = (H/8)(W/8) = 1024 tokens at 256^2, 8 heads at
+// C = 512, 4.3 GFLOP per image and block (SURVEY.md a6) — latency/occupancy bound, not worth a TMA/wgmma pipeline.
 //
 // Layout: qkv [N][T][3C] bf16 (channel blocks q | k | v; head h owns channels h*64..h*64+63 of each block, the
 // "b (h d) x y -> b h (x y) d" rearrange of ae.py:79-89 is pure addressing), out [N][T][C] bf16, lse [N][heads][T] fp32.

@@ -9,12 +9,6 @@ namespace vqb {
 
 static thread_local char g_err[512] = "";
 static std::atomic<int> g_launches{0};
-#ifdef VQB_DEBUG
-static std::atomic<int> g_debug{0};
-int debug_mode() { return g_debug.load(std::memory_order_relaxed); }
-#else
-int debug_mode() { return 0; }  // product build: the perf-experiment switches do not exist (see build_native.py --debug)
-#endif
 
 int set_error(int code, const char* fmt, ...) {
     va_list ap;
@@ -103,7 +97,7 @@ int num_sms() {
     return n;
 }
 
-bool device_is_sm100() {
+bool device_is_sm90() {
     int dev = 0, major = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) {
         (void)cudaGetLastError();
@@ -113,7 +107,7 @@ bool device_is_sm100() {
         (void)cudaGetLastError();
         return false;
     }
-    return major == 10;
+    return major == 9;
 }
 
 }  // namespace vqb
@@ -122,17 +116,7 @@ extern "C" {
 
 const char* vqb_last_error(void) { return vqb::g_err; }
 int vqb_version(void) { return 100; }
-int vqb_device_ok(void) { return (vqb::device_is_sm100() && vqb::get_encode_fn() != nullptr) ? 1 : 0; }
+int vqb_device_ok(void) { return (vqb::device_is_sm90() && vqb::get_encode_fn() != nullptr) ? 1 : 0; }
 int vqb_kernel_launch_count(void) { return vqb::g_launches.load(std::memory_order_relaxed); }
-int vqb_set_debug_mode(int m) {
-#ifdef VQB_DEBUG
-    vqb::g_debug.store(m);
-    return 0;
-#else
-    if (m != 0) return vqb::set_error(VQB_EINVAL, "vqb_set_debug_mode(%d): perf-experiment switches exist only in the "
-                                                  "-DVQB_DEBUG build (libvqb200_dbg.so)", m);
-    return 0;
-#endif
-}
 
 }  // extern "C"

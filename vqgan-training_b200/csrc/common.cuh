@@ -20,8 +20,7 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
                      const uint32_t* box, int swizzle_bytes);
 
 int num_sms();
-int debug_mode();  // bring-up/perf experiments only: 0 normal, 1 = no TMA loads, 2 = no MMA issue
-bool device_is_sm100();
+bool device_is_sm90();
 
 #define VQB_CHECK(cond, ...)                              \
     do {                                                  \

@@ -1,929 +1,289 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (forward and data-gradient).
+// Implicit-GEMM convolution on Hopper wgmma tensor cores (forward and data-gradient).
 //
 //   out[n,h,w,co] = epi( sum_t sum_c A_view(t)[n, h+dh_t, w+dw_t, c] * Wp[co][t*C + c] )
 //
-// GEMM view: M = output pixels (tiles of 128 = BW x BH x BN box of the NHWC tensor), N = Cout,
-// K = ntaps * C walked in 64-channel chunks. Per K-chunk the TMA producer issues ONE 4-D tiled load
-// of the activation box shifted by the tap offset (out-of-range rows/cols/channels are zero-filled by
-// the TMA unit -> conv padding costs nothing) and ONE 2-D load of the packed weights; both land in
-// 128B-swizzled K-major smem tiles that a single thread feeds to tcgen05.mma (M=128, N=BLOCK_N,
-// K=16 x4). Accumulators live in TMEM, double buffered, so the 4 epilogue warps drain tile i
-// (tcgen05.ld -> bias/residual/ReLU/mask -> bf16 NHWC or strided fp32) while tile i+1 is in the MMA
-// pipe. Persistent: one CTA per SM walks tiles round-robin.
+// GEMM view: M = output pixels (tiles of 128 = BW x BH x BN box of the NHWC tensor), N = Cout (tiles of BLOCK_N),
+// K = ntaps * C walked in 64-channel chunks. Per K-chunk the TMA producer issues ONE 4-D tiled load of the activation
+// box shifted by the tap offset (out-of-range rows/cols/channels are zero-filled by the TMA unit -> conv padding costs
+// nothing) and ONE 2-D load of the packed weights; both land in 128B-swizzled K-major smem tiles of a multi-stage
+// mbarrier ring. Two consumer warpgroups each own 64 rows of the tile and issue wgmma (M = 64, N = BLOCK_N, K = 16 x4)
+// with fp32 accumulators in registers; their epilogue (bias / residual / ReLU / mask / GroupNorm statistics -> bf16
+// NHWC or strided fp32) runs while the producer already streams the next tile's operands. Persistent: one CTA per SM
+// walks tiles round-robin.
 //
 // Replaces the cuDNN kernels behind nn.Conv2d at reference ae.py:105-117,143-154,160-167 and the
 // torchvision VGG convs reached from utils.py:95-111,150-154 (see include/vqb200.h).
 #include "common.cuh"
 #include "ptx.cuh"
 
-#include <cstdlib>
-
 namespace vqb {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB per stage
-constexpr int kThreads = 256;                   // warp0 TMA, warp1 MMA, warp2 TMEM alloc, warp3 idle, warps4-7 epilogue
-constexpr int kMaxStages = 12;
+constexpr int kThreads = 384;                   // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue
+constexpr int kMaxStages = 8;
+constexpr int kConsumerWarps = 8;
 
 struct alignas(64) ConvParams {
     CUtensorMap amap[VQB_MAX_VIEWS];
     CUtensorMap bmap;
-    CUtensorMap omap;  // output tensor (TMA-store epilogue)
-    CUtensorMap xmap;  // residual (or ReLU-gate mask) tensor, same geometry as omap (TMA-prefetched epilogue operand)
     int32_t tap_view[VQB_MAX_TAPS];
     int32_t tap_dw[VQB_MAX_TAPS];
     int32_t tap_dh[VQB_MAX_TAPS];
     int32_t ntaps, kchunks, C, Cout;
     int32_t N, H, W;
     int32_t lbw, lbh, lbn;
-    int32_t tiles_w, tiles_h, tiles_nb;
+    int32_t tiles_w, tiles_h;
     int32_t n_tiles, total_tiles;
-    int32_t block_n, stages, tmem_cols;
-    int32_t mtiles, nbuf;
-    int32_t tma_store, mt_dh, mt_dn, do_stats;  // TMA-store epilogue enabled; box offset of the second sub-tile  // 128-row accumulator sub-tiles per CTA tile (1|2); TMEM accumulator buffers (2..4)
+    int32_t stages, do_stats;
     int32_t flags, out_f32;
-    int32_t dbg, aux_tma;  // aux_tma: 1 = residual, 2 = mask arrives through xmap
-    // halo mode: ONE activation box with a halo serves every tap of a 64-channel chunk (tap shift = descriptor offset)
-    int32_t halo, h_bytes, h_stages, h_sbo;  // enabled; bytes per halo stage (1024-aligned); stages; 8-row group stride
-    int32_t h_w0, h_h0, mt_dw, h_tx;         // most negative tap offsets (box origin); w offset of the second sub-tile; box bytes
-    uint32_t tap_off16[VQB_MAX_TAPS];        // descriptor start offset of tap t inside the halo tile, in 16-byte units
-    // swap mode (halo mode, Cout <= 128): the weights are the M = 128 operand and 256 pixels (8 x 32) the N operand, so
-    // each MMA is M128 x N256 (96 B/clk of shared-memory operand reads instead of the 128 B/clk of an N = 128 MMA);
-    // the accumulator is [channel lane][pixel column] and the epilogue transposes through the staging tiles.
-    int32_t swap, epi_bytes;
-    // pair mode (halo mode, Cout == 128): two CTAs of a cluster form a cta_group::2 pair. Each owns one 8 x 16 sub-tile
-    // (its own halo tile and TMEM accumulator) and HALF of every weight tile; the leader issues M = 256 MMAs. Per SM an
-    // MMA then reads 4 KB of activations + 2 KB of weights per 64 cycles (96 B/clk) instead of the 128 B/clk of two
-    // independent N = 128 streams, which is the measured limiter of the 128-channel layers.
-    int32_t pair, tps;  // tps: taps (weight tiles) per ring stage in halo mode (1, or 3 in pair mode)
     int64_t on, oh, ow, oc;
     void* out;
     const void* res;
     const void* mask;
     const float* bias;
     float* stats;
-    // fused GroupNorm(+SiLU)-backward statistics (VQB_EPI_GNBWD, aux_tma == 3): this launch is the data gradient of the
-    // conv that consumed y = silu(GN(x)); its output IS dy of that GroupNorm, so the epilogue also reads the x tile
-    // (through xmap) and accumulates cs[n][c] = (sum_p du, sum_p du * xhat), du = dy * silu'(gamma*xhat + beta) — the
+    // fused GroupNorm(+SiLU)-backward statistics (vqb_conv_gemm_gnbwd): this launch is the data gradient of the conv
+    // that consumed y = silu(GN(x)); its output IS dy of that GroupNorm, so the epilogue also reads x (same layout as
+    // the output) and accumulates cs[n][c] = (sum_p du, sum_p du * xhat), du = dy * silu'(gamma*xhat + beta) — the
     // whole "reduce" pass of the GroupNorm backward (x and dy read once more from HBM) disappears.
+    const __nv_bfloat16* gn_x;
     const float* gn_mr;     // [N][G][2] mean, rstd
     const float* gn_gamma;  // [C]
     const float* gn_beta;   // [C]
     float* gn_cs;           // [N][C][2], pre-zeroed
     int32_t gn_G, gn_lcpg;  // groups, log2(channels per group)
-    int32_t lean, issue2;   // lean production issue loop / second issue thread (VQB_LEAN_ISSUE, VQB_ISSUE2 for A/B runs)
 };
 
-// One step of the transposing butterfly used by the fused GroupNorm-backward statistics: lanes whose bit OFF is set
-// keep the upper HALF of the (still 2*HALF) per-lane values, the others the lower, and each adds its partner's copy.
-template <int HALF, int OFF>
-__device__ __forceinline__ void bfly_step(float (&s1)[16], float (&s2)[16], uint32_t lane) {
-    const bool upper = (lane & OFF) != 0;
-#pragma unroll
-    for (int i = 0; i < HALF; ++i) {
-        const float k1 = upper ? s1[i + HALF] : s1[i], t1 = upper ? s1[i] : s1[i + HALF];
-        const float k2 = upper ? s2[i + HALF] : s2[i], t2 = upper ? s2[i] : s2[i + HALF];
-        s1[i] = k1 + __shfl_xor_sync(0xffffffffu, t1, OFF);
-        s2[i] = k2 + __shfl_xor_sync(0xffffffffu, t2, OFF);
-    }
-}
-
-template <bool PAIR>
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t lane = threadIdx.x & 31;
-    // PAIR is a template parameter: cta_group::2 / cluster instructions make a kernel require a cluster launch, so
-    // they may only exist in the instantiation that is launched with cluster dimension 2
-    constexpr bool pair = PAIR;
-    uint32_t crank = 0u;  // 0 = leader of the CTA pair
-    if constexpr (PAIR) crank = cluster_ctarank();
-    const int tile0 = pair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-    const int tstep = pair ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-    const int wsh = pair ? static_cast<int>(crank) * 8 : 0;  // this CTA's sub-tile inside the pair's 16-wide tile
-
+    constexpr uint32_t kBBytes = BN * kBlockK * 2;
+    constexpr uint32_t kStageBytes = kABytes + kBBytes;  // a multiple of 2 KB: every tile stays 1024-B aligned
     // carve shared memory (1024-B aligned for the 128B swizzle atoms)
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t stages = p.stages;
-    const uint32_t a_bytes = static_cast<uint32_t>(p.mtiles) * kABytes;
-    const uint32_t b_bytes = static_cast<uint32_t>(p.swap ? 128 : (p.pair ? p.block_n / 2 : p.block_n)) * kBlockK * 2;
-    const uint32_t mtiles = p.mtiles, nbuf = p.nbuf;
-    uint8_t* sA = base;  // halo mode: h_stages halo tiles; else `stages` 128-row tap tiles
-    uint8_t* sB = base + (p.halo ? static_cast<uint32_t>(p.h_stages * p.h_bytes) : stages * a_bytes);
-    uint8_t* sOut = sB + stages * b_bytes * static_cast<uint32_t>(p.tps);  // 2 x 16 KB output staging tiles (128 rows x 128 B, 128B-swizzled)
-    float* sStat = reinterpret_cast<float*>(sOut + 2 * 16384);  // [4 warps][64 ch][2] (GroupNorm statistics combine)
-    uint8_t* sAux = sOut + 2 * 16384 + 2048;  // 2 x 16 KB residual / mask tiles (same swizzled layout as sOut)
-    // Two issue threads (warp 1 and the otherwise idle warp 3) for the production halo path with two accumulators per
-    // tile (Cout = 128 layers): each owns one accumulator's four MMAs per tap, so neither single-thread instruction stream
-    // has to keep up with both halves of the tensor work. Every ring / halo stage is then released by TWO tcgen05.commit.
-    const bool issue2 = !PAIR && p.issue2 && p.lean && p.halo && !p.swap && p.mtiles == 2 && (p.dbg & 3) != 2;
-    uint64_t* full = reinterpret_cast<uint64_t*>(sOut + p.epi_bytes);
+    float* sStat = reinterpret_cast<float*>(base + stages * kStageBytes);  // [8 consumer warps][BN][2]
+    uint64_t* full = reinterpret_cast<uint64_t*>(sStat + kConsumerWarps * BN * 2);
     uint64_t* empty = full + stages;
-    uint64_t* tfull = empty + stages;
-    uint64_t* tempty = tfull + 4;
-    uint64_t* afull = tempty + 4;
-    uint64_t* hfull = afull + 2;   // halo ring (<= 4 stages)
-    uint64_t* hempty = hfull + 4;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(hempty + 4);
+    const uint32_t wg = threadIdx.x >> 7;
+    const uint32_t warp = (threadIdx.x >> 5) & 3u;  // warp inside its warpgroup
+    const uint32_t lane = threadIdx.x & 31u;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int v = 0; v < VQB_MAX_VIEWS; ++v) {
             bool used = false;
             for (int t = 0; t < p.ntaps; ++t) used |= (p.tap_view[t] == v);
             if (used) tma_prefetch_desc(&p.amap[v]);
         }
         tma_prefetch_desc(&p.bmap);
-        if (p.tma_store) tma_prefetch_desc(&p.omap);
-        if (p.aux_tma) tma_prefetch_desc(&p.xmap);
-    }
-    if (warp == 1 && lane == 0) {
         for (uint32_t i = 0; i < stages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], issue2 ? 2 : 1);
-        }
-        for (int i = 0; i < 4; ++i) {
-            mbar_init(&tfull[i], 1);
-            mbar_init(&tempty[i], pair ? 256 : 128);  // pair: the leader's barrier collects both CTAs' epilogues
-        }
-        mbar_init(&afull[0], 1);
-        mbar_init(&afull[1], 1);
-        for (int i = 0; i < 4; ++i) {
-            mbar_init(&hfull[i], 1);
-            mbar_init(&hempty[i], issue2 ? 2 : 1);
+            mbar_init(&empty[i], kConsumerWarps);  // lane 0 of every consumer warp releases the stage
         }
         fence_mbar_init();
     }
-    if (warp == 2) {
-        if constexpr (PAIR) {
-            tmem_alloc_pair(tmem_slot, p.tmem_cols);
-            tmem_relinquish_pair();
-        } else {
-            tmem_alloc(tmem_slot, p.tmem_cols);
-            tmem_relinquish();
-        }
-    }
-    tc_fence_before();
-    if constexpr (PAIR)
-        cluster_sync_all();  // the peer's barriers must be initialised before anything is signalled on them
-    else
-        __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
 
     const int num_kb = p.ntaps * p.kchunks;
-
-    // The single-thread roles are entered through elect.sync (not `lane == 0`): ptxas then knows the region runs in
-    // exactly one lane with warp-uniform operands and emits the TMA / tcgen05 instructions back to back from uniform
-    // registers. With `lane == 0` every UTCHMMA was wrapped in an ELECT / PLOP3 / BRA.U.ANY loop plus R2UR moves — ~190
-    // SASS instructions per tap in the issue thread, 1058 cycles per tap against the 512 the tensor core needs
-    // (ncu source-level sampling, profiles/r02_ncu_conv128_issue_bound.txt): the issue thread, not shared memory, was
-    // what held the 128-channel layers at ~50 % tensor-pipe utilisation.
-    if (warp == 0) {
-      if (elect_one()) {
-      if (p.halo) {
-        // ===================== TMA producer, halo mode: per 64-channel chunk ONE activation box (tile + halo) and one
-        // weight tile per tap. The activation bytes per FLOP drop by ~ntaps/1.3; the weight tiles stream through
-        // their own ring.
-        uint32_t stage = 0, phase = 0, hs = 0, hph = 0;
-        uint8_t* b_dst = sB;
-        uint8_t* h_dst = sA;
-        const uint32_t h_tx = static_cast<uint32_t>(p.h_tx);
-        for (int tile = tile0; tile < p.total_tiles; tile += tstep) {
-            const int n_tile = tile % p.n_tiles;
-            const int m_tile = tile / p.n_tiles;
-            const int tw = m_tile % p.tiles_w;
-            const int th = (m_tile / p.tiles_w) % p.tiles_h;
-            const int tn = m_tile / (p.tiles_w * p.tiles_h);
-            const int w0 = (tw << p.lbw) + p.h_w0 + wsh, h0 = (th << p.lbh) + p.h_h0;
-            const int ncol0 = n_tile * p.block_n + (pair ? static_cast<int>(crank) * 64 : 0);
-            for (int kc = 0; kc < p.kchunks; ++kc) {
-                mbar_wait(&hempty[hs], hph ^ 1);
-                if constexpr (PAIR) {
-                    // both CTAs' boxes complete on the LEADER's barrier (which expects the bytes of both)
-                    if (crank == 0) mbar_arrive_expect_tx(&hfull[hs], 2 * h_tx);
-                    tma_load_4d_pair(&p.amap[0], mapa_u32(smem_u32(&hfull[hs]), 0), h_dst, kc * kBlockK, w0, h0, tn);
-                } else if ((p.dbg & 3) == 1) {
-                    mbar_arrive(&hfull[hs]);
-                } else {
-                    mbar_arrive_expect_tx(&hfull[hs], h_tx);
-                    tma_load_4d(&p.amap[0], &hfull[hs], h_dst, kc * kBlockK, w0, h0, tn);
-                }
-                if (++hs == static_cast<uint32_t>(p.h_stages)) {
-                    hs = 0;
-                    hph ^= 1;
-                    h_dst = sA;
-                } else {
-                    h_dst += p.h_bytes;
-                }
-                int kcol = kc * kBlockK;
-                const int tps = p.tps;
-                for (int t = 0; t < p.ntaps; t += tps, kcol += tps * p.C) {
-                    mbar_wait(&empty[stage], phase ^ 1);
-                    if constexpr (PAIR) {
-                        // one ring stage = tps weight tiles (both CTAs' halves complete on the leader's barrier)
-                        if (crank == 0) mbar_arrive_expect_tx(&full[stage], 2 * b_bytes * tps);
-                        const uint32_t fa = mapa_u32(smem_u32(&full[stage]), 0);
-                        for (int j = 0; j < tps; ++j)
-                            tma_load_2d_pair(&p.bmap, fa, b_dst + j * b_bytes, kcol + j * p.C, ncol0);
-                    } else if ((p.dbg & 3) == 1) {
-                        mbar_arrive(&full[stage]);
-                    } else {
-                        mbar_arrive_expect_tx(&full[stage], b_bytes);
-                        tma_load_2d(&p.bmap, &full[stage], b_dst, kcol, ncol0);
-                    }
-                    if (++stage == stages) {
-                        stage = 0;
-                        phase ^= 1;
-                        b_dst = sB;
-                    } else {
-                        b_dst += b_bytes * tps;
-                    }
-                }
-            }
-        }
-      } else {
-        // ===================== TMA producer (one thread; keep the per-K-block instruction count small) =========
-        uint32_t stage = 0, phase = 0, tile_iter = 0;
-        uint8_t* a_dst = sA;
-        uint8_t* b_dst = sB;
-        const uint32_t tx_bytes = a_bytes + b_bytes;
-        for (int tile = tile0; tile < p.total_tiles; tile += tstep, ++tile_iter) {
-            const int n_tile = tile % p.n_tiles;
-            const int m_tile = tile / p.n_tiles;
-            const int tw = m_tile % p.tiles_w;
-            const int th = (m_tile / p.tiles_w) % p.tiles_h;
-            const int tn = m_tile / (p.tiles_w * p.tiles_h);
-            const int w0 = tw << p.lbw, h0 = th << p.lbh, n0 = tn << p.lbn;
-            const int ncol0 = n_tile * p.block_n;
-            // K-blocks are walked from a per-CTA rotated start (neutral in measurements; keeps lock-stepped CTAs from
-            // requesting identical weight rows at the same instant)
-            const int rot = (p.dbg & 4) ? 0 : static_cast<int>((blockIdx.x * 5u + tile_iter * 3u) % static_cast<uint32_t>(num_kb));
-            int t = rot / p.kchunks;
-            int kc = rot - t * p.kchunks;
-            for (int kbi = 0; kbi < num_kb; ++kbi) {
-                mbar_wait(&empty[stage], phase ^ 1);
-                if ((p.dbg & 3) == 1) {
-                    mbar_arrive(&full[stage]);
-                } else {
-                    mbar_arrive_expect_tx(&full[stage], tx_bytes);
-                    tma_load_4d(&p.amap[p.tap_view[t]], &full[stage], a_dst, kc * kBlockK, w0 + p.tap_dw[t],
-                                h0 + p.tap_dh[t], n0);
-                    tma_load_2d(&p.bmap, &full[stage], b_dst, t * p.C + kc * kBlockK, ncol0);
-                }
-                if (++kc == p.kchunks) {
-                    kc = 0;
-                    if (++t == p.ntaps) t = 0;
-                }
-                if (++stage == stages) {
-                    stage = 0;
-                    phase ^= 1;
-                    a_dst = sA;
-                    b_dst = sB;
-                } else {
-                    a_dst += a_bytes;
-                    b_dst += b_bytes;
-                }
-            }
-        }
-      }
-      }
-    } else if (warp == 1 || (warp == 3 && issue2)) {
-      const uint32_t role = (warp == 3) ? 1u : 0u;  // 0: accumulator 0 (and 1 unless issue2); 1: accumulator 1 only
-      if (crank == 0 && elect_one()) {
-        // ===================== MMA issuer (single thread; in pair mode only the leader CTA's) =====================
-        // This thread must issue 4*mtiles MMAs per K-block in well under the ~512*mtiles cycles the tensor core needs
-        // for them: descriptors are base + increments (no divisions, no per-K-block descriptor builds).
-        const uint32_t idesc = make_idesc_bf16(pair ? 2 * kBlockM : kBlockM, p.block_n, 0, 0);
-        const uint64_t da_base = make_smem_desc(smem_u32(sA), 0, 1024, 2);
-        const uint64_t db_base = make_smem_desc(smem_u32(sB), 0, 1024, 2);
-        const uint32_t a_step = a_bytes >> 4, b_step = b_bytes >> 4;  // descriptor address field is (addr >> 4)
-        const bool two = (mtiles == 2);
-        const bool do_mma = (p.dbg & 3) != 2;
-        uint32_t stage = 0, phase = 0, a_off = 0, b_off = 0, hstage = 0, hphase = 0;
-        uint32_t buf = 0, bpar = 0;  // next TMEM accumulator buffer and the parity of its use count
-        for (int tile = tile0; tile < p.total_tiles; tile += tstep) {
-            const uint32_t b0 = buf;
-            if (role == 0) mbar_wait(&tempty[buf], bpar ^ 1);  // epilogue has drained the previous use of this buffer
-            if (++buf == nbuf) {
-                buf = 0;
-                bpar ^= 1;
-            }
-            uint32_t b1 = b0;
-            const bool mine1 = two && (role == 1 || !issue2);  // does this thread issue accumulator 1's MMAs?
-            if (two) {
-                b1 = buf;
-                if (mine1) mbar_wait(&tempty[buf], bpar ^ 1);
-                if (++buf == nbuf) {
-                    buf = 0;
-                    bpar ^= 1;
-                }
-            }
-            tc_fence_after();
-            const uint32_t d0 = tmem_base + b0 * p.block_n, d1 = tmem_base + b1 * p.block_n;
-            uint32_t acc = 0;
-            if (!PAIR && p.lean && p.halo && !p.swap && do_mma) {
-                // ---- production halo path, written for the shortest possible instruction stream in this one thread
-                // (ncu: the issue thread is ~78 % busy even after the elect.sync fix): loop constants in locals, 32-bit
-                // arithmetic on the descriptors' low words, next tap's descriptor offset fetched while this tap's MMAs
-                // are being issued.
-                const uint64_t dh64 = make_smem_desc(smem_u32(sA), 0, static_cast<uint32_t>(p.h_sbo), 2);
-                const uint32_t dh_lo = static_cast<uint32_t>(dh64), dh_hi = static_cast<uint32_t>(dh64 >> 32);
-                const uint32_t db_lo0 = static_cast<uint32_t>(db_base), db_hi = static_cast<uint32_t>(db_base >> 32);
-                const uint32_t h_step = static_cast<uint32_t>(p.h_bytes) >> 4;
-                const uint32_t mt_off = static_cast<uint32_t>(p.mt_dw) * 8u;
-                const int ntaps = p.ntaps, kchunks = p.kchunks;
-                const uint32_t nhst = static_cast<uint32_t>(p.h_stages);
-                uint32_t off = p.tap_off16[0];
-                for (int kc = 0; kc < kchunks; ++kc) {
-                    mbar_wait(&hfull[hstage], hphase);
-                    const uint32_t dah_lo = dh_lo + hstage * h_step;
-                    for (int t = 0; t < ntaps; ++t) {
-                        mbar_wait(&full[stage], phase);
-                        tc_fence_after();
-                        const uint32_t a_lo = dah_lo + off, b_lo = db_lo0 + b_off;
-                        if (role == 0) {
-#pragma unroll
-                            for (int k = 0; k < kBlockK / 16; ++k)
-                                umma_bf16_lohi(d0, a_lo + 2 * k, dh_hi, b_lo + 2 * k, db_hi, idesc, acc | k);
-                        }
-                        if (mine1) {
-#pragma unroll
-                            for (int k = 0; k < kBlockK / 16; ++k)
-                                umma_bf16_lohi(d1, a_lo + mt_off + 2 * k, dh_hi, b_lo + 2 * k, db_hi, idesc, acc | k);
-                        }
-                        off = p.tap_off16[t + 1 < ntaps ? t + 1 : 0];  // in flight while the MMAs above are queued
-                        umma_commit(&empty[stage]);
-                        acc = 1;
+    if (wg == 0) {
+        // ===================== TMA producer (one elected thread) =====================
+        if (warp == 0 && elect_one()) {
+            uint32_t stage = 0, phase = 0;
+            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+                const int n_tile = tile % p.n_tiles;
+                const int m_tile = tile / p.n_tiles;
+                const int tw = m_tile % p.tiles_w;
+                const int th = (m_tile / p.tiles_w) % p.tiles_h;
+                const int tn = m_tile / (p.tiles_w * p.tiles_h);
+                const int w0 = tw << p.lbw, h0 = th << p.lbh, n0 = tn << p.lbn;
+                const int ncol0 = n_tile * BN;
+                for (int t = 0; t < p.ntaps; ++t) {
+                    for (int kc = 0; kc < p.kchunks; ++kc) {
+                        mbar_wait(&empty[stage], phase ^ 1);
+                        uint8_t* a_dst = base + stage * kStageBytes;
+                        mbar_arrive_expect_tx(&full[stage], kStageBytes);
+                        tma_load_4d(&p.amap[p.tap_view[t]], &full[stage], a_dst, kc * kBlockK, w0 + p.tap_dw[t],
+                                    h0 + p.tap_dh[t], n0);
+                        tma_load_2d(&p.bmap, &full[stage], a_dst + kABytes, t * p.C + kc * kBlockK, ncol0);
                         if (++stage == stages) {
                             stage = 0;
                             phase ^= 1;
-                            b_off = 0;
-                        } else {
-                            b_off += b_step;
                         }
                     }
-                    umma_commit(&hempty[hstage]);  // every tap of this chunk has been issued: the halo tile may be refilled
-                    if (++hstage == nhst) {
-                        hstage = 0;
-                        hphase ^= 1;
-                    }
                 }
-            } else if (p.halo) {
-                // halo mode: the A descriptor of tap t is the halo tile's descriptor plus a row offset (the 128B swizzle is
-                // a function of absolute smem address bits, so row-shifted starts and an 8-row group stride of one
-                // halo-tile line read exactly the rows the TMA unit wrote: tools/gpu_probe.py shift)
-                const uint64_t dh_base = make_smem_desc(smem_u32(sA), 0, static_cast<uint32_t>(p.h_sbo), 2);
-                const uint32_t h_step = static_cast<uint32_t>(p.h_bytes) >> 4;
-                const uint32_t mt_off = static_cast<uint32_t>(p.mt_dw) * 8u;  // mt_dw rows of 128 B, in 16-byte units
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    mbar_wait(&hfull[hstage], hphase);
-                    const uint64_t dah = dh_base + hstage * h_step;
-                    const int tps = p.tps;
-                    for (int t = 0; t < p.ntaps; t += tps) {
-                        mbar_wait(&full[stage], phase);
-                        tc_fence_after();
-                        const uint64_t da = dah + p.tap_off16[t], db = db_base + b_off;
-                        if constexpr (PAIR) {
-                            for (int j = 0; j < tps; ++j) {
-                                const uint64_t daj = dah + p.tap_off16[t + j], dbj = db + j * b_step;
-#pragma unroll
-                                for (int k = 0; k < kBlockK / 16; ++k)
-                                    umma_bf16_pair(d0, daj + 2 * k, dbj + 2 * k, idesc, (acc | j) | k);
-                            }
-                            umma_commit_pair(&empty[stage], 3);
-                        } else if (do_mma && p.swap) {
-#pragma unroll
-                            for (int k = 0; k < kBlockK / 16; ++k) umma_bf16(d0, db + 2 * k, da + 2 * k, idesc, acc | k);
-                        } else if (do_mma) {
-#pragma unroll
-                            for (int k = 0; k < kBlockK / 16; ++k) umma_bf16(d0, da + 2 * k, db + 2 * k, idesc, acc | k);
-                            if (two) {
-#pragma unroll
-                                for (int k = 0; k < kBlockK / 16; ++k)
-                                    umma_bf16(d1, da + mt_off + 2 * k, db + 2 * k, idesc, acc | k);
-                            }
-                        }
-                        if (!pair) umma_commit(&empty[stage]);
-                        acc = 1;
-                        if (++stage == stages) {
-                            stage = 0;
-                            phase ^= 1;
-                            b_off = 0;
-                        } else {
-                            b_off += b_step * tps;
-                        }
-                    }
-                    // every tap of this chunk has been issued: the halo tile may be refilled
-                    if constexpr (PAIR)
-                        umma_commit_pair(&hempty[hstage], 3);
-                    else
-                        umma_commit(&hempty[hstage]);
-                    if (++hstage == static_cast<uint32_t>(p.h_stages)) {
-                        hstage = 0;
-                        hphase ^= 1;
-                    }
-                }
-            } else
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint64_t da = da_base + a_off, db = db_base + b_off;
-                if (do_mma) {
-#pragma unroll
-                    for (int k = 0; k < kBlockK / 16; ++k) umma_bf16(d0, da + 2 * k, db + 2 * k, idesc, acc | k);
-                    if (two) {
-#pragma unroll
-                        for (int k = 0; k < kBlockK / 16; ++k)
-                            umma_bf16(d1, da + (kABytes >> 4) + 2 * k, db + 2 * k, idesc, acc | k);
-                    }
-                }
-                umma_commit(&empty[stage]);  // frees the smem slot once these MMAs retire
-                acc = 1;
-                if (++stage == stages) {
-                    stage = 0;
-                    phase ^= 1;
-                    a_off = 0;
-                    b_off = 0;
-                } else {
-                    a_off += a_step;
-                    b_off += b_step;
-                }
-            }
-            if constexpr (PAIR) {
-                umma_commit_pair(&tfull[b0], 3);  // both CTAs' epilogues drain their half of the M = 256 accumulator
-            } else {
-                if (role == 0) umma_commit(&tfull[b0]);  // accumulator(s) complete -> epilogue
-                if (mine1) umma_commit(&tfull[b1]);
             }
         }
-      }
-    } else if (warp >= 4) {
-        // ===================== epilogue (4 warps = 128 accumulator rows) =====================
-        const uint32_t ew = warp - 4;  // == warp % 4: the TMEM lane quarter this warp may read
-        const bool has_bias = p.flags & VQB_EPI_BIAS, has_res = p.flags & VQB_EPI_RES;
-        const bool do_relu = p.flags & VQB_EPI_RELU, has_mask = p.flags & VQB_EPI_MASK;
-        const bool vec_path = (p.oc == 1) && (p.out_f32 == 0);
-        const bool no_store = (p.dbg & 128) != 0;  // experiment: drain TMEM but skip the global stores
-        if (p.swap) {
-            // -------- transposed epilogue: accumulator lane = output channel, column = pixel of the 8 x 32 tile.
-            // Four 16 KB staging tiles = 2 sets x (channels 0-63, 64-127) of one 8 x 16 sub-tile; a set is filled by TMA
-            // with the residual / mask tile one step ahead (when there is one), updated IN PLACE, then TMA-stored.
-            const uint32_t co = ew * 32 + lane;
-            const uint32_t half = ew >> 1;
-            const uint32_t cchunk = (co & 63u) >> 3, cin = (co & 7u) * 2u;
-            const bool co_ok = static_cast<int>(co) < p.Cout;
-            const float bias_v = (has_bias && co_ok) ? __ldg(p.bias + co) : 0.f;
-            const bool aux_tma = p.aux_tma != 0;
-            const bool elected = (ew == 0 && lane == 0);
-            uint32_t ebuf = 0, epar = 0, step = 0;
-            int ptile = tile0;
-            uint32_t ps = 0, pstep = 0;
-            auto aux_issue_next = [&]() {
-                if (ptile >= p.total_tiles) return;
-                const int tw = ptile % p.tiles_w;
-                const int th = (ptile / p.tiles_w) % p.tiles_h;
-                const int tn = ptile / (p.tiles_w * p.tiles_h);
-                uint8_t* dst = sOut + (pstep & 1u) * 32768u;
-                mbar_arrive_expect_tx(&afull[pstep & 1u], 32768u);
-                tma_load_4d(&p.xmap, &afull[pstep & 1u], dst, 0, tw << 3, (th << 5) + static_cast<int>(ps) * 16, tn);
-                tma_load_4d(&p.xmap, &afull[pstep & 1u], dst + 16384, 64, tw << 3, (th << 5) + static_cast<int>(ps) * 16, tn);
-                ++pstep;
-                ps ^= 1u;
-                if (ps == 0) ptile += tstep;
-            };
-            if (aux_tma && elected) aux_issue_next();  // step 0
-            for (int tile = tile0; tile < p.total_tiles; tile += tstep) {
-                const int tw = tile % p.tiles_w;
-                const int th = (tile / p.tiles_w) % p.tiles_h;
-                const int tn = tile / (p.tiles_w * p.tiles_h);
-                const uint32_t as = ebuf, aph = epar;
-                if (++ebuf == nbuf) {
-                    ebuf = 0;
-                    epar ^= 1;
-                }
-                mbar_wait(&tfull[as], aph);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((ew * 32u) << 16) + as * p.block_n;
-                float ssum = 0.f, ssq = 0.f;
-                for (uint32_t sub = 0; sub < 2; ++sub, ++step) {
-                    uint8_t* set = sOut + (step & 1u) * 32768u + half * 16384u;
-                    if (elected) {
-                        if (aux_tma) {
-                            bulk_wait_read<0>();  // the other set's store has drained: refill it for the next step
-                            aux_issue_next();
-                        } else {
-                            bulk_wait_read<1>();  // this set's previous store (two steps ago) has drained
-                        }
-                    }
-                    named_bar_sync(1, 128);
-                    if (aux_tma) mbar_wait(&afull[step & 1u], (step >> 1) & 1u);
-#pragma unroll 1
-                    for (uint32_t chunk = 0; chunk < 4; ++chunk) {
-                        uint32_t v[32];
-                        tmem_ld32(taddr + sub * 128u + chunk * 32u, v);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (uint32_t i = 0; i < 32; ++i) {
-                            __nv_bfloat16* cell = reinterpret_cast<__nv_bfloat16*>(
-                                set + (chunk * 32u + i) * 128u + (((cchunk ^ (i & 7u)) << 4) | cin));
-                            float f = __uint_as_float(v[i]) + bias_v;
-                            if (p.aux_tma == 1) f += __bfloat162float(*cell);
-                            if (do_relu) f = fmaxf(f, 0.f);
-                            if (p.aux_tma == 2 && !(__bfloat162float(*cell) > 0.f)) f = 0.f;
-                            const __nv_bfloat16 b = __float2bfloat16(f);
-                            if (p.do_stats) {
-                                const float fb = __bfloat162float(b);
-                                ssum += fb;
-                                ssq = fmaf(fb, fb, ssq);
-                            }
-                            *cell = b;
-                        }
-                    }
-                    fence_proxy_async_smem();
-                    named_bar_sync(1, 128);
-                    if (elected && !no_store) {
-                        uint8_t* s0 = sOut + (step & 1u) * 32768u;
-                        const int oh0 = (th << 5) + static_cast<int>(sub) * 16;
-                        tma_store_4d(&p.omap, s0, 0, tw << 3, oh0, tn);
-                        if (p.Cout > 64) tma_store_4d(&p.omap, s0 + 16384, 64, tw << 3, oh0, tn);
-                        bulk_commit();
-                    }
-                }
-                if (p.do_stats && co_ok) {
-                    atomicAdd(p.stats + (static_cast<int64_t>(tn) * p.Cout + co) * 2, ssum);
-                    atomicAdd(p.stats + (static_cast<int64_t>(tn) * p.Cout + co) * 2 + 1, ssq);
-                }
-                tc_fence_before();
-                mbar_arrive(&tempty[as]);
-            }
-            if (elected) bulk_wait_all();
-        } else {
-        uint32_t ebuf = 0, epar = 0, obuf = 0;
-        // Residual / mask tiles are fetched by TMA one 64-channel group AHEAD of the group being drained (per-thread
-        // loads of this operand were latency bound: a residual epilogue ran at 0.6x the speed of a plain one). The
-        // elected thread walks the same (tile, sub-tile, channel group) sequence one step ahead.
-        const bool aux_tma = p.aux_tma != 0;
-        const bool elected = (ew == 0 && lane == 0);
-        int ptile = tile0;
-        uint32_t pmt = 0, pq = 0;
-        int pcg = 0;
-        auto aux_issue_next = [&]() {
-            if (ptile >= p.total_tiles) return;
-            const int n_tile = ptile % p.n_tiles;
-            const int m_tile = ptile / p.n_tiles;
-            const int tw = m_tile % p.tiles_w;
-            const int th = (m_tile / p.tiles_w) % p.tiles_h;
-            const int tn = m_tile / (p.tiles_w * p.tiles_h);
-            const int col = n_tile * p.block_n + pcg * 64;
-            mbar_arrive_expect_tx(&afull[pq & 1u], 16384u);
-            tma_load_4d(&p.xmap, &afull[pq & 1u], sAux + (pq & 1u) * 16384u, col, (tw << p.lbw) + (pmt ? p.mt_dw : 0) + wsh,
-                        (th << p.lbh) + (pmt ? p.mt_dh : 0), (tn << p.lbn) + (pmt ? p.mt_dn : 0));
-            ++pq;
-            ++pcg;
-            if (pcg * 64 >= p.block_n || n_tile * p.block_n + pcg * 64 >= p.Cout) {
-                pcg = 0;
-                if (++pmt == mtiles) {
-                    pmt = 0;
-                    ptile += tstep;
-                }
-            }
-        };
-        if (aux_tma && elected) aux_issue_next();  // group 0
-        for (int tile = tile0; tile < p.total_tiles; tile += tstep) {
-          const int n_tile = tile % p.n_tiles;
-          const int m_tile = tile / p.n_tiles;
-          const int tw = m_tile % p.tiles_w;
-          const int th = (m_tile / p.tiles_w) % p.tiles_h;
-          const int tn = m_tile / (p.tiles_w * p.tiles_h);
-          const int col0 = n_tile * p.block_n;
-          for (uint32_t mt = 0; mt < mtiles; ++mt) {
-            const uint32_t as = ebuf, aph = epar;
-            if (++ebuf == nbuf) {
-                ebuf = 0;
-                epar ^= 1;
-            }
-            const uint32_t row = mt * 128 + ew * 32 + lane;  // row of the (128*mtiles)-pixel box
-            int wi = row & ((1 << p.lbw) - 1);
-            int hi = (row >> p.lbw) & ((1 << p.lbh) - 1);
-            int ni = row >> (p.lbw + p.lbh);
-            if (p.halo) {  // sub-tile = 8 columns x 16 rows, second sub-tile to the right
-                wi = static_cast<int>((row & 7u) + mt * 8u);
-                hi = static_cast<int>((row >> 3) & 15u);
-                ni = 0;
-            }
-            const int w = (tw << p.lbw) + wi + wsh, h = (th << p.lbh) + hi, n = (tn << p.lbn) + ni;
-            const bool valid = (w < p.W) && (h < p.H) && (n < p.N) && !no_store;
-            const int64_t pix = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh +
-                                static_cast<int64_t>(w) * p.ow;
-
-            mbar_wait(&tfull[as], aph);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((ew * 32u) << 16) + as * p.block_n;
-            if (p.tma_store) {
-                // -------- staged epilogue: registers -> 128B-swizzled smem tile -> one TMA store per 64 channels.
-                // (direct per-thread stores write 32 B per lane at a 2*Cout-byte pitch: measured to cost up to half of the
-                // kernel time on short-K layers)
-                const int ow0 = (tw << p.lbw) + (mt ? p.mt_dw : 0) + wsh;
-                const int oh0 = (th << p.lbh) + (mt ? p.mt_dh : 0);
-                const int on0 = (tn << p.lbn) + (mt ? p.mt_dn : 0);
-                const uint32_t r = ew * 32 + lane;
-                const int ngroups = (p.block_n + 63) >> 6;
-                for (int cg = 0; cg < ngroups; ++cg) {
-                    if (col0 + cg * 64 >= p.Cout) break;  // uniform
-                    uint8_t* sbuf = sOut + (obuf & 1u) * 16384u;
-                    if (elected) bulk_wait_read<1>();  // the store issued from this buffer has drained it
-                    named_bar_sync(1, 128);
-                    // every thread is past its reads of the other aux tile (previous group): refill it for the next group
-                    if (aux_tma && elected) aux_issue_next();
-                    const uint8_t* abuf = sAux + (obuf & 1u) * 16384u;
-                    // both 32-column TMEM loads of this group are issued before the single wait (latency overlap)
-                    uint32_t v0[32], v1[32];
-                    const int cbase = cg * 64;
-                    const bool h0 = cbase < p.block_n, h1 = cbase + 32 < p.block_n;  // uniform
-                    if (h0) tmem_ld32(taddr + cbase, v0);
-                    if (h1) tmem_ld32(taddr + cbase + 32, v1);
-                    tmem_ld_wait();
-                    if (aux_tma) mbar_wait(&afull[obuf & 1u], (obuf >> 1) & 1u);
-#pragma unroll
-                    for (int c4 = 0; c4 < 4; ++c4) {
-                        const int c0 = cbase + c4 * 16;
-                        const int col = col0 + c0;
-                        float f[16];
-                        const bool have = (c4 < 2) ? h0 : h1;
-                        if (have) {  // uniform branch (no per-element selects: the epilogue is close to critical)
-#pragma unroll
-                            for (int j = 0; j < 16; ++j)
-                                f[j] = __uint_as_float((c4 < 2) ? v0[(c4 & 1) * 16 + j] : v1[(c4 & 1) * 16 + j]);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) f[j] = 0.f;
-                        }
-                        const bool live = (col + 16 <= p.Cout);  // uniform (Cout % 16 == 0 on this path)
-                        if (live) {
-                            if (has_bias) {  // 16 channels = four 16-byte loads (col % 16 == 0, bias base 16-byte aligned)
-                                const float4* bp = reinterpret_cast<const float4*>(p.bias + col);
-#pragma unroll
-                                for (int j4 = 0; j4 < 4; ++j4) {
-                                    const float4 b4 = __ldg(bp + j4);
-                                    f[4 * j4] += b4.x;
-                                    f[4 * j4 + 1] += b4.y;
-                                    f[4 * j4 + 2] += b4.z;
-                                    f[4 * j4 + 3] += b4.w;
-                                }
-                            }
-                            if (has_res && (valid || p.aux_tma == 1)) {
-                                uint4 r0, r1;
-                                if (p.aux_tma == 1) {  // out-of-range rows were zero-filled by the TMA load
-                                    const uint8_t* arow = abuf + r * 128u;
-                                    r0 = *reinterpret_cast<const uint4*>(arow + (((2 * c4) ^ (r & 7u)) << 4));
-                                    r1 = *reinterpret_cast<const uint4*>(arow + (((2 * c4 + 1) ^ (r & 7u)) << 4));
-                                } else {
-                                    const uint4* rp = reinterpret_cast<const uint4*>(
-                                        reinterpret_cast<const __nv_bfloat16*>(p.res) + pix + col);
-                                    r0 = __ldg(rp);
-                                    r1 = __ldg(rp + 1);
-                                }
-                                const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) {
-                                    float2 t = unpack_bf16x2(rr[j]);
-                                    f[2 * j] += t.x;
-                                    f[2 * j + 1] += t.y;
-                                }
-                            }
-                            if (do_relu) {
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], 0.f);
-                            }
-                            if (has_mask && (valid || p.aux_tma == 2)) {
-                                uint4 m0, m1;
-                                if (p.aux_tma == 2) {
-                                    const uint8_t* arow = abuf + r * 128u;
-                                    m0 = *reinterpret_cast<const uint4*>(arow + (((2 * c4) ^ (r & 7u)) << 4));
-                                    m1 = *reinterpret_cast<const uint4*>(arow + (((2 * c4 + 1) ^ (r & 7u)) << 4));
-                                } else {
-                                    const uint4* mp = reinterpret_cast<const uint4*>(
-                                        reinterpret_cast<const __nv_bfloat16*>(p.mask) + pix + col);
-                                    m0 = __ldg(mp);
-                                    m1 = __ldg(mp + 1);
-                                }
-                                const uint32_t mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) {
-                                    float2 t = unpack_bf16x2(mm[j]);
-                                    if (!(t.x > 0.f)) f[2 * j] = 0.f;
-                                    if (!(t.y > 0.f)) f[2 * j + 1] = 0.f;
-                                }
-                            }
-                        }
-                        uint4 o0, o1;
-                        o0.x = pack_bf16x2(f[0], f[1]);
-                        o0.y = pack_bf16x2(f[2], f[3]);
-                        o0.z = pack_bf16x2(f[4], f[5]);
-                        o0.w = pack_bf16x2(f[6], f[7]);
-                        o1.x = pack_bf16x2(f[8], f[9]);
-                        o1.y = pack_bf16x2(f[10], f[11]);
-                        o1.z = pack_bf16x2(f[12], f[13]);
-                        o1.w = pack_bf16x2(f[14], f[15]);
-                        uint8_t* rowp = sbuf + r * 128u;
-                        *reinterpret_cast<uint4*>(rowp + (((2 * c4) ^ (r & 7u)) << 4)) = o0;
-                        *reinterpret_cast<uint4*>(rowp + (((2 * c4 + 1) ^ (r & 7u)) << 4)) = o1;
-                        if (p.aux_tma == 3) {
-                            // ---- GroupNorm-backward statistics of these 16 channels of this row (dy = the bf16 values
-                            // just staged, x = the TMA-prefetched tile of the GroupNorm's input)
-                            const uint8_t* arow = abuf + r * 128u;
-                            const uint4 x0 = *reinterpret_cast<const uint4*>(arow + (((2 * c4) ^ (r & 7u)) << 4));
-                            const uint4 x1 = *reinterpret_cast<const uint4*>(arow + (((2 * c4 + 1) ^ (r & 7u)) << 4));
-                            const uint32_t xx[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-                            const uint32_t dd[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w};
-                            float s1[16], s2[16];
-                            const float* mrn = p.gn_mr + static_cast<int64_t>(on0) * p.gn_G * 2;
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float2 xv = unpack_bf16x2(xx[j]);
-                                const float2 dv = unpack_bf16x2(dd[j]);
-#pragma unroll
-                                for (int h = 0; h < 2; ++h) {
-                                    const int c = col + 2 * j + h;
-                                    const int g = c >> p.gn_lcpg;
-                                    const float mean = live ? __ldg(mrn + 2 * g) : 0.f;
-                                    const float rstd = live ? __ldg(mrn + 2 * g + 1) : 0.f;
-                                    const float ga = live ? __ldg(p.gn_gamma + c) : 0.f;
-                                    const float be = live ? __ldg(p.gn_beta + c) : 0.f;
-                                    const float xh = ((h ? xv.y : xv.x) - mean) * rstd;
-                                    const float u = fmaf(xh, ga, be);
-                                    float sg;
-                                    asm("tanh.approx.f32 %0, %1;" : "=f"(sg) : "f"(0.5f * u));
-                                    sg = fmaf(0.5f, sg, 0.5f);
-                                    const float du = (h ? dv.y : dv.x) * (sg * (1.f + u * (1.f - sg)));
-                                    s1[2 * j + h] = live ? du : 0.f;
-                                    s2[2 * j + h] = live ? du * xh : 0.f;
-                                }
-                            }
-                            // transposing butterfly: 16 channels x 32 rows -> lane l ends with channel (l >> 1) & 15
-                            bfly_step<8, 16>(s1, s2, lane);
-                            bfly_step<4, 8>(s1, s2, lane);
-                            bfly_step<2, 4>(s1, s2, lane);
-                            bfly_step<1, 2>(s1, s2, lane);
-                            s1[0] += __shfl_xor_sync(0xffffffffu, s1[0], 1);
-                            s2[0] += __shfl_xor_sync(0xffffffffu, s2[0], 1);
-                            if ((lane & 1u) == 0)
-                                *reinterpret_cast<float2*>(sStat + (ew * 64 + c4 * 16 + ((lane >> 1) & 15u)) * 2) =
-                                    make_float2(s1[0], s2[0]);
-                        }
-                    }
-                    fence_proxy_async_smem();
-                    named_bar_sync(1, 128);
-                    if (ew == 0 && lane == 0 && !no_store) {
-                        tma_store_4d(&p.omap, sbuf, col0 + cg * 64, ow0, oh0, on0);
-                        bulk_commit();
-                    }
-                    if (p.do_stats) {
-                        // GroupNorm statistics of the tile that was just staged (the bf16 values the consumer will read):
-                        // lane l sums channels 2l, 2l+1 of this 64-channel group over the warp's 32 rows (conflict-free
-                        // 32-bit reads of the swizzled rows), the 4 warps are combined through smem, then 128 fp32 atomics.
-                        float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
-                        const uint32_t jc = lane >> 2, wd = (lane & 3u) << 2;
-#pragma unroll 8
-                        for (uint32_t rr = 0; rr < 32; ++rr) {
-                            const uint32_t row = ew * 32 + rr;
-                            const uint32_t u = *reinterpret_cast<const uint32_t*>(sbuf + row * 128u + (((jc ^ (row & 7u)) << 4) | wd));
-                            const float2 xy = unpack_bf16x2(u);
-                            s0 += xy.x;
-                            q0 = fmaf(xy.x, xy.x, q0);
-                            s1 += xy.y;
-                            q1 = fmaf(xy.y, xy.y, q1);
-                        }
-                        float4* sc = reinterpret_cast<float4*>(sStat + (ew * 64 + 2 * lane) * 2);
-                        *sc = make_float4(s0, q0, s1, q1);
-                        named_bar_sync(2, 128);
-                        const uint32_t t = ew * 32 + lane;  // 0..127 -> (channel t/2, stat t&1)
-                        const int c = cg * 64 + static_cast<int>(t >> 1);
-                        if (col0 + c < p.Cout) {
-                            const float v = sStat[t] + sStat[128 + t] + sStat[256 + t] + sStat[384 + t];
-                            atomicAdd(p.stats + (static_cast<int64_t>(on0) * p.Cout + col0 + c) * 2 + (t & 1u), v);
-                        }
-                        named_bar_sync(2, 128);  // sStat is reused by the next group
-                    }
-                    if (p.aux_tma == 3) {
-                        named_bar_sync(2, 128);
-                        const uint32_t t = ew * 32 + lane;  // 0..127 -> (channel t/2, stat t&1)
-                        const int c = cg * 64 + static_cast<int>(t >> 1);
-                        if (col0 + c < p.Cout) {
-                            const float v = sStat[t] + sStat[128 + t] + sStat[256 + t] + sStat[384 + t];
-                            atomicAdd(p.gn_cs + (static_cast<int64_t>(on0) * p.Cout + col0 + c) * 2 + (t & 1u), v);
-                        }
-                        named_bar_sync(2, 128);  // sStat is reused by the next group
-                    }
-                    ++obuf;
-                }
-            } else
-            for (int c0 = 0; c0 < p.block_n; c0 += 16) {
-                uint32_t v[16];
-                tmem_ld16(taddr + c0, v);
-                tmem_ld_wait();
-                const int col = col0 + c0;
-                if (col >= p.Cout) continue;  // warp-uniform
-                float f[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
-                if (has_bias) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (col + j < p.Cout) f[j] += __ldg(p.bias + col + j);
-                }
-                const bool full16 = (col + 16 <= p.Cout);
-                if (vec_path && full16) {
-                    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + pix + col;
-                    if (valid) {
-                        if (has_res) {
-                            const uint4* r = reinterpret_cast<const uint4*>(
-                                reinterpret_cast<const __nv_bfloat16*>(p.res) + pix + col);
-                            uint4 r0 = __ldg(r), r1 = __ldg(r + 1);
-                            const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                float2 t = unpack_bf16x2(rr[j]);
-                                f[2 * j] += t.x;
-                                f[2 * j + 1] += t.y;
-                            }
-                        }
-                        if (do_relu) {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], 0.f);
-                        }
-                        if (has_mask) {
-                            const uint4* m = reinterpret_cast<const uint4*>(
-                                reinterpret_cast<const __nv_bfloat16*>(p.mask) + pix + col);
-                            uint4 m0 = __ldg(m), m1 = __ldg(m + 1);
-                            const uint32_t mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                float2 t = unpack_bf16x2(mm[j]);
-                                if (!(t.x > 0.f)) f[2 * j] = 0.f;
-                                if (!(t.y > 0.f)) f[2 * j + 1] = 0.f;
-                            }
-                        }
-                        uint4 o0, o1;
-                        o0.x = pack_bf16x2(f[0], f[1]);
-                        o0.y = pack_bf16x2(f[2], f[3]);
-                        o0.z = pack_bf16x2(f[4], f[5]);
-                        o0.w = pack_bf16x2(f[6], f[7]);
-                        o1.x = pack_bf16x2(f[8], f[9]);
-                        o1.y = pack_bf16x2(f[10], f[11]);
-                        o1.z = pack_bf16x2(f[12], f[13]);
-                        o1.w = pack_bf16x2(f[14], f[15]);
-                        reinterpret_cast<uint4*>(o)[0] = o0;
-                        reinterpret_cast<uint4*>(o)[1] = o1;
-                    }
-                } else if (valid) {
-                    // generic strided / ragged path (small Cout, NCHW fp32 outputs)
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        if (col + j < p.Cout) {
-                            const int64_t a = pix + static_cast<int64_t>(col + j) * p.oc;
-                            float x = f[j];
-                            if (has_res) x += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.res)[a]);
-                            if (do_relu) x = fmaxf(x, 0.f);
-                            if (has_mask &&
-                                !(__bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.mask)[a]) > 0.f))
-                                x = 0.f;
-                            if (p.out_f32)
-                                reinterpret_cast<float*>(p.out)[a] = x;
-                            else
-                                reinterpret_cast<__nv_bfloat16*>(p.out)[a] = __float2bfloat16(x);
-                            f[j] = x;
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            if constexpr (PAIR) {
-                if (crank != 0)
-                    mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[as]), 0));
-                else
-                    mbar_arrive(&tempty[as]);
-            } else {
-                mbar_arrive(&tempty[as]);
-            }
-          }
-        }
-        if (p.tma_store && ew == 0 && lane == 0) bulk_wait_all();  // smem must outlive the last bulk stores
-        }
+        return;
     }
 
-    tc_fence_before();
-    if constexpr (PAIR)
-        cluster_sync_all();  // neither CTA may exit (or free TMEM) while the other still signals into it
-    else
-        __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        if constexpr (PAIR)
-            tmem_dealloc_pair(tmem_base, p.tmem_cols);
-        else
-            tmem_dealloc(tmem_base, p.tmem_cols);
+    // ===================== consumers: warpgroup cw owns rows 64*cw .. 64*cw + 63 of every tile =====================
+    const uint32_t cw = wg - 1;
+    const uint32_t cwarp = cw * 4 + warp;  // 0..7
+    const uint32_t ctid = threadIdx.x - 128;  // 0..255
+    const uint32_t ring = smem_u32(base);
+    const bool has_bias = p.flags & VQB_EPI_BIAS, has_res = p.flags & VQB_EPI_RES;
+    const bool do_relu = p.flags & VQB_EPI_RELU, has_mask = p.flags & VQB_EPI_MASK;
+    const bool vec_path = (p.oc == 1) && (p.out_f32 == 0);
+    const bool do_gn = p.gn_cs != nullptr;
+    const bool reduce = p.do_stats || do_gn;
+    const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.res);
+    const __nv_bfloat16* mask = reinterpret_cast<const __nv_bfloat16*>(p.mask);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    uint32_t stage = 0, phase = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        uint32_t prev = 0;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const uint32_t a = ring + stage * kStageBytes;
+            const uint64_t da = make_smem_desc(a + cw * 8192u, 16, 1024);
+            const uint64_t db = make_smem_desc(a + kABytes, 16, 1024);
+            fence_operands(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kBlockK / 16; ++k)  // +32 B per K = 16 step inside the swizzle atom
+                wgmma_bf16<BN, 0, 0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+            wgmma_commit();
+            fence_operands(acc);
+            // keep this K-chunk's group in flight while the next stage is awaited; the previous one has retired
+            wgmma_wait<1>();
+            if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
+            prev = stage;
+            if (++stage == stages) {
+                stage = 0;
+                phase ^= 1;
+            }
+        }
+        wgmma_wait<0>();
+        fence_operands(acc);  // the epilogue's reads of acc stay below the wait
+        if (lane == 0) mbar_arrive(&empty[prev]);  // num_kb >= 1 (ntaps >= 1, C > 0)
+
+        // ---------------- epilogue straight from the accumulator fragment
+        const int n_tile = tile % p.n_tiles;
+        const int m_tile = tile / p.n_tiles;
+        const int tw = m_tile % p.tiles_w;
+        const int th = (m_tile / p.tiles_w) % p.tiles_h;
+        const int tn = m_tile / (p.tiles_w * p.tiles_h);
+        const int col0 = n_tile * BN;
+        int64_t pix[2];
+        bool valid[2];
+        int img[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const uint32_t row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;  // row of the 128-pixel box
+            const int w = (tw << p.lbw) + static_cast<int>(row & ((1u << p.lbw) - 1));
+            const int h = (th << p.lbh) + static_cast<int>((row >> p.lbw) & ((1u << p.lbh) - 1));
+            const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh));
+            valid[i] = (w < p.W) && (h < p.H) && (n < p.N);
+            img[i] = n;
+            pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh + static_cast<int64_t>(w) * p.ow;
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int col = col0 + j * 8 + 2 * static_cast<int>(lane & 3u);
+            const bool ok0 = col < p.Cout, ok1 = col + 1 < p.Cout;
+            float b0 = 0.f, b1 = 0.f;
+            if (has_bias) {
+                b0 = ok0 ? __ldg(p.bias + col) : 0.f;
+                b1 = ok1 ? __ldg(p.bias + col + 1) : 0.f;
+            }
+            float r1[2] = {0.f, 0.f}, r2[2] = {0.f, 0.f};  // per column: statistics partial sums over this thread's rows
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                float f[2] = {acc[4 * j + 2 * i] + b0, acc[4 * j + 2 * i + 1] + b1};
+                if (!valid[i]) continue;
+                if (vec_path && ok1) {
+                    const int64_t o = pix[i] + col;  // 4-byte aligned: pixel strides % 8 == 0, col even
+                    if (has_res) {
+                        const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(res + o));
+                        f[0] += r.x;
+                        f[1] += r.y;
+                    }
+                    if (do_relu) {
+                        f[0] = fmaxf(f[0], 0.f);
+                        f[1] = fmaxf(f[1], 0.f);
+                    }
+                    if (has_mask) {
+                        const float2 m = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(mask + o));
+                        if (!(m.x > 0.f)) f[0] = 0.f;
+                        if (!(m.y > 0.f)) f[1] = 0.f;
+                    }
+                    const __nv_bfloat162 ob = __floats2bfloat162_rn(f[0], f[1]);
+                    *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.out) + o) = ob;
+                    if (reduce) {
+                        const float2 v = __bfloat1622float2(ob);  // the bf16 values the consumer will read
+                        if (do_gn) {
+                            const float2 xv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.gn_x + o));
+                            const float* mr = p.gn_mr + static_cast<int64_t>(img[i]) * p.gn_G * 2;
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int c = col + e;
+                                const int g = c >> p.gn_lcpg;
+                                const float xh = ((e ? xv.y : xv.x) - __ldg(mr + 2 * g)) * __ldg(mr + 2 * g + 1);
+                                const float u = fmaf(xh, __ldg(p.gn_gamma + c), __ldg(p.gn_beta + c));
+                                float sg;
+                                asm("tanh.approx.f32 %0, %1;" : "=f"(sg) : "f"(0.5f * u));
+                                sg = fmaf(0.5f, sg, 0.5f);
+                                const float du = (e ? v.y : v.x) * (sg * (1.f + u * (1.f - sg)));
+                                r1[e] += du;
+                                r2[e] = fmaf(du, xh, r2[e]);
+                            }
+                        } else {
+                            r1[0] += v.x;
+                            r2[0] = fmaf(v.x, v.x, r2[0]);
+                            r1[1] += v.y;
+                            r2[1] = fmaf(v.y, v.y, r2[1]);
+                        }
+                    }
+                } else {
+                    // generic strided / ragged path (small or odd Cout, NCHW fp32 outputs)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        if (!(e ? ok1 : ok0)) continue;
+                        const int64_t o = pix[i] + static_cast<int64_t>(col + e) * p.oc;
+                        float x = f[e];
+                        if (has_res) x += __bfloat162float(res[o]);
+                        if (do_relu) x = fmaxf(x, 0.f);
+                        if (has_mask && !(__bfloat162float(mask[o]) > 0.f)) x = 0.f;
+                        if (p.out_f32)
+                            reinterpret_cast<float*>(p.out)[o] = x;
+                        else
+                            reinterpret_cast<__nv_bfloat16*>(p.out)[o] = __float2bfloat16(x);
+                    }
+                }
+            }
+            if (reduce) {  // warp-uniform: sum the 8 row groups of the warp (lane bits 2..4), then stage per warp
+#pragma unroll
+                for (int off = 4; off < 32; off <<= 1) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        r1[e] += __shfl_xor_sync(0xffffffffu, r1[e], off);
+                        r2[e] += __shfl_xor_sync(0xffffffffu, r2[e], off);
+                    }
+                }
+                if (lane < 4) {
+                    float* s = sStat + (cwarp * BN + j * 8 + 2 * lane) * 2;
+                    *reinterpret_cast<float4*>(s) = make_float4(r1[0], r2[0], r1[1], r2[1]);
+                }
+            }
+        }
+        if (reduce) {
+            // the statistics need every row of the tile inside one image (checked on the host: vqb_conv_stats_ok)
+            named_bar_sync(1, 256);
+            float* dst = do_gn ? p.gn_cs : p.stats;
+            const int n_img = tn << p.lbn;
+            for (uint32_t idx = ctid; idx < BN * 2u; idx += 256u) {
+                const int c = col0 + static_cast<int>(idx >> 1);
+                float v = 0.f;
+#pragma unroll
+                for (int w8 = 0; w8 < kConsumerWarps; ++w8) v += sStat[w8 * BN * 2 + idx];
+                if (c < p.Cout) atomicAdd(dst + (static_cast<int64_t>(n_img) * p.Cout + c) * 2 + (idx & 1u), v);
+            }
+            named_bar_sync(1, 256);  // sStat is reused by the next tile
+        }
     }
 }
 
@@ -940,6 +300,21 @@ static int fill_views(const VqbView* views, int nviews, const void* a, int C, in
         int rc = encode_tmap_bf16(&maps[v], base, 4, dims, str, box, 128);
         if (rc != VQB_OK) return rc;
     }
+    return VQB_OK;
+}
+
+template <int BN>
+static int launch_conv(const ConvParams& p, void* stream) {
+    constexpr size_t stage_bytes = kABytes + BN * kBlockK * 2;
+    const size_t smem = 1024 + p.stages * stage_bytes + kConsumerWarps * BN * 2 * sizeof(float) + 2 * 8 * p.stages;
+    static bool attr_set = false;
+    if (!attr_set) {
+        VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        attr_set = true;
+    }
+    const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
+    conv_gemm_kernel<BN><<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
+    VQB_CUDA(cudaGetLastError());
     return VQB_OK;
 }
 
@@ -970,7 +345,7 @@ extern "C" int vqb_conv_gnbwd_ok(const VqbConvDesc* d, int groups) {
     const int cpg = d->Cout / groups;
     if ((cpg & (cpg - 1)) != 0) return 0;
     if (d->flags & (VQB_EPI_RES | VQB_EPI_MASK | VQB_EPI_STATS | VQB_EPI_RELU)) return 0;
-    return vqb_conv_stats_ok(d);  // same geometry conditions: staged epilogue, whole sub-tiles inside one image
+    return vqb_conv_stats_ok(d);  // same geometry conditions: NHWC bf16 output, whole tiles inside one image
 }
 
 // 1 if vqb_conv_gemm can produce GroupNorm statistics (VQB_EPI_STATS) for this descriptor, else 0.
@@ -999,135 +374,39 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     if ((d->flags & VQB_EPI_RES)) VQB_CHECK(res != nullptr, "vqb_conv_gemm: VQB_EPI_RES without res");
     if ((d->flags & VQB_EPI_MASK)) VQB_CHECK(mask != nullptr, "vqb_conv_gemm: VQB_EPI_MASK without mask");
     if ((d->flags & VQB_EPI_STATS)) VQB_CHECK(stats != nullptr, "vqb_conv_gemm: VQB_EPI_STATS without stats");
-    if (d->oc == 1 && !d->out_f32) {
+    const bool nhwc_bf16 = d->oc == 1 && !d->out_f32;
+    if (nhwc_bf16) {
         VQB_CHECK(d->on % 8 == 0 && d->oh % 8 == 0 && d->ow % 8 == 0 &&
                       (reinterpret_cast<uintptr_t>(out) & 15u) == 0,
                   "vqb_conv_gemm: NHWC bf16 output needs 16-byte aligned pixel rows");
+        const uintptr_t ops = reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(mask) |
+                              reinterpret_cast<uintptr_t>(gn ? gn->x : nullptr);
+        VQB_CHECK((ops & 3u) == 0, "vqb_conv_gemm: residual / mask / GroupNorm input must be 4-byte aligned");
     }
     for (int t = 0; t < d->ntaps; ++t)
         VQB_CHECK(d->taps[t].view >= 0 && d->taps[t].view < d->nviews, "vqb_conv_gemm: tap %d view out of range", t);
-    if (!query_only && !device_is_sm100()) return set_error(VQB_ENODEVICE, "vqb_conv_gemm: current device is not sm_100");
+    if (!query_only && !device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_conv_gemm: current device is not sm_90");
 
-    ConvParams p;  // ~2.7 KB, filled per call, passed by value (__grid_constant__) to the kernel
-    const int p_dbg = debug_mode();
-    // Halo mode: one dense view, taps = shifts within a <= 3x3 window, 64-channel chunks, staged bf16 NHWC output.
-    // Tile = 16 x 16 output pixels of one image (two 8 x 16 sub-tiles side by side) x 128 output channels.
-    // (Cout < 128: 64-column MMAs are issue/smem bound either way and the per-tap path measured ~10 % faster)
-    //  Cout <= 32 (decoder conv_out, data gradients of 3-channel layers; any output format, direct-store epilogue): the
-    //  nine-fold L2->SM re-read of the activations is all there is to save, so the halo wins there too)
-    // (round 2: with the issue thread no longer the limiter the halo tile also wins for 64-channel outputs — VGG 64->64 @
-    //  256^2 — VQB_HALO_MIN_COUT overrides the threshold for A/B measurements)
-    static const int halo_min_cout = [] {
-        const char* e = getenv("VQB_HALO_MIN_COUT");
-        return e ? atoi(e) : 128;
-    }();
-    const bool halo_big = d->oc == 1 && !d->out_f32 && d->Cout % 16 == 0 && d->Cout >= halo_min_cout && !(p_dbg & 256);
-    bool halo = !(p_dbg & 1024) && d->nviews == 1 && d->ntaps >= 2 && d->C % 64 == 0 && d->W > 8 && d->H > 8 &&
-                (halo_big || d->Cout <= 32);
-    int dwmin = 0, dwmax = 0, dhmin = 0, dhmax = 0;
-    if (halo) {
-        dwmin = dwmax = d->taps[0].dw;
-        dhmin = dhmax = d->taps[0].dh;
-        for (int t = 0; t < d->ntaps; ++t) {
-            dwmin = d->taps[t].dw < dwmin ? d->taps[t].dw : dwmin;
-            dwmax = d->taps[t].dw > dwmax ? d->taps[t].dw : dwmax;
-            dhmin = d->taps[t].dh < dhmin ? d->taps[t].dh : dhmin;
-            dhmax = d->taps[t].dh > dhmax ? d->taps[t].dh : dhmax;
-        }
-        if (dwmax - dwmin > 2 || dhmax - dhmin > 2) halo = false;
-    }
-    int block_n;
-    const bool f_res = d->flags & VQB_EPI_RES, f_mask = d->flags & VQB_EPI_MASK;
-    const bool swap = halo && d->Cout > 64 && d->Cout <= 128 && d->H >= 32 && !(f_res && f_mask) &&
-                      !((f_res || f_mask) && (p_dbg & 512)) && (p_dbg & 4096);
-    // (swap mode is OFF by default: measured 906 vs 1164 TFLOP/s on 128->128 @ 256^2 — the transposed epilogue's 16-bit
-    //  shared-memory stores/loads compete with the MMA operand reads for the shared-memory port and stop overlapping;
-    //  kept behind debug bit 4096 with its tests for the stmatrix-based epilogue that would fix it)
-    // N = 256 keeps the MMA's shared-memory operand reads under 128 B/clk (an M128 x N128 x K16 MMA reads 8 KB in its 64
-    // cycles: exactly the limit); with 256 columns one 8 x 16 sub-tile per CTA tile leaves room for TMEM double buffering.
-    const int halo_mtiles = (d->Cout >= 256 && !(p_dbg & 2048)) ? 1 : 2;
-    // CTA pairs (cta_group::2, M = 256 MMAs, half a weight tile per CTA) for the 128-channel layers: functionally complete
-    // and tested, but measured SLOWER than two independent N = 128 streams (1040 vs 1192 TFLOP/s on 128->128 @ 256^2
-    // with three weight tiles per ring stage; 814 with one) — the single issuing thread now feeds two tensor cores and
-    // every stage hand-off crosses SMs. Opt-in through debug bit 8192 until that is understood.
-    const bool pair = halo && !swap && halo_big && d->Cout == 128 && (p_dbg & 8192);
-    p.pair = pair ? 1 : 0;
-    if (swap)
-        block_n = 256;  // accumulator columns = pixels
-    else if (halo)
-        block_n = d->Cout >= 256 ? (halo_mtiles == 1 ? 256 : 128) : (d->Cout >= 128 ? 128 : ((d->Cout + 31) / 32) * 32);
-    else if (d->Cout >= 256)
-        block_n = 256;
-    else
-        block_n = ((d->Cout + 15) / 16) * 16;
-    p.block_n = block_n;
-    p.n_tiles = swap ? 1 : (d->Cout + block_n - 1) / block_n;
-    p.swap = swap ? 1 : 0;
-    // Pixel box per CTA tile: 128*mtiles output pixels. mtiles = 2 shares every weight tile between two 128-row
-    // accumulators (25-33 % less L2->SM traffic per FLOP, the measured limiter); it is used when it does not cost
-    // more in wave quantisation than it gains.
-    auto tiles_for = [&](int mt, uint32_t& bw, uint32_t& bh, uint32_t& bn) {
-        const uint32_t px = 128u * mt;
-        bw = next_pow2(d->W);
-        if (bw > 128) bw = 128;  // <= 256 rows per TMA box dimension; keep W boxes at 128
-        bh = next_pow2(d->H);
-        if (bh > px / bw) bh = px / bw;
-        bn = px / (bw * bh);
-        return static_cast<int64_t>((d->W + bw - 1) / bw) * ((d->H + bh - 1) / bh) * ((d->N + bn - 1) / bn) * p.n_tiles;
-    };
-    uint32_t bw, bh, bn, bw2, bh2, bn2;
-    const int64_t t1 = tiles_for(1, bw, bh, bn);
-    const int64_t t2 = tiles_for(2, bw2, bh2, bn2);
-    const int sms = num_sms() > 0 ? num_sms() : 148;
-    // measured gain of the double tile (tools/perf_experiments.py): ~1.15-1.3x when BLOCK_N <= 128 (four TMEM buffers keep
-    // the epilogue fully overlapped), ~1.05x at BLOCK_N = 256, a loss for short K loops (1x1 convs: epilogue bound)
-    const int num_kb_host = d->ntaps * ((d->C + kBlockK - 1) / kBlockK);
-    const double gain = block_n <= 128 ? 1.2 : 1.05;
-    const double cost1 = static_cast<double>((t1 + sms - 1) / sms) * 1.0;
-    const double cost2 = static_cast<double>((t2 + sms - 1) / sms) * 2.0 / gain;
-    int mtiles = (!(p_dbg & 32) && bn2 <= 256 && num_kb_host >= 9 && cost2 < cost1) ? 2 : 1;
-    if (mtiles == 2) {
-        bw = bw2;
-        bh = bh2;
-        bn = bn2;
-    }
-    if (halo) {
-        mtiles = (swap || pair) ? 1 : halo_mtiles;
-        bw = pair ? 16 : 8 * mtiles;  // pair: the 16-wide tile is split between the two CTAs (8 columns each)
-        bh = swap ? 32 : 16;
-        bn = 1;
-    }
-    p.mtiles = mtiles;
+    ConvParams p;  // ~2.5 KB, filled per call, passed by value (__grid_constant__) to the kernel
+    // BLOCK_N: 128 accumulator columns per warpgroup (64 fp32 registers per thread) for wide layers; narrow layers
+    // round Cout up to the next wgmma width so that no tensor-core work is spent on padding beyond it.
+    const int block_n = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : (d->Cout > 16 ? 32 : 16));
+    p.n_tiles = (d->Cout + block_n - 1) / block_n;
+    // pixel box per CTA tile: 128 output pixels, as wide as the image (<= 128), then as tall, then across images
+    uint32_t bw = next_pow2(d->W);
+    if (bw > 128) bw = 128;
+    uint32_t bh = next_pow2(d->H);
+    if (bh > 128 / bw) bh = 128 / bw;
+    const uint32_t bn = 128 / (bw * bh);
     p.lbw = ilog2(bw);
     p.lbh = ilog2(bh);
     p.lbn = ilog2(bn);
     p.tiles_w = (d->W + bw - 1) / bw;
     p.tiles_h = (d->H + bh - 1) / bh;
-    p.tiles_nb = (d->N + bn - 1) / bn;
-    p.total_tiles = p.tiles_w * p.tiles_h * p.tiles_nb * p.n_tiles;
-    // TMA-store epilogue: NHWC bf16 outputs (any pixel strides) with Cout % 16 == 0
-    const bool tma_store = (d->oc == 1) && !d->out_f32 && (d->Cout % 16 == 0) && (block_n % 32 == 0) && !(p_dbg & 256);
-    p.tma_store = tma_store ? 1 : 0;
-    p.mt_dh = 0;
-    p.mt_dn = 0;
-    uint32_t obw = bw, obh = bh, obn = bn;  // 128-pixel store box = one accumulator sub-tile
-    p.mt_dw = 0;
-    p.halo = halo ? 1 : 0;
-    if (halo) {
-        obw = 8;
-        obh = 16;
-        p.mt_dw = 8;
-    } else if (mtiles == 2) {
-        if (bn >= 2) {
-            obn = bn / 2;
-            p.mt_dn = static_cast<int32_t>(obn);
-        } else {
-            obh = bh / 2;
-            p.mt_dh = static_cast<int32_t>(obh);
-        }
-    }
-    // GroupNorm statistics in the epilogue: staged path only, every 128-row sub-tile inside one image, no ragged tiles
-    const bool stats_ok = tma_store && obn == 1 && (d->W % bw == 0) && (d->H % bh == 0) && (d->Cout % 64 == 0);
+    const int tiles_nb = (d->N + bn - 1) / bn;
+    p.total_tiles = p.tiles_w * p.tiles_h * tiles_nb * p.n_tiles;
+    // GroupNorm statistics in the epilogue: NHWC bf16 output, every tile inside one image, no ragged tiles
+    const bool stats_ok = nhwc_bf16 && bn == 1 && (d->W % bw == 0) && (d->H % bh == 0) && (d->Cout % 64 == 0);
     if (d->flags & VQB_EPI_STATS) {
         if (!stats_ok)
             return set_error(VQB_EINVAL, "vqb_conv_gemm: VQB_EPI_STATS unsupported for this shape (N=%d H=%d W=%d Cout=%d)",
@@ -1135,15 +414,17 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     }
     p.do_stats = (d->flags & VQB_EPI_STATS) ? 1 : 0;
     if (query_only) return stats_ok ? 1 : 0;
+    p.gn_x = nullptr;
     p.gn_mr = p.gn_gamma = p.gn_beta = nullptr;
     p.gn_cs = nullptr;
     p.gn_G = p.gn_lcpg = 0;
     if (gn) {
         const int cpg = d->Cout / gn->groups;
-        VQB_CHECK(stats_ok && !(p_dbg & 512) && d->Cout % gn->groups == 0 && (cpg & (cpg - 1)) == 0 &&
+        VQB_CHECK(stats_ok && d->Cout % gn->groups == 0 && (cpg & (cpg - 1)) == 0 &&
                       !(d->flags & (VQB_EPI_RES | VQB_EPI_MASK | VQB_EPI_STATS | VQB_EPI_RELU)),
                   "vqb_conv_gemm_gnbwd: unsupported shape / flags (N=%d H=%d W=%d Cout=%d groups=%d)", d->N, d->H, d->W,
                   d->Cout, gn->groups);
+        p.gn_x = static_cast<const __nv_bfloat16*>(gn->x);
         p.gn_mr = gn->mr;
         p.gn_gamma = gn->gamma;
         p.gn_beta = gn->beta;
@@ -1151,44 +432,11 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
         p.gn_G = gn->groups;
         p.gn_lcpg = ilog2(static_cast<uint32_t>(cpg));
     }
-    const int stage_bytes = mtiles * kABytes + block_n * kBlockK * 2;
-    // residual / ReLU-gate operand through TMA (debug bit 512 keeps the per-thread loads)
-    const int aux_tma = gn ? 3 : ((tma_store && !(p_dbg & 512)) ? ((d->flags & VQB_EPI_RES) ? 1 : ((d->flags & VQB_EPI_MASK) ? 2 : 0)) : 0);
-    p.aux_tma = aux_tma;
-    const int epi_smem = swap ? 4 * 16384 + 2048 : (tma_store ? 2 * 16384 + 2048 : 0) + (aux_tma ? 2 * 16384 : 0);
-    p.epi_bytes = epi_smem;
-    int stages = (227 * 1024 - 1536 - epi_smem) / stage_bytes;
-    size_t ring_bytes = 0;
-    p.h_bytes = p.h_stages = p.h_sbo = p.h_w0 = p.h_h0 = p.h_tx = 0;
-    p.tps = 1;
-    if (halo) {
-        const int P = 8 * mtiles + (dwmax - dwmin), Q = (swap ? 32 : 16) + (dhmax - dhmin);  // per CTA
-        p.h_sbo = P * 128;
-        p.h_tx = P * Q * 128;
-        p.h_bytes = (p.h_tx + 1023) / 1024 * 1024;
-        p.h_stages = pair ? 4 : 2;  // pair: a chunk is only 9 x 256 MMA cycles, shorter than one halo load's latency
-        p.h_w0 = dwmin;
-        p.h_h0 = dhmin;
-        p.tps = (pair && d->ntaps % 3 == 0 && !(p_dbg & 16384)) ? 3 : 1;
-        if (pair) p.h_stages = (p.tps == 3 && aux_tma) ? 3 : 4;
-        const int b_bytes = (swap ? 128 : (pair ? block_n / 2 : block_n)) * kBlockK * 2 * p.tps;  // per ring stage
-        stages = (227 * 1024 - 1536 - epi_smem - p.h_stages * p.h_bytes) / b_bytes;
-        if (stages > kMaxStages) stages = kMaxStages;
-        VQB_CHECK(stages >= 2, "vqb_conv_gemm: halo mode does not fit in shared memory");
-        ring_bytes = static_cast<size_t>(p.h_stages) * p.h_bytes + static_cast<size_t>(stages) * b_bytes;
-        for (int t = 0; t < d->ntaps; ++t)
-            p.tap_off16[t] = static_cast<uint32_t>(((d->taps[t].dh - dhmin) * P + (d->taps[t].dw - dwmin)) * 8);
-    } else {
-        if (stages > kMaxStages) stages = kMaxStages;
-        ring_bytes = static_cast<size_t>(stages) * stage_bytes;
-    }
+    const int stage_bytes = kABytes + block_n * kBlockK * 2;
+    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages;
+    int stages = (227 * 1024 - fixed) / stage_bytes;
+    if (stages > kMaxStages) stages = kMaxStages;
     p.stages = stages;
-    int nbuf = 512 / block_n;
-    if (nbuf > 4) nbuf = 4;
-    p.nbuf = nbuf;
-    uint32_t tc = next_pow2(nbuf * block_n);
-    if (tc < 32) tc = 32;
-    p.tmem_cols = tc;
     p.ntaps = d->ntaps;
     p.kchunks = (d->C + kBlockK - 1) / kBlockK;
     p.C = d->C;
@@ -1207,11 +455,6 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     p.mask = mask;
     p.bias = bias;
     p.stats = stats;
-    p.dbg = debug_mode();
-    static const int lean_issue = [] { const char* e = getenv("VQB_LEAN_ISSUE"); return e ? atoi(e) : 1; }();
-    p.lean = lean_issue;
-    static const int issue2_env = [] { const char* e = getenv("VQB_ISSUE2"); return e ? atoi(e) : 0; }();
-    p.issue2 = issue2_env;
     for (int t = 0; t < d->ntaps; ++t) {
         p.tap_view[t] = d->taps[t].view;
         p.tap_dw[t] = d->taps[t].dw;
@@ -1219,67 +462,21 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     }
     int rc = fill_views(d->views, d->nviews, a, d->C, p.lbw, p.lbh, p.lbn, p.amap);
     if (rc != VQB_OK) return rc;
-    if (halo) {  // the activation box is the 16 x 16 tile plus its halo
-        const VqbView& vw = d->views[0];
-        uint64_t dims[4] = {static_cast<uint64_t>(d->C), static_cast<uint64_t>(vw.Wv), static_cast<uint64_t>(vw.Hv),
-                            static_cast<uint64_t>(vw.Nv)};
-        uint64_t str[3] = {static_cast<uint64_t>(vw.sw) * 2, static_cast<uint64_t>(vw.sh) * 2,
-                           static_cast<uint64_t>(vw.sn) * 2};
-        uint32_t box[4] = {kBlockK, static_cast<uint32_t>(8 * mtiles + dwmax - dwmin),
-                           static_cast<uint32_t>((swap ? 32 : 16) + dhmax - dhmin), 1};
-        rc = encode_tmap_bf16(&p.amap[0], static_cast<const uint8_t*>(a) + vw.offset * 2, 4, dims, str, box, 128);
-        if (rc != VQB_OK) return rc;
-    }
     {
         const uint64_t ktot = static_cast<uint64_t>(d->ntaps) * d->C;
         uint64_t dims[2] = {ktot, static_cast<uint64_t>(d->Cout)};
         uint64_t str[1] = {ktot * 2};
-        uint32_t box[2] = {kBlockK, static_cast<uint32_t>(swap ? 128 : (pair ? block_n / 2 : block_n))};
+        uint32_t box[2] = {kBlockK, static_cast<uint32_t>(block_n)};
         rc = encode_tmap_bf16(&p.bmap, w_packed, 2, dims, str, box, 128);
         if (rc != VQB_OK) return rc;
     }
-    if (tma_store) {
-        uint64_t dims[4] = {static_cast<uint64_t>(d->Cout), static_cast<uint64_t>(d->W), static_cast<uint64_t>(d->H),
-                            static_cast<uint64_t>(d->N)};
-        uint64_t str[3] = {static_cast<uint64_t>(d->ow) * 2, static_cast<uint64_t>(d->oh) * 2,
-                           static_cast<uint64_t>(d->on) * 2};
-        uint32_t box[4] = {64, obw, obh, obn};
-        rc = encode_tmap_bf16(&p.omap, out, 4, dims, str, box, 128);
-        if (rc != VQB_OK) return rc;
-        if (aux_tma) {
-            rc = encode_tmap_bf16(&p.xmap, aux_tma == 1 ? res : (aux_tma == 2 ? mask : gn->x), 4, dims, str, box, 128);
-            if (rc != VQB_OK) return rc;
-        }
+    switch (block_n) {
+        case 16: rc = launch_conv<16>(p, stream); break;
+        case 32: rc = launch_conv<32>(p, stream); break;
+        case 64: rc = launch_conv<64>(p, stream); break;
+        default: rc = launch_conv<128>(p, stream); break;
     }
-    const size_t smem = 1024 + ring_bytes + epi_smem + 512;
-    static bool attr_set = false;
-    if (!attr_set) {
-        VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set = true;
-    }
-    int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-    if (pair) {
-        // one cluster of two CTAs (a cta_group::2 pair on one TPC) per tile stream
-        int pairs = num_sms() / 2;
-        if (pairs > p.total_tiles) pairs = p.total_tiles;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(static_cast<unsigned>(2 * pairs));
-        cfg.blockDim = dim3(kThreads);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = static_cast<cudaStream_t>(stream);
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        VQB_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<true>, p));
-    } else {
-        conv_gemm_kernel<false><<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
-    }
-    VQB_CUDA(cudaGetLastError());
+    if (rc != VQB_OK) return rc;
     count_launch();
     return VQB_OK;
 }

@@ -36,7 +36,7 @@ __device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&f)[8]) {
 }
 // sigmoid(x) = 0.5 + 0.5 tanh(x/2) with the single-instruction MUFU.TANH (abs error of the sigmoid <= ~2.5e-4, an order
 // of magnitude below the bf16 rounding of the activations it multiplies): one SFU op instead of ex2 + rcp. The GroupNorm
-// kernels sit at the SFU / FP32-issue / HBM triple point (ncu: XU 42 %, issue 52 %, DRAM 57 %), so this is time.
+// kernels are limited by special-function and FP32 issue throughput as much as by HBM bandwidth, so this is time.
 __device__ __forceinline__ float sigmoidf_(float x) {
 #if VQB_EXACT_SIGMOID
     return 1.f / (1.f + __expf(-x));
@@ -333,8 +333,8 @@ __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, const 
         const int p0 = blockIdx.x * pix_per_chunk;
         const int p1 = min(HW, p0 + pix_per_chunk);
         const int64_t base = (static_cast<int64_t>(n) * HW) * C + cv * 8;
-        // 4 pixel rows (8 x 16-byte loads) in flight per thread: with 2 rows the kernel sat at 57 % of HBM bandwidth on
-        // load latency (ncu: 16 warps/SM, long-scoreboard stalls)
+        // 4 pixel rows (8 x 16-byte loads) in flight per thread: with few warps per SM, fewer rows leave the kernel
+        // waiting on load latency instead of streaming HBM
         for (int p = p0 + pr; p < p1; p += U * R) {
             uint4 ux[U], ud[U];
 #pragma unroll
@@ -486,9 +486,9 @@ gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
 // ------------------------------------------------------------------ GroupNorm backward, persistent L2-pipelined form
 // One persistent launch does reduce AND apply. The two-kernel form reads x and dy twice from HBM (10 B/element, 12 with
 // the skip gradient). Here the work is ordered  R(0) R(1) A(0) R(2) A(1) ... A(N-1)  (R(n) = statistics of sample n,
-// A(n) = dx of sample n): when A(n) re-reads x, dy of sample n they were streamed at most one sample ago and (for every
-// layer of the FLUX config: x + dy of one sample <= 34 MB of the 126 MB L2) are still L2 resident — HBM traffic drops to
-// read-once + write-once = 6 (8) B/element. R loads carry an L2 evict_last policy, A loads / dx stores evict_first.
+// A(n) = dx of sample n): when A(n) re-reads x, dy of sample n they were streamed at most one sample ago and (for layers
+// whose x + dy of one sample fit VQB_GNP_MB, default 20 MB: two samples within the H100's 50 MB L2) are still L2 resident
+// — HBM traffic drops to read-once + write-once = 6 (8) B/element. R loads carry an L2 evict_last policy, A loads / dx stores evict_first.
 // Sync: R units add their per-channel partials to cs[n] (fp32 atomics) and bump done[n]; A units spin (acquire) until
 // done[n] == units. Every CTA walks the same global order and only ever waits on work that precedes its own position in
 // every CTA's list, and the grid is sized to be fully co-resident, so the wait cannot deadlock.
@@ -904,7 +904,7 @@ __global__ void wavelet_fwd_kernel(const float* __restrict__ x, __nv_bfloat16* _
 
 static inline int gs_blocks(int64_t total, int threads) {
     int64_t b = (total + threads - 1) / threads;
-    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 148) * 16;
+    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (b > cap) b = cap;
     if (b < 1) b = 1;
     return static_cast<int>(b);
@@ -927,7 +927,7 @@ static inline void cv_grid(int HW, int C, int N, Kernel kernel, size_t smem, int
     const int R = T / V > 0 ? T / V : 1;
     int bpsm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bpsm, kernel, T, smem) != cudaSuccess || bpsm < 1) bpsm = 4;
-    const int concurrent = (num_sms() > 0 ? num_sms() : 148) * bpsm;
+    const int concurrent = (num_sms() > 0 ? num_sms() : 132) * bpsm;
     const int min_ppc = R * 4;
     int best_chunks = 1;
     for (int waves = 1; waves <= 8; ++waves) {
@@ -1089,17 +1089,16 @@ static int gn_silu_bwd_impl(const void* x, const void* dy, const void* add, void
     float* gsum = ws;
     // Persistent L2-pipelined form (reduce + apply in one launch, x / dy read from HBM once): used when one sample's
     // x + dy (+ add) comfortably fits the L2 next to the following sample's, and there is enough work to pipeline.
-    // VQB_GN_BWD_PERSISTENT=1 opts into the persistent form. Measured (tools/gn_bwd_bench.py, N=32, profiles/
-    // r02_gn_bwd_variants.txt): 1.5-2x SLOWER than the two-kernel form on every shape (e.g. 128 ch @ 256^2: 1010 us vs
-    // 682 us) — two 128-register CTAs per SM keep too few loads in flight and every unit pays barrier + fence + atomics —
-    // so the default stays the two-kernel form.
+    // VQB_GN_BWD_PERSISTENT=1 opts into the persistent form; it has not been measured on the H100 (tools/gn_bwd_bench.py
+    // compares the two), so the default stays the two-kernel form: two 128-register CTAs per SM keep fewer loads in
+    // flight, and every unit pays barrier + fence + atomics.
     static const int gnp_mode = [] {
         const char* e = getenv("VQB_GN_BWD_PERSISTENT");
         return e ? atoi(e) : 0;
     }();
     static const int gnp_depth = [] { const char* e = getenv("VQB_GNP_DEPTH"); return e ? atoi(e) : 1; }();
     static const int gnp_hints = [] { const char* e = getenv("VQB_GNP_HINTS"); return e ? atoi(e) : 1; }();
-    static const int gnp_mb = [] { const char* e = getenv("VQB_GNP_MB"); return e ? atoi(e) : 36; }();
+    static const int gnp_mb = [] { const char* e = getenv("VQB_GNP_MB"); return e ? atoi(e) : 20; }();
     const int64_t sample_bytes = static_cast<int64_t>(HW) * C * 2 * (add ? 3 : 2);
     if (!cs_pre && gnp_mode && T <= 256 && T % (C / 8) == 0 && sample_bytes <= (static_cast<int64_t>(gnp_mb) << 20) &&
         static_cast<int64_t>(N) * HW * C >= (1 << 18)) {
@@ -1114,7 +1113,7 @@ static int gn_silu_bwd_impl(const void* x, const void* dy, const void* add, void
             if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bpsm, kern, T, smem) != cudaSuccess || bpsm < 1)
                 return set_error(VQB_ECUDA, "vqb_gn_silu_bwd: occupancy query failed");
             if (bpsm > 2) bpsm = 2;
-            const int grid = (num_sms() > 0 ? num_sms() : 148) * bpsm;
+            const int grid = (num_sms() > 0 ? num_sms() : 132) * bpsm;
             // sample groups of S samples whose x + dy (+ add) fit the L2 budget; each group is cut into ~grid units
             int S = static_cast<int>((static_cast<int64_t>(gnp_mb) << 20) / sample_bytes);
             if (S < 1) S = 1;
@@ -1236,7 +1235,7 @@ int vqb_colsum(const void* x, float* out, int64_t P, int C, void* stream) {
     int bpsm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bpsm, colsum_kernel, T, C * sizeof(float)) != cudaSuccess || bpsm < 1)
         bpsm = 4;
-    const int64_t concurrent = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 148) * bpsm;
+    const int64_t concurrent = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * bpsm;
     int64_t nblk = concurrent;
     while (nblk < concurrent * 8 && (P + nblk - 1) / nblk > 2048) nblk += concurrent;
     int64_t ppc = (P + nblk - 1) / nblk;

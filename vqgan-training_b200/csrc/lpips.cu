@@ -275,7 +275,7 @@ __global__ void lpips_tail_bwd_kernel(const __nv_bfloat16* __restrict__ f0, cons
 
 static inline int gs_blocks2(int64_t total, int threads) {
     int64_t b = (total + threads - 1) / threads;
-    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 148) * 16;
+    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (b > cap) b = cap;
     if (b < 1) b = 1;
     return static_cast<int>(b);
@@ -317,7 +317,7 @@ static int lpips_tail_fwd_impl(const void* f0, const void* f1, const float* w, f
     VQB_CHECK(C % 64 == 0 && C <= 512 && ((C / 8) <= 32 || (C / 8) % 32 == 0), "vqb_lpips_tail_fwd: C=%d unsupported", C);
     const int V = C / 8, G = V < 32 ? V : 32, VPL = V / G;
     VQB_CHECK((G & (G - 1)) == 0, "vqb_lpips_tail_fwd: C/8 must be a power of two");
-    int ppb = (HW + 148 * 4 - 1) / (148 * 4);
+    int ppb = (HW + 132 * 4 - 1) / (132 * 4);
     const int per_pass = 8 * (32 / G);
     if (ppb < per_pass * 2) ppb = per_pass * 2;
     dim3 grid((HW + ppb - 1) / ppb, N);
@@ -362,7 +362,7 @@ static int lpips_tail_bwd_impl(const void* f0, const void* f1, const float* w, c
     VQB_CHECK(C % 64 == 0 && C <= 512, "vqb_lpips_tail_bwd: C=%d unsupported", C);
     const int V = C / 8, G = V < 32 ? V : 32, VPL = V / G;
     VQB_CHECK((G & (G - 1)) == 0, "vqb_lpips_tail_bwd: C/8 must be a power of two");
-    int ppb = (HW + 148 * 4 - 1) / (148 * 4);
+    int ppb = (HW + 132 * 4 - 1) / (132 * 4);
     const int per_pass = 8 * (32 / G);
     if (ppb < per_pass * 2) ppb = per_pass * 2;
     dim3 grid((HW + ppb - 1) / ppb, N);

@@ -79,8 +79,8 @@ static_assert(sizeof(PackJob) == sizeof(VqbPackJob), "PackJob must mirror VqbPac
 
 // One block = an (8 rows) x (64 k) tile of one job, all slots: the OIHW source is read in contiguous runs (64*T floats per
 // row for the forward layout, 8*T floats per k for the transposed one) into shared memory, then every slot's 64
-// consecutive bf16 (128 B) are written coalesced. (The first version read with a stride of T floats: 1.14 ms per step
-// for 0.65 GB of weights; this form is HBM/L2 streaming.)
+// consecutive bf16 (128 B) are written coalesced, so the re-pack streams HBM / L2 instead of reading with a stride of T
+// floats.
 constexpr int kPackRows = 8, kPackK = 64, kPackMaxT = 16;
 
 __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackJob* __restrict__ jobs, int njobs) {
@@ -169,7 +169,7 @@ int vqb_adamw_flat(float* params, const float* grads, float* exp_avg, float* exp
         h.bc2_sqrt[i] = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(s.beta2), static_cast<double>(s.step))));
     }
     int64_t blocks = nchunks;
-    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 148) * 16;
+    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (blocks > cap) blocks = cap;
     adamw_flat_kernel<<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         params, grads, exp_avg, exp_avg_sq, chunk_group, nchunks, h, nullptr, grad_scale);
@@ -204,7 +204,7 @@ int vqb_adamw_flat_dev(float* params, const float* grads, float* exp_avg, float*
               "vqb_adamw_flat_dev: buffers must be 16-byte aligned");
     if (nchunks <= 0) return VQB_OK;
     int64_t blocks = nchunks;
-    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 148) * 16;
+    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (blocks > cap) blocks = cap;
     AdamwGroups dummy = {};
     adamw_flat_kernel<<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(

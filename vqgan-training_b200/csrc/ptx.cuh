@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), fences.
+// Thin inline-PTX wrappers for the sm_90a features the hot path uses:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared memory), fences.
 // Everything here is device-only and header-only; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cstdint>
@@ -12,12 +12,6 @@ namespace vqb {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ uint32_t lane_id() {
-    uint32_t l;
-    asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
-    return l;
 }
 
 // Returns 1 in exactly one (elected) lane of a fully converged warp.
@@ -82,27 +76,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const uint64_t t0 = globaltimer_ns();
     while (!mbar_try_wait(bar, parity)) {
-        if (globaltimer_ns() - t0 > 4000000000ull) {  // 4 s: a dead pipeline, not a slow one
-            printf("vqb: mbarrier watchdog block=%d thread=%d bar=%u parity=%u\n", (int)blockIdx.x,
-                   (int)threadIdx.x, smem_u32(bar), parity);
-            __trap();
-        }
+        // 4 s: a dead pipeline, not a slow one. (No printf, not even in the producer's waits only: any call inside
+        // the kernel makes ptxas serialize every wgmma of the consumer warpgroups, warning C7510.)
+        if (globaltimer_ns() - t0 > 4000000000ull) __trap();
     }
 #else
     while (!mbar_try_wait(bar, parity)) {
     }
 #endif
-}
-
-// ---------------------------------------------------------------- fences
-__device__ __forceinline__ void fence_proxy_async_smem() {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -130,208 +111,129 @@ __device__ __forceinline__ void tma_load_4d(const void* desc, uint64_t* bar, voi
         : "memory");
 }
 
-__device__ __forceinline__ void tma_load_5d(const void* desc, uint64_t* bar, void* smem, int32_t c0, int32_t c1,
-                                            int32_t c2, int32_t c3, int32_t c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        :
-        : "r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-          "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-
-// smem tile -> global tensor (bulk async group); out-of-range parts of the box are clipped by the TMA unit
-__device__ __forceinline__ void tma_store_4d(const void* desc, const void* smem, int32_t c0, int32_t c1, int32_t c2,
-                                             int32_t c3) {
-    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                 :
-                 : "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() {  // at most N groups still reading their smem source
-    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// ---------------------------------------------------------------- wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {  // at most N committed groups of this warpgroup still in flight
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2) and clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `smem_addr` (a shared::cta address of this CTA's layout) inside CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads of a CTA pair: data lands in THIS CTA's shared memory, completion bytes are signalled on an mbarrier that
-// may live in the peer CTA (the pair's leader collects both halves on one barrier).
-__device__ __forceinline__ void tma_load_2d_pair(const void* desc, uint32_t mbar_cluster_addr, void* smem, int32_t c0,
-                                                 int32_t c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4}], [%2];"
-        :
-        : "r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(mbar_cluster_addr), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(const void* desc, uint32_t mbar_cluster_addr, void* smem, int32_t c0,
-                                                 int32_t c1, int32_t c2, int32_t c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        :
-        : "r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(mbar_cluster_addr), "r"(c0), "r"(c1), "r"(c2),
-          "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// M = 256 MMA across the pair (128 rows per CTA, B split N/2 per CTA). Issued by ONE thread of the leader CTA.
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n"
-        :
-        : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in every CTA of `cta_mask` once the pair's MMAs retire
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(cta_mask)
-        : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate. Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n"
-        :
-        : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Same, with the two 64-bit shared-memory descriptors passed as (low word, high word) pairs: the issue loop then does
-// its per-MMA address arithmetic with single 32-bit adds on the low words (the 14-bit address field cannot overflow into
-// the LBO field for shared-memory addresses < 256 KB) while the high words stay loop constants.
-__device__ __forceinline__ void umma_bf16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                               uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        ".reg .b64 da, db;\n"
-        "setp.ne.b32 p, %6, 0;\n"
-        "mov.b64 da, {%1, %2};\n"
-        "mov.b64 db, {%3, %4};\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n"
-        "}\n"
-        :
-        : "r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread (thread i <-> lane base+i).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-        " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-        " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (tcgen05). Fields (bit ranges):
+// Shared-memory matrix descriptor (wgmma, 128B swizzle). Fields (bit ranges):
 //   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4
-//   [32,46) stride byte offset >> 4 [46,48) version = 1 (sm_100)
-//   [49,52) base offset = 0         [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout) {
+//   [32,46) stride byte offset >> 4 [49,52) base offset = 0   [62,64) layout: 1 = 128B swizzle
+// K-major operands: SBO = 1024 (8 rows of 128 B), LBO unused. MN-major operands: SBO = 1024 (8 K-rows of 128 B),
+// LBO = distance between consecutive 64-element MN atoms.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= 1ull << 46;
-    d |= static_cast<uint64_t>(layout & 7u) << 61;
+    d |= 1ull << 62;
     return d;
 }
 
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt (1 = bf16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn, uint32_t b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn << 15) | (b_mn << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands in shared memory, fp32 accumulators in registers, issued by all
+// 128 threads of a warpgroup. TA / TB = 1: the operand is MN-major (transposed) instead of K-major. scale_d = 0
+// overwrites D. Accumulator fragment of thread t (warp w = t / 32, lane l): d[4j + 2i + e] is row 16w + l/4 + 8i,
+// column 8j + 2(l%4) + e.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %10, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, %8, %9, p, 1, 1, %11, %12;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, %16, %17, p, 1, 1, %19, %20;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, %35, %36;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, %67, %68;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+
+// Keeps the compiler from moving reads or writes of the accumulators across this point (wgmma updates them
+// asynchronously; the registers may only be touched once the group that writes them has been waited for).
+template <int N>
+__device__ __forceinline__ void fence_operands(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+    if constexpr (N == 16) wgmma_m64n16<TA, TB>(d, da, db, scale_d);
+    else if constexpr (N == 32) wgmma_m64n32<TA, TB>(d, da, db, scale_d);
+    else if constexpr (N == 64) wgmma_m64n64<TA, TB>(d, da, db, scale_d);
+    else {
+        static_assert(N == 128, "wgmma_bf16: N must be 16, 32, 64 or 128");
+        wgmma_m64n128<TA, TB>(d, da, db, scale_d);
+    }
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {

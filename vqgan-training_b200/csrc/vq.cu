@@ -112,7 +112,7 @@ int vqb_vq_argmin(const float* z, const float* e, long long* idx, float* zq, flo
         attr_set = 200 * 1024;
     }
     int blocks = (M + kVqRowsPerBlock - 1) / kVqRowsPerBlock;
-    const int cap = (num_sms() > 0 ? num_sms() : 148) * 2;
+    const int cap = (num_sms() > 0 ? num_sms() : 132) * 2;
     if (blocks > cap) blocks = cap;
     vq_argmin_kernel<<<blocks, 256, smem, static_cast<cudaStream_t>(stream)>>>(z, e, idx, zq, sqerr, M, K, D, kVqChunk);
     VQB_CUDA(cudaGetLastError());

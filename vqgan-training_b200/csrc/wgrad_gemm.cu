@@ -1,15 +1,14 @@
-// Convolution weight gradient on tcgen05 tensor cores.
+// Convolution weight gradient on Hopper wgmma tensor cores.
 //
 //   dWp[co][t*C64 + c] = sum_{n,h,w} dy[n,h,w,co] * X_view(t)[n, h+dh_t, w+dw_t, c]
 //
-// GEMM view: M = Cout (tiles of 128), N = ntaps*C64 flattened (tap, channel) columns in tiles of
-// BLOCK_N (a whole number of 64-channel atoms), K = output pixels walked in boxes of 64 pixels.
-// Both operands are "MN-major": dy[pixel][co] and x[pixel][c] have the GEMM M/N index contiguous
-// and K (the pixel) strided, which tcgen05 consumes directly from 128B-swizzled [64 px][64 ch]
-// atoms (no transposes, no im2col buffer). The tap shift is a coordinate offset of the TMA box and
-// conv padding is TMA zero fill. K is split across CTAs (ksplit); each split writes its fp32
-// partial tile with plain vector stores, vqb_wgrad_reduce sums the splits deterministically and
-// emits the OIHW fp32 gradient the optimizer sees.
+// GEMM view: M = Cout (tiles of 128, two consumer warpgroups of 64 rows), N = ntaps*C64 flattened (tap, channel)
+// columns in tiles of BLOCK_N (a whole number of 64-channel atoms), K = output pixels walked in boxes of 64 pixels.
+// Both operands are "MN-major": dy[pixel][co] and x[pixel][c] have the GEMM M/N index contiguous and K (the pixel)
+// strided, which wgmma consumes directly (transposed operands) from 128B-swizzled [64 px][64 ch] atoms (no transposes,
+// no im2col buffer). The tap shift is a coordinate offset of the TMA box and conv padding is TMA zero fill. K is split
+// across CTAs (ksplit); each split writes its fp32 partial tile with plain vector stores, vqb_wgrad_reduce sums the
+// splits deterministically and emits the OIHW fp32 gradient the optimizer sees.
 //
 // Replaces the wgrad half of aten::convolution_backward for the trainable convs of ae.py and the
 // PatchDiscriminator (reference call sites listed in include/vqb200.h).
@@ -18,9 +17,11 @@
 
 namespace vqb {
 
-constexpr int kWM = 128;              // Cout rows per tile
-constexpr int kWThreads = 256;
+constexpr int kWM = 128;       // Cout rows per tile
+constexpr int kWThreads = 384;  // warpgroup 0: TMA producer; warpgroups 1, 2: 64 Cout rows each
 constexpr int kWMaxStages = 8;
+constexpr int kWPix = 64;                     // pixels per K block
+constexpr uint32_t kAtomBytes = kWPix * 128;  // [64 px][64 ch] bf16
 
 struct alignas(64) WgradParams {
     CUtensorMap ymap;
@@ -30,54 +31,37 @@ struct alignas(64) WgradParams {
     int32_t tap_dh[VQB_MAX_TAPS];
     int32_t ntaps, C, C64, Cout;
     int32_t lbw, lbh, lbn;
-    int32_t tiles_w, tiles_h, tiles_nb, pixel_boxes;
-    int32_t m_tiles, n_tiles, ksplit, total_units;
-    int32_t block_n, natoms, stages, tmem_cols;
-    int32_t dbg, kpix, use5d, apl, mtiles;  // mtiles: 128-row Cout sub-tiles per unit (2 = 256x256 tiles, 5-D maps only)  // kpix: pixels per K block (64|128); use5d: one TMA per operand; apl: atoms per B load
-    int64_t ld;  // ntaps*C64: row stride of the partial buffer
+    int32_t tiles_w, tiles_h, pixel_boxes;
+    int32_t n_tiles, ksplit, total_units;
+    int32_t stages;
+    int64_t ld;  // row stride of the partial buffer
     float* partial;
 };
 
+template <int BN>
 __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t lane = threadIdx.x & 31;
+    constexpr int kAtoms = BN / 64;
+    constexpr uint32_t kABytes = 2 * kAtomBytes;
+    constexpr uint32_t kStageBytes = kABytes + kAtoms * kAtomBytes;
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t stages = p.stages;
-    const uint32_t atom_bytes = static_cast<uint32_t>(p.kpix) * 128u;  // [kpix px][64 ch] bf16
-    const uint32_t a_bytes = 2 * static_cast<uint32_t>(p.mtiles) * atom_bytes;
-    const uint32_t b_bytes = static_cast<uint32_t>(p.natoms) * atom_bytes;
-    uint8_t* sA = base;
-    uint8_t* sB = base + stages * a_bytes;
-    uint64_t* full = reinterpret_cast<uint64_t*>(sB + stages * b_bytes);
+    uint64_t* full = reinterpret_cast<uint64_t*>(base + stages * kStageBytes);
     uint64_t* empty = full + stages;
-    uint64_t* tfull = empty + stages;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+    const uint32_t wg = threadIdx.x >> 7;
+    const uint32_t warp = (threadIdx.x >> 5) & 3u;
+    const uint32_t lane = threadIdx.x & 31u;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.ymap);
         tma_prefetch_desc(&p.xmap[0]);
-    }
-    if (warp == 1 && lane == 0) {
         for (uint32_t i = 0; i < stages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull[i], 1);
-            mbar_init(&tempty[i], 128);
+            mbar_init(&empty[i], 8);  // lane 0 of every consumer warp releases the stage
         }
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, p.tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     // unit -> (m_tile, n_tile, split); splits of one tile are adjacent so they share L2-resident x/dy
     auto unit_range = [&](int unit, int& m_tile, int& n_tile, int& s, int& kb0, int& kb1) {
@@ -89,185 +73,115 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
         kb1 = static_cast<int>((static_cast<int64_t>(p.pixel_boxes) * (s + 1)) / p.ksplit);
     };
 
-    // single-thread roles are entered through elect.sync so that ptxas emits the TMA / tcgen05 instructions from uniform
-    // registers without per-instruction ELECT loops (see conv_gemm.cu)
-    if (warp == 0) {
-      if (elect_one()) {
-        // ===================== TMA producer =====================
-        uint32_t stage = 0, phase = 0;
-        for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x) {
-            int m_tile, n_tile, s, kb0, kb1;
-            unit_range(unit, m_tile, n_tile, s, kb0, kb1);
-            const int co0 = m_tile * kWM * p.mtiles;
-            const int colbase = n_tile * p.block_n;
-            const int nkb = kb1 - kb0;
-            // no rotation by default: CTAs working on the same pixel split stream the same x / dy boxes in lock-step, so each
-            // box is fetched from HBM once and hit in L2 by the other tiles (a per-CTA rotated start destroys that reuse)
-            const int rot = (nkb > 0 && (p.dbg & 4)) ? static_cast<int>((blockIdx.x * 37u) % static_cast<uint32_t>(nkb)) : 0;
-            for (int kbi = 0; kbi < nkb; ++kbi) {
-                int kb = kb0 + kbi + rot;
-                if (kb >= kb1) kb -= nkb;
-                const int tw = kb % p.tiles_w;
-                const int th = (kb / p.tiles_w) % p.tiles_h;
-                const int tn = kb / (p.tiles_w * p.tiles_h);
-                const int w0 = tw << p.lbw, h0 = th << p.lbh, n0 = tn << p.lbn;
-                mbar_wait(&empty[stage], phase ^ 1);
-                if ((p.dbg & 3) == 1) {  // experiment: MMA throughput without any TMA traffic
-                    mbar_arrive(&full[stage]);
+    if (wg == 0) {
+        // ===================== TMA producer (one elected thread) =====================
+        if (warp == 0 && elect_one()) {
+            uint32_t stage = 0, phase = 0;
+            for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x) {
+                int m_tile, n_tile, s, kb0, kb1;
+                unit_range(unit, m_tile, n_tile, s, kb0, kb1);
+                const int co0 = m_tile * kWM;
+                const int colbase = n_tile * BN;
+                // CTAs working on the same pixel split stream the same x / dy boxes in lock-step, so each box is
+                // fetched from HBM once and hit in L2 by the other tiles
+                for (int kb = kb0; kb < kb1; ++kb) {
+                    const int tw = kb % p.tiles_w;
+                    const int th = (kb / p.tiles_w) % p.tiles_h;
+                    const int tn = kb / (p.tiles_w * p.tiles_h);
+                    const int w0 = tw << p.lbw, h0 = th << p.lbh, n0 = tn << p.lbn;
+                    mbar_wait(&empty[stage], phase ^ 1);
+                    mbar_arrive_expect_tx(&full[stage], kStageBytes);
+                    uint8_t* a = base + stage * kStageBytes;
+                    uint8_t* b = a + kABytes;
+                    tma_load_4d(&p.ymap, &full[stage], a, co0, w0, h0, n0);
+                    tma_load_4d(&p.ymap, &full[stage], a + kAtomBytes, co0 + 64, w0, h0, n0);
+#pragma unroll
+                    for (int j = 0; j < kAtoms; ++j) {
+                        const int col = colbase + 64 * j;
+                        const int t = col / p.C64;
+                        const int c0 = col - t * p.C64;
+                        tma_load_4d(&p.xmap[p.tap_view[t]], &full[stage], b + j * kAtomBytes, c0, w0 + p.tap_dw[t],
+                                    h0 + p.tap_dh[t], n0);
+                    }
                     if (++stage == stages) {
                         stage = 0;
                         phase ^= 1;
                     }
-                    continue;
-                }
-                mbar_arrive_expect_tx(&full[stage], a_bytes + b_bytes);
-                uint8_t* a = sA + stage * a_bytes;
-                uint8_t* b = sB + stage * b_bytes;
-                if (p.use5d) {
-                    // 5-D maps (c_lo, w, h, n, c_hi): one request brings several 64-channel atoms, atom-major in smem
-                    tma_load_5d(&p.ymap, &full[stage], a, 0, w0, h0, n0, co0 >> 6);
-                    for (int j = 0; j < p.natoms; j += p.apl) {
-                        const int col = colbase + 64 * j;
-                        const int t = col / p.C64;
-                        const int c0 = col - t * p.C64;
-                        tma_load_5d(&p.xmap[p.tap_view[t]], &full[stage], b + j * atom_bytes, 0, w0 + p.tap_dw[t],
-                                    h0 + p.tap_dh[t], n0, c0 >> 6);
-                    }
-                } else {
-                    tma_load_4d(&p.ymap, &full[stage], a, co0, w0, h0, n0);
-                    tma_load_4d(&p.ymap, &full[stage], a + atom_bytes, co0 + 64, w0, h0, n0);
-                    for (int j = 0; j < p.natoms; ++j) {
-                        const int col = colbase + 64 * j;
-                        const int t = col / p.C64;
-                        const int c0 = col - t * p.C64;
-                        tma_load_4d(&p.xmap[p.tap_view[t]], &full[stage], b + j * atom_bytes, c0, w0 + p.tap_dw[t],
-                                    h0 + p.tap_dh[t], n0);
-                    }
-                }
-                if (++stage == stages) {
-                    stage = 0;
-                    phase ^= 1;
                 }
             }
         }
-      }
-    } else if (warp == 1) {
-      if (elect_one()) {
-        // ===================== MMA issuer (lean: descriptors are base + increments) =====================
-        const uint32_t idesc = make_idesc_bf16(kWM, p.block_n, 1, 1);  // both operands MN-major
-        // MN-major, 128B swizzle: SBO = 8 K-rows (1024 B), LBO = next 64-wide MN atom (atom_bytes)
-        const uint64_t da_base = make_smem_desc(smem_u32(sA), atom_bytes, 1024, 2);
-        const uint64_t db_base = make_smem_desc(smem_u32(sB), atom_bytes, 1024, 2);
-        const uint32_t a_step = a_bytes >> 4, b_step = b_bytes >> 4;
-        const int ksteps = p.kpix >> 4;
-        const bool do_mma = (p.dbg & 3) != 2;
-        uint32_t stage = 0, phase = 0, it = 0, a_off = 0, b_off = 0;
-        for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x, ++it) {
-            int m_tile, n_tile, s, kb0, kb1;
-            unit_range(unit, m_tile, n_tile, s, kb0, kb1);
-            // mtiles == 1: double-buffered accumulators (as = it & 1); mtiles == 2: both buffers belong to this unit
-            const bool two = (p.mtiles == 2);
-            const uint32_t as = two ? 0u : (it & 1), aph = two ? (it & 1) : ((it >> 1) & 1);
-            mbar_wait(&tempty[as], aph ^ 1);
-            if (two) mbar_wait(&tempty[1], aph ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + as * p.block_n;
-            const uint32_t d_tmem1 = tmem_base + p.block_n;
-            const uint32_t mt_step = (2 * atom_bytes) >> 4;
-            uint32_t acc = 0;
-            for (int kb = kb0; kb < kb1; ++kb) {
-                mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint64_t da = da_base + a_off, db = db_base + b_off;
-                if (do_mma) {
-                    if (ksteps == 8) {
-#pragma unroll
-                        for (int k = 0; k < 8; ++k) umma_bf16(d_tmem, da + 128 * k, db + 128 * k, idesc, acc | k);
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, da + 128 * k, db + 128 * k, idesc, acc | k);
-                        if (two) {
-#pragma unroll
-                            for (int k = 0; k < 4; ++k)
-                                umma_bf16(d_tmem1, da + mt_step + 128 * k, db + 128 * k, idesc, acc | k);
-                        }
-                    }
-                }
-                umma_commit(&empty[stage]);
-                acc = 1;
-                if (++stage == stages) {
-                    stage = 0;
-                    phase ^= 1;
-                    a_off = 0;
-                    b_off = 0;
-                } else {
-                    a_off += a_step;
-                    b_off += b_step;
-                }
-            }
-            if (two) umma_commit(&tfull[1]);
-            umma_commit(&tfull[as]);
-        }
-      }
-    } else if (warp >= 4) {
-        // ===================== epilogue: fp32 partial tile -> global =====================
-        const uint32_t ew = warp - 4;
-        uint32_t it = 0;
-        for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x, ++it) {
-            int m_tile, n_tile, s, kb0, kb1;
-            unit_range(unit, m_tile, n_tile, s, kb0, kb1);
-          for (int mt = 0; mt < p.mtiles; ++mt) {
-            const bool two = (p.mtiles == 2);
-            const uint32_t as = two ? static_cast<uint32_t>(mt) : (it & 1), aph = two ? (it & 1) : ((it >> 1) & 1);
-            const int co = (m_tile * p.mtiles + mt) * kWM + ew * 32 + lane;
-            const bool valid = co < p.Cout;
-            float* orow = p.partial + (static_cast<int64_t>(s) * p.Cout + co) * p.ld + n_tile * p.block_n;
-            mbar_wait(&tfull[as], aph);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((ew * 32u) << 16) + as * p.block_n;
-            const bool empty_range = (kb1 <= kb0);  // more splits than pixel boxes: contributes zeros
-            for (int c0 = 0; c0 < p.block_n; c0 += 16) {
-                uint32_t v[16];
-                tmem_ld16(taddr + c0, v);
-                tmem_ld_wait();
-                if (valid) {
-                    float4* o = reinterpret_cast<float4*>(orow + c0);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float4 f;
-                        f.x = empty_range ? 0.f : __uint_as_float(v[4 * j]);
-                        f.y = empty_range ? 0.f : __uint_as_float(v[4 * j + 1]);
-                        f.z = empty_range ? 0.f : __uint_as_float(v[4 * j + 2]);
-                        f.w = empty_range ? 0.f : __uint_as_float(v[4 * j + 3]);
-                        o[j] = f;
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tempty[as]);
-          }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, p.tmem_cols);
+    // ===================== consumers: warpgroup cw owns Cout rows 64*cw .. 64*cw + 63 of every tile =====================
+    const uint32_t cw = wg - 1;
+    const uint32_t ring = smem_u32(base);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    uint32_t stage = 0, phase = 0;
+    for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x) {
+        int m_tile, n_tile, s, kb0, kb1;
+        unit_range(unit, m_tile, n_tile, s, kb0, kb1);
+        uint32_t prev = 0;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const uint32_t a = ring + stage * kStageBytes;
+            // MN-major, 128B swizzle: SBO = 8 K-rows (1024 B), LBO = next 64-wide MN atom
+            const uint64_t da = make_smem_desc(a + cw * kAtomBytes, kAtomBytes, 1024);
+            const uint64_t db = make_smem_desc(a + kABytes, kAtomBytes, 1024);
+            fence_operands(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kWPix / 16; ++k)  // 16 pixel rows of 128 B per K = 16 step
+                wgmma_bf16<BN, 1, 1>(acc, da + 128 * k, db + 128 * k, (kb > kb0 || k > 0) ? 1u : 0u);
+            wgmma_commit();
+            fence_operands(acc);
+            // keep this K-block's group in flight while the next stage is awaited; the previous one has retired
+            wgmma_wait<1>();
+            if (kb > kb0 && lane == 0) mbar_arrive(&empty[prev]);
+            prev = stage;
+            if (++stage == stages) {
+                stage = 0;
+                phase ^= 1;
+            }
+        }
+        wgmma_wait<0>();
+        fence_operands(acc);  // the epilogue's reads of acc stay below the wait
+        if (kb1 > kb0 && lane == 0) mbar_arrive(&empty[prev]);
+        // ---------------- epilogue: fp32 partial tile -> global
+        const bool empty_range = (kb1 <= kb0);  // more splits than pixel boxes: contributes zeros
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int co = m_tile * kWM + static_cast<int>(cw * 64 + warp * 16 + (lane >> 2)) + 8 * i;
+            if (co >= p.Cout) continue;
+            float* orow = p.partial + (static_cast<int64_t>(s) * p.Cout + co) * p.ld + n_tile * BN + 2 * (lane & 3u);
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const float2 f = empty_range ? make_float2(0.f, 0.f)
+                                             : make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+                *reinterpret_cast<float2*>(orow + 8 * j) = f;
+            }
+        }
     }
 }
 
-static int encode_view(const VqbView& vw, const void* basep, int C, int lbw, int lbh, int lbn, int atoms5d,
-                       CUtensorMap* m) {
-    const void* base = static_cast<const uint8_t*>(basep) + vw.offset * 2;
-    if (atoms5d > 0) {
-        uint64_t dims[5] = {64, static_cast<uint64_t>(vw.Wv), static_cast<uint64_t>(vw.Hv),
-                            static_cast<uint64_t>(vw.Nv), static_cast<uint64_t>(C / 64)};
-        uint64_t str[4] = {static_cast<uint64_t>(vw.sw) * 2, static_cast<uint64_t>(vw.sh) * 2,
-                           static_cast<uint64_t>(vw.sn) * 2, 128};
-        uint32_t box[5] = {64, 1u << lbw, 1u << lbh, 1u << lbn, static_cast<uint32_t>(atoms5d)};
-        return encode_tmap_bf16(m, base, 5, dims, str, box, 128);
+template <int BN>
+static int launch_wgrad(const WgradParams& p, void* stream) {
+    const size_t smem = 1024 + static_cast<size_t>(p.stages) * (2 + BN / 64) * kAtomBytes + 16 * p.stages;
+    static bool attr_set = false;
+    if (!attr_set) {
+        VQB_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        attr_set = true;
     }
+    const int grid = p.total_units < num_sms() ? p.total_units : num_sms();
+    wgrad_gemm_kernel<BN><<<grid, kWThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
+    VQB_CUDA(cudaGetLastError());
+    return VQB_OK;
+}
+
+static int encode_view(const VqbView& vw, const void* basep, int C, int lbw, int lbh, int lbn, CUtensorMap* m) {
+    const void* base = static_cast<const uint8_t*>(basep) + vw.offset * 2;
     uint64_t dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(vw.Wv), static_cast<uint64_t>(vw.Hv),
                         static_cast<uint64_t>(vw.Nv)};
     uint64_t str[3] = {static_cast<uint64_t>(vw.sw) * 2, static_cast<uint64_t>(vw.sh) * 2,
@@ -290,16 +204,12 @@ extern "C" int vqb_wgrad_gemm(const VqbWgradDesc* d, const void* dy, const void*
               "vqb_wgrad_gemm: ntaps/nviews out of range");
     VQB_CHECK(d->ksplit >= 1, "vqb_wgrad_gemm: ksplit must be >= 1");
     VQB_CHECK((reinterpret_cast<uintptr_t>(partial) & 15u) == 0, "vqb_wgrad_gemm: partial not 16-byte aligned");
-    if (!device_is_sm100()) return set_error(VQB_ENODEVICE, "vqb_wgrad_gemm: current device is not sm_100");
+    VQB_CHECK(d->col_offset % 2 == 0 && d->ld_override % 2 == 0,
+              "vqb_wgrad_gemm: col_offset / ld_override must be even (8-byte partial stores)");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_wgrad_gemm: current device is not sm_90");
 
     WgradParams p;
-    p.dbg = debug_mode();
-    const bool can5d = (!(p.dbg & 16) && d->C % 64 == 0 && d->Cout % 64 == 0);
-    // 256(Cout) x BLOCK_N tiles with two accumulators when Cout >= 256: each x tile is shared by two dy sub-tiles
-    // (less L2->SM traffic per FLOP); needs the 5-D maps and 64-pixel K blocks to fit three smem stages
-    p.mtiles = (can5d && d->Cout >= 256 && !(p.dbg & 64)) ? 2 : 1;
-    p.kpix = ((p.dbg & 8) || p.mtiles == 2) ? 64 : 128;  // 128-pixel K blocks: fewer, larger TMA requests
-    const uint32_t kp = static_cast<uint32_t>(p.kpix);
+    const uint32_t kp = kWPix;
     uint32_t bw = next_pow2(d->W);
     if (bw > kp) bw = kp;
     uint32_t bh = next_pow2(d->H);
@@ -310,69 +220,38 @@ extern "C" int vqb_wgrad_gemm(const VqbWgradDesc* d, const void* dy, const void*
     p.lbn = ilog2(bn);
     p.tiles_w = (d->W + bw - 1) / bw;
     p.tiles_h = (d->H + bh - 1) / bh;
-    p.tiles_nb = (d->N + bn - 1) / bn;
-    p.pixel_boxes = p.tiles_w * p.tiles_h * p.tiles_nb;
+    p.pixel_boxes = p.tiles_w * p.tiles_h * ((d->N + bn - 1) / bn);
     p.ntaps = d->ntaps;
     p.C = d->C;
     p.C64 = ((d->C + 63) / 64) * 64;
     p.Cout = d->Cout;
-    const int cols = d->ntaps * p.C64;
-    int block_n = 64;
-    const int cands[4] = {256, 192, 128, 64};
-    for (int i = 0; i < 4; ++i)
-        if (cols % cands[i] == 0) {
-            block_n = cands[i];
-            break;
-        }
-    p.block_n = block_n;
-    p.natoms = block_n / 64;
-    p.m_tiles = (d->Cout + kWM * p.mtiles - 1) / (kWM * p.mtiles);
+    const int cols = vqb_wgrad_cols(d->ntaps, d->C);
+    const int block_n = (cols % 128 == 0) ? 128 : 64;  // 64 fp32 accumulator registers per thread at most
+    const int m_tiles = (d->Cout + kWM - 1) / kWM;
     p.n_tiles = cols / block_n;
     p.ksplit = d->ksplit;
-    p.total_units = p.m_tiles * p.n_tiles * p.ksplit;
+    p.total_units = m_tiles * p.n_tiles * p.ksplit;
     // ld_override / col_offset: several launches may fill column ranges of one partial buffer (folded upsample conv)
     p.ld = d->ld_override > 0 ? d->ld_override : cols;
     p.partial = partial + d->col_offset;
-    // 5-D (c_lo, w, h, n, c_hi) tensor maps: one TMA request per operand instead of one per 64-channel atom
-    p.use5d = can5d ? 1 : 0;
-    p.apl = 1;
-    if (p.use5d) {
-        if (block_n % p.C64 == 0)
-            p.apl = p.C64 / 64;  // the tile covers whole taps: one request per tap
-        else if (p.C64 % block_n == 0)
-            p.apl = p.natoms;    // the tile lies inside one tap: one request
-        else
-            p.apl = 1;
-    }
-    const int atom_bytes = p.kpix * 128;
-    const int stage_bytes = 2 * p.mtiles * atom_bytes + p.natoms * atom_bytes;
+    const int stage_bytes = (2 + block_n / 64) * static_cast<int>(kAtomBytes);
     int stages = (200 * 1024) / stage_bytes;
     if (stages > kWMaxStages) stages = kWMaxStages;
     p.stages = stages;
-    uint32_t tc = next_pow2(2 * block_n);
-    if (tc < 32) tc = 32;
-    p.tmem_cols = tc;
     for (int t = 0; t < d->ntaps; ++t) {
         VQB_CHECK(d->taps[t].view >= 0 && d->taps[t].view < d->nviews, "vqb_wgrad_gemm: tap view out of range");
         p.tap_view[t] = d->taps[t].view;
         p.tap_dw[t] = d->taps[t].dw;
         p.tap_dh[t] = d->taps[t].dh;
     }
-    int rc = encode_view(d->dy_view, dy, d->Cout, p.lbw, p.lbh, p.lbn, p.use5d ? 2 * p.mtiles : 0, &p.ymap);
+    int rc = encode_view(d->dy_view, dy, d->Cout, p.lbw, p.lbh, p.lbn, &p.ymap);
     if (rc != VQB_OK) return rc;
     for (int v = 0; v < d->nviews; ++v) {
-        rc = encode_view(d->views[v], x, d->C, p.lbw, p.lbh, p.lbn, p.use5d ? p.apl : 0, &p.xmap[v]);
+        rc = encode_view(d->views[v], x, d->C, p.lbw, p.lbh, p.lbn, &p.xmap[v]);
         if (rc != VQB_OK) return rc;
     }
-    const size_t smem = 1024 + static_cast<size_t>(stages) * stage_bytes + 256;
-    static bool attr_set = false;
-    if (!attr_set) {
-        VQB_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set = true;
-    }
-    int grid = p.total_units < num_sms() ? p.total_units : num_sms();
-    wgrad_gemm_kernel<<<grid, kWThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
-    VQB_CUDA(cudaGetLastError());
+    rc = block_n == 128 ? launch_wgrad<128>(p, stream) : launch_wgrad<64>(p, stream);
+    if (rc != VQB_OK) return rc;
     count_launch();
     return VQB_OK;
 }

@@ -185,7 +185,7 @@ class FlatAdamW(torch.optim.Optimizer):
     @torch.no_grad()
     def step(self, closure=None):
         if not self.store.params.is_cuda:
-            raise RuntimeError("FlatAdamW.step: the fused optimizer kernel runs on sm_100a only (no CPU fallback)")
+            raise RuntimeError("FlatAdamW.step: the fused optimizer kernel runs on sm_90a only (no CPU fallback)")
         active = self.store.collect()
         if not any(active):
             return None

@@ -2,7 +2,7 @@
 
 This is the only place Python touches the native layer. Tensors are passed as raw device pointers
 (`tensor.data_ptr()`) plus the current CUDA stream; shapes travel in plain C structs. There is no
-fallback: if the shared library is missing or the device is not sm_100 every op raises.
+fallback: if the shared library is missing or the device is not sm_90 (H100) every op raises.
 """
 from __future__ import annotations
 
@@ -12,8 +12,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# VQB_DEBUG_LIB=1 selects the -DVQB_DEBUG build (perf-experiment switches + bring-up kernels; build_native.py --debug)
-_LIB_PATH = os.path.join(_HERE, "libvqb200_dbg.so" if os.environ.get("VQB_DEBUG_LIB", "0") == "1" else "libvqb200.so")
+_LIB_PATH = os.path.join(_HERE, "libvqb200.so")
 
 VQB_MAX_VIEWS = 16
 VQB_MAX_TAPS = 16
@@ -74,7 +73,7 @@ def load():
         return _lib
     if not os.path.exists(_LIB_PATH):
         raise RuntimeError(
-            f"{_LIB_PATH} is missing: run `python vqgan-training_b200/build_native.py` (nvcc, sm_100a). "
+            f"{_LIB_PATH} is missing: run `python vqgan-training_b200/build_native.py` (nvcc, sm_90a). "
             "There is no CPU / PyTorch fallback for the hot path.")
     L = C.CDLL(_LIB_PATH)
     vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
@@ -94,7 +93,6 @@ def load():
         "vqb_nhwc_to_nchw": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, vp]),
         "vqb_gn_silu_fwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, vp]),
         "vqb_gn_silu_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp]),
-        "vqb_dbg_shift_mma": (i32, [vp, i32, vp, vp, i32, i32, i32, vp]),
         "vqb_wavelet_fwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
         "vqb_upsample2x_fwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),
         "vqb_upsample2x_bwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),
@@ -109,7 +107,6 @@ def load():
         "vqb_lpips_dropout_mask": (i32, [C.c_uint64, i32, i32, i32, vp, vp]),
         "vqb_attn_fwd": (i32, [vp, vp, vp, i32, i32, i32, vp]),
         "vqb_attn_bwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]),
-        "vqb_set_debug_mode": (i32, [i32]),
         "vqb_vq_argmin": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, vp]),
         "vqb_nchw_to_nhwc_pad": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
         "vqb_nhwc_to_nchw_pad": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp]),

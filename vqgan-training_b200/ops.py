@@ -1,4 +1,4 @@
-"""torch.autograd.Functions over the native sm_100a kernels (libvqb200.so).
+"""torch.autograd.Functions over the native sm_90a kernels (libvqb200.so).
 
 Internal activation format: contiguous bf16 tensors of shape [N, H, W, Cp] (NHWC, Cp = channels padded to a multiple
 of 8, pad channels zero). Master weights / gradients stay fp32 OIHW nn.Parameters (the reference's state_dict
@@ -29,7 +29,7 @@ def _L():
 
 def require_cuda(t: torch.Tensor):
     if not t.is_cuda:
-        raise RuntimeError("vqgan-training_b200: the hot path runs on sm_100a CUDA tensors only (no CPU fallback)")
+        raise RuntimeError("vqgan-training_b200: the hot path runs on sm_90a CUDA tensors only (no CPU fallback)")
 
 
 def tapmap_tensor(tapmap, device) -> torch.Tensor:
@@ -228,21 +228,27 @@ def grad_out(param: torch.Tensor) -> torch.Tensor:
     return torch.empty(param.shape, device=param.device, dtype=torch.float32)
 
 
+H100_SMS = 132  # H100 SXM; used when no device is visible (host-side planning and tests)
+
+
+def _num_sms() -> int:
+    """SM count of the current device (the kernels size their persistent grids from it), else an H100 SXM's."""
+    if torch.cuda.is_available():
+        return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    return H100_SMS
+
+
 def _wgrad_block_n(cols: int) -> int:
-    for c in (256, 192, 128, 64):
-        if cols % c == 0:
-            return c
-    return 64
+    return 128 if cols % 128 == 0 else 64
 
 
 def choose_ksplit(g: plans.ConvGeom, Cout_pad: int) -> int:
-    """Split-K factor of the weight-gradient GEMM: the split count whose (tile, split) unit count best fills ONE wave of
-    the 148 persistent CTAs (measured: one full wave beats two). Mirrors the tile shape rules of csrc/wgrad_gemm.cu
-    (256-row tiles + 64-pixel K blocks when Cout >= 256, else 128/128)."""
+    """Split-K factor of the weight-gradient GEMM: the split count whose (tile, split) unit count best fills whole waves
+    of the persistent CTAs (one per SM of an H100 SXM), preferring one wave. Mirrors the tile shape rules of
+    csrc/wgrad_gemm.cu (128 Cout rows x 128 or 64 columns, 64-pixel K blocks)."""
     cols = len(g.taps) * ((g.C + 63) // 64) * 64
-    big = Cout_pad >= 256 and g.C % 64 == 0 and Cout_pad % 64 == 0
-    rows = 256 if big else 128
-    kpix = 64 if big else 128
+    rows = 128
+    kpix = 64
     tiles = ((Cout_pad + rows - 1) // rows) * (cols // _wgrad_block_n(cols))
 
     def p2(v, cap):
@@ -255,11 +261,9 @@ def choose_ksplit(g: plans.ConvGeom, Cout_pad: int) -> int:
     bh = p2(g.Ho, kpix // bw)
     bn = kpix // (bw * bh)
     boxes = -(-g.Wo // bw) * -(-g.Ho // bh) * -(-g.N // bn)
-    # pick the split count whose (tile, split) unit count best fills ONE wave of 148 persistent CTAs: every unit pays a
-    # fixed pipeline-fill + fp32-partial-tile epilogue, and the reduction kernel reads ksplit partials, so a single
-    # full wave beats two (measured, tools/gpu_probe.py wgbench: 512->512 @ 32^2 ks=4 1471 vs ks=8 1305 TFLOP/s;
-    # 128->128 @ 256^2 ks=24 1052 vs ks=49 978; 256->256 @ 128^2 ks=16 1598 vs ks=32 1456)
-    sms = 148
+    # every unit pays a fixed pipeline-fill + fp32-partial-tile epilogue, and the reduction kernel reads ksplit partials:
+    # each extra wave and each extra split is penalised
+    sms = _num_sms()
     max_ks = max(1, min(boxes // 4, 128, (256 << 20) // max(1, Cout_pad * cols * 4)))
     best, best_score = 1, -1.0
     for ks in range(1, max_ks + 1):
@@ -285,9 +289,8 @@ class GnLink:
         self.groups, self.silu, self.sums = 0, False, None
 
 
-# Opt-in (VQB_GN_BWD_FUSE=1): measured on the B=32 step, the extra ~1200 instructions per 64-channel group in the four
-# epilogue warps are NOT hidden behind the main loop of the 128-channel layers (conv_gemm total 46.1 -> 64.9 ms for a
-# 5.2 ms saving in gn_bwd_reduce); kept, with its parity test, for layers with long K loops.
+# Opt-in (VQB_GN_BWD_FUSE=1): the extra epilogue work runs on the MMA warpgroups of the conv, and whether the saved
+# GroupNorm reduction pass pays for it has not been measured on the H100; kept, with its parity test.
 _GN_BWD_FUSE = os.environ.get("VQB_GN_BWD_FUSE", "0") == "1"
 _GN_BWD_FUSE_MIN_C = int(os.environ.get("VQB_GN_BWD_FUSE_MIN_C", "0"))
 
@@ -533,7 +536,7 @@ def to_nchw(y, C):
 
 # ----------------------------------------------------------------------------------------------------------------------
 class ConvFn(torch.autograd.Function):
-    """Convolution through the tcgen05 implicit-GEMM kernel.
+    """Convolution through the wgmma implicit-GEMM kernel.
 
     kind: "s1" (k x k stride 1 same), "s2" (Downsample: pad (0,1,0,1) + 3x3 stride 2), "patch" (k x k stride k).
     opts: relu (fused ReLU epilogue; the incoming gradient is then expected to be already gated by out > 0, which every

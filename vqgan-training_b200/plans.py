@@ -1,7 +1,7 @@
 """Geometry descriptors (views + taps) for every convolution variant on the hot path.
 
 A "plan" is a filled VqbConvDesc / VqbWgradDesc plus the tap map used to pack the OIHW fp32 master
-weights into the bf16 [rows][slot][K] matrix the tcgen05 kernels read. Plans depend only on shapes
+weights into the bf16 [rows][slot][K] matrix the wgmma kernels read. Plans depend only on shapes
 and are cached by the modules.
 
 Variants (reference call sites):
@@ -154,8 +154,8 @@ def geom_up_dgrad(N, h, w, Cop) -> ConvGeom:
 # The image lives in a zero-framed buffer [N][H+2][W+2][8]; horizontally adjacent pixels are CONTIGUOUS, so the conv
 # becomes 3 taps (kh) whose K run starts at pixel (w-1) and covers the 8 pixels w-1..w+6 = 64 elements = one full
 # 128-byte K chunk: columns 0..23 carry the three real taps (kw*8 + c), columns 24..63 meet ZERO weights. The run is 64
-# wide (not 24) on purpose: ncu showed the TMA unit spending ~28 cycles per row when the box's inner dimension is
-# partly out of range (24 of 64: 640 us for a layer whose HBM floor is 90 us); a fully in-range 128-byte row costs ~1.
+# wide (not 24) on purpose: a TMA box whose inner dimension is partly out of range is served row by row, a fully in-range
+# 128-byte row in one piece.
 # The buffer carries 64 elements of zeroed slack so the last rows stay inside the allocation.
 FAT_K = 64
 

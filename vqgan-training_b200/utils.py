@@ -1,9 +1,9 @@
-"""B200-native drop-in for the reference `utils.py`: LPIPS, ScalingLayer, NetLinLayer, vgg16, PatchDiscriminator,
+"""H100-native drop-in for the reference `utils.py`: LPIPS, ScalingLayer, NetLinLayer, vgg16, PatchDiscriminator,
 normalize_tensor, spatial_average, and the wavelet front-end — same class names, constructor signatures and
-state_dict keys (utils.py:8-247), with the VGG16 trunks, LPIPS tail and discriminator heads running on the sm_100a
+state_dict keys (utils.py:8-247), with the VGG16 trunks, LPIPS tail and discriminator heads running on the sm_90a
 kernels of libvqb200.so:
 
-  13 VGG conv3x3 + bias + ReLU        -> tcgen05 implicit-GEMM conv with fused bias/ReLU epilogue (csrc/conv_gemm.cu);
+  13 VGG conv3x3 + bias + ReLU        -> wgmma implicit-GEMM conv with fused bias/ReLU epilogue (csrc/conv_gemm.cu);
                                          the data-gradient epilogue applies the ReLU gate of the producing layer
   4 max-pools                         -> csrc/lpips.cu (backward fuses the ReLU gate)
   LPIPS tail (normalise, diff^2, lin, spatial mean, 5-way sum; ~12 ATen kernels per layer in the reference)
@@ -69,7 +69,7 @@ def broadcast_module_state(module: nn.Module, src: int = 0):
 
 
 def _as_b200_conv(layer: nn.Conv2d):
-    """Wraps a torchvision conv's Parameters into a tcgen05-backed StandardizedC2d without consuming RNG."""
+    """Wraps a torchvision conv's Parameters into a wgmma-backed StandardizedC2d without consuming RNG."""
     from ae import StandardizedC2d
 
     with torch.random.fork_rng(devices=[]):

@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference `vae_trainer.py` (the torchrun DDP entry, its CLI flags and the loss/autograd
+"""H100-native drop-in for the reference `vae_trainer.py` (the torchrun DDP entry, its CLI flags and the loss/autograd
 glue): GradNormFunction / gradnorm / avg_scalar_over_nodes / gan_disc_loss / vae_loss_function / blurriness_heatmap /
 create_dataloader / cleanup / train_ddp keep their names and argument meaning (vae_trainer.py:27-338); the step
 ordering of the loop follows vae_trainer.py:524-710.
