@@ -193,6 +193,34 @@ int vqb_gn_silu_bwd_pre(const void* x, const void* dy, const void* add, void* dx
  */
 int vqb_wavelet_fwd(const float* x, void* y, const float* filt, int N, int C, int H, int W, int Cpad, void* stream);
 
+/*
+ * bf16 inference path (README.hf.md "How to use": `VAE(...).cuda().bfloat16()`, `vae.encoder(img)`, `vae.decoder(z)`;
+ * the bf16 modules' nn.Conv2d / F.group_norm / F.scaled_dot_product_attention calls at ae.py:47-53,76-93,105-117,
+ * 143-154,160-167,197-199,230-232,282-284,307-309 then run on bf16 parameters and return bf16 tensors). Every entry
+ * point below validates its arguments (VQB_EINVAL) and fails with VQB_ENODEVICE without an sm_90 device.
+ *
+ * Weight packing from bf16 OIHW masters: the layouts of vqb_pack_weights / vqb_pack_weights_fold. The plain re-layout
+ * is exact (no rounding); folded taps are summed in fp32 and rounded once, like the fp32 path. vqb_pack_weights_multi
+ * takes bf16 masters through VqbPackJob.w_bf16.
+ */
+int vqb_pack_weights_bf16(const void* w_oihw, void* out, int Cout, int Cin, int T, int nslots, const int* tapmap_dev,
+                          int transpose, int Kpad, void* stream);
+int vqb_pack_weights_fold_bf16(const void* w_oihw, void* out, int Cout, int Cin, int T, int nslots,
+                               const int* tapmask_dev, int transpose, int Kpad, void* stream);
+/* bf16 NCHW image / latent -> bf16 NHWC (plain, or into the interior of a pre-zeroed [N][H+2pad][W+2pad][Cpad] frame for
+ * the fat-pixel first-layer conv), same (x - shift) * inv_scale option as vqb_nchw_to_nhwc; no fp32 copy of the input */
+int vqb_nchw_to_nhwc_bf16(const void* x, void* y, int N, int C, int H, int W, int Cpad, const float* shift,
+                          const float* inv_scale, void* stream);
+int vqb_nchw_to_nhwc_pad_bf16(const void* x, void* y, int N, int C, int H, int W, int Cpad, int pad,
+                              const float* shift, const float* inv_scale, void* stream);
+/* bf16 NHWC -> bf16 NCHW module-boundary output (a submodule called directly on an NCHW tensor); an exact copy */
+int vqb_nhwc_to_nchw_bf16(const void* y, void* x, int N, int C, int H, int W, int Cpad, void* stream);
+/* wavelet front-end (utils.py:229-247) of a bf16 image; filter sums in fp32 */
+int vqb_wavelet_fwd_bf16(const void* x, void* y, const float* filt, int N, int C, int H, int W, int Cpad,
+                         void* stream);
+/* The encoder z / decoder image of a bf16 module come straight out of conv_out's epilogue as bf16 NCHW through
+ * vqb_conv_gemm with out_f32 = 0 and NCHW output strides (oc = H*W): no separate conversion. */
+
 /* nearest-neighbour x2 up-sampling (ae.py:165) and its backward (2x2 sum), bf16 NHWC */
 int vqb_upsample2x_fwd(const void* x, void* y, int N, int H, int W, int C, void* stream);
 int vqb_upsample2x_bwd(const void* dy, void* dx, int N, int H, int W, int C, void* stream);
@@ -276,12 +304,12 @@ int vqb_adamw_flat_dev(float* params, const float* grads, float* exp_avg, float*
  * Replaces: the per-step fp32->bf16 weight casts of torch.autocast (vae_trainer.py:453,623).
  */
 typedef struct VqbPackJob {
-    const float* w;
+    const void* w;       /* OIHW master: fp32, or bf16 when w_bf16 = 1 */
     void* out;
     const int* tapmap;
     int32_t Cout, Cin, T, nslots, transpose, Kpad, fold, sg, ld_g, ld_r;
     int32_t first_block; /* prefix sum of the tile-block counts of the preceding jobs */
-    int32_t _pad;
+    int32_t w_bf16;      /* 1: w is a bf16 master (inference-only module; exact re-layout, folds summed in fp32) */
 } VqbPackJob;
 int vqb_pack_weights_multi(const VqbPackJob* jobs_dev, int njobs, int total_blocks, void* stream);
 

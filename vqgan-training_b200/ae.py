@@ -9,7 +9,9 @@ state_dict keys / fp32 OIHW shapes — but every forward/backward runs hand-writ
   AttnBlock                                                      -> GN kernel + 1x1 conv kernels + flash-style core
 
 Internally activations are bf16 NHWC (`Act`); modules accept either an `Act` (internal) or a plain NCHW tensor
-(reference calling convention: converted at the boundary, result returned as fp32 NCHW).
+(reference calling convention: converted at the boundary, result returned as NCHW in the dtype of the module's
+parameters). Modules converted with `.bfloat16()` run the same kernels from bf16 master weights and return bf16, like
+the reference's model-card inference recipe; they are inference-only (a backward through them raises).
 
 Reference citations: ae.py:13-14 swish, :41-53 FP32GroupNorm, :56-93 AttnBlock, :96-140 ResnetBlock, :143-154 Downsample,
 :157-167 Upsample, :170-257 Encoder, :260-333 Decoder, :336-348 DiagonalGaussian, :351-392 VAE.
@@ -56,15 +58,34 @@ class Act:
         return (n, self.C, h, w)
 
 
-def _enter(x):
+def _param_dtype(module: nn.Module):
+    """dtype of the module's parameters (fp32, or bf16 for an inference-only module); other dtypes raise here, before
+    anything is launched."""
+    p = next(module.parameters(), None)
+    if p is None:
+        return torch.float32
+    ops.check_master_dtype(p, f"{type(module).__name__} parameter")
+    return p.dtype
+
+
+def _enter(x, module: nn.Module):
     """NCHW tensor -> Act (or pass an Act through). Returns (act, was_external)."""
     if isinstance(x, Act):
         return x, False
+    _param_dtype(module)
     return Act(ops.to_nhwc(x), x.shape[1]), True
 
 
-def _exit(a: Act, external: bool):
-    return ops.to_nchw(a.t, a.C) if external else a
+def _exit(a: Act, external: bool, module: nn.Module):
+    return ops.to_nchw(a.t, a.C, _param_dtype(module)) if external else a
+
+
+def _stats_fusion() -> bool:
+    """Accumulate GroupNorm statistics in the producing conv's epilogue? Its fp32 atomics make the sums' order, and so
+    the last bits of every later activation, vary between launches. That is what training pays for one read pass less
+    per GroupNorm; without autograd (inference) the statistics come from the GroupNorm's own fixed-order pass instead,
+    so the forward is deterministic and a CUDA-graph replay equals the eager run bit for bit."""
+    return torch.is_grad_enabled() and os.environ.get("VQB_GN_STATS_FUSION", "1") == "1"
 
 
 def swish(x):
@@ -110,8 +131,8 @@ class StandardizedC2d(nn.Conv2d):
             return self.forward_act(x)
         if self._kind() == "s2":
             raise RuntimeError("stride-2 StandardizedC2d is only reachable through Downsample")
-        a, ext = _enter(x)
-        return _exit(self.forward_act(a), ext)
+        a, ext = _enter(x, self)
+        return _exit(self.forward_act(a), ext, self)
 
 
 class FP32GroupNorm(nn.GroupNorm):
@@ -121,15 +142,15 @@ class FP32GroupNorm(nn.GroupNorm):
         super().__init__(*args, **kwargs)
 
     def forward(self, input, silu: bool = False):
-        a, ext = _enter(input)
-        link = ops.GnLink() if (silu and not ext) else None
+        a, ext = _enter(input, self)
+        link = ops.GnLink() if (silu and not ext and torch.is_grad_enabled()) else None
         y = ops.group_norm_silu(a.t, self.weight, self.bias, self.num_groups, self.eps, silu, chsums=a.stats, link=link)
-        return _exit(Act(y, a.C, link=link), ext)
+        return _exit(Act(y, a.C, link=link), ext, self)
 
     def forward_with_skip(self, a: "Act", silu: bool = True):
         """-> (normalised activation, the input again). Consumers of the second output (the residual path) get their
         gradient summed inside the GroupNorm backward kernel (no separate accumulation pass)."""
-        link = ops.GnLink() if silu else None
+        link = ops.GnLink() if (silu and torch.is_grad_enabled()) else None  # backward-only state
         y, skip = ops.group_norm_silu(a.t, self.weight, self.bias, self.num_groups, self.eps, silu, with_skip=True,
                                       chsums=a.stats, link=link)
         return Act(y, a.C, link=link), Act(skip, a.C)
@@ -148,7 +169,7 @@ class AttnBlock(nn.Module):
         nn.init.normal_(self.proj_out.weight, std=0.2 / math.sqrt(in_channels))
 
     def attention(self, h_) -> Act:
-        a, _ = _enter(h_)
+        a, _ = _enter(h_, self)
         return self.attention_from_normed(self.norm(a))
 
     def attention_from_normed(self, h: Act) -> Act:
@@ -159,11 +180,11 @@ class AttnBlock(nn.Module):
         return Act(o, self.in_channels)
 
     def forward(self, x):
-        a, ext = _enter(x)
+        a, ext = _enter(x, self)
         hn, a_skip = self.norm.forward_with_skip(a, silu=False)
         h = self.attention_from_normed(hn)
         out = self.proj_out.forward_act(h, residual=a_skip)  # x + proj_out(attn(x)) fused in the conv epilogue
-        return _exit(out, ext)
+        return _exit(out, ext, self)
 
 
 class ResnetBlock(nn.Module):
@@ -185,13 +206,13 @@ class ResnetBlock(nn.Module):
         self.counter = 0
 
     def forward(self, x):
-        a, ext = _enter(x)
+        a, ext = _enter(x, self)
         h, a_skip = self.norm1.forward_with_skip(a, silu=True)
-        h = self.conv1.forward_act(h, want_stats=True)  # norm2's statistics come out of conv1's epilogue
+        h = self.conv1.forward_act(h, want_stats=_stats_fusion())  # norm2's statistics from conv1's epilogue
         h = self.norm2(h, silu=True)
         skip = self.nin_shortcut.forward_act(a_skip) if self.in_channels != self.out_channels else a_skip
-        out = self.conv2.forward_act(h, residual=skip, want_stats=True)  # x + h fused in conv2's epilogue
-        return _exit(out, ext)
+        out = self.conv2.forward_act(h, residual=skip, want_stats=_stats_fusion())  # x + h fused in the epilogue
+        return _exit(out, ext, self)
 
 
 class Downsample(nn.Module):
@@ -201,8 +222,8 @@ class Downsample(nn.Module):
 
     def forward(self, x):
         # F.pad(x, (0,1,0,1)) + stride-2 conv (ae.py:150-154): the pad row/column is the TMA unit's zero fill
-        a, ext = _enter(x)
-        return _exit(self.conv.forward_act(a, want_stats=True), ext)
+        a, ext = _enter(x, self)
+        return _exit(self.conv.forward_act(a, want_stats=_stats_fusion()), ext, self)
 
 
 class Upsample(nn.Module):
@@ -213,15 +234,15 @@ class Upsample(nn.Module):
     def forward(self, x):
         # nearest x2 + conv3x3 as four 2x2-tap phase convs over the low-res tensor (no 4x intermediate, 4/9 of the MACs);
         # VQB_UPSAMPLE_FOLD=0 selects the literal form (copy kernel + conv), kept for A/B measurements
-        a, ext = _enter(x)
+        a, ext = _enter(x, self)
         if os.environ.get("VQB_UPSAMPLE_FOLD", "1") == "1":
-            fuse = os.environ.get("VQB_GN_STATS_FUSION", "1") == "1"
+            fuse = _stats_fusion()
             y = ops.upsample_conv(a.t, self.conv.weight, self.conv.bias, self.conv._packed, want_stats=fuse)
             if fuse:
-                return _exit(Act(y[0], self.conv.out_channels, y[1]), ext)
-            return _exit(Act(y, self.conv.out_channels), ext)
+                return _exit(Act(y[0], self.conv.out_channels, y[1]), ext, self)
+            return _exit(Act(y, self.conv.out_channels), ext, self)
         up = Act(ops.upsample2x(a.t), a.C)
-        return _exit(self.conv.forward_act(up, want_stats=True), ext)
+        return _exit(self.conv.forward_act(up, want_stats=_stats_fusion()), ext, self)
 
 
 class Encoder(nn.Module):
@@ -284,6 +305,7 @@ class Encoder(nn.Module):
                 nn.init.zeros_(module.bias)
 
     def forward(self, x) -> Tensor:
+        _param_dtype(self)
         if self.use_wavelet and x.is_cuda and not x.requires_grad:
             # wavelet analysis (utils.py:229-247) fused with the NCHW->NHWC conversion: one kernel, no fp32 intermediate
             import utils as _u
@@ -293,7 +315,7 @@ class Encoder(nn.Module):
             h = self.wavelet_transform(x)
             fat = h.shape[1] <= 8 and ops.fat_conv_enabled()  # RGB input: 3 fat taps of 24, not 9 taps of 8 channels
             a = Act(ops.to_nhwc(h, frame=fat), h.shape[1], framed=fat)
-        a = self.conv_in.forward_act(a, want_stats=True)
+        a = self.conv_in.forward_act(a, want_stats=_stats_fusion())
         for i_level in range(self.num_resolutions):
             for i_block in range(self.num_res_blocks):
                 a = self.down[i_level].block[i_block](a)
@@ -306,7 +328,7 @@ class Encoder(nn.Module):
             a = self.mid.attn_1(a)
         a = self.mid.block_2(a)
         a = self.norm_out(a, silu=True)
-        return self.conv_out.forward_act(a, nchw_out=True)  # fp32 [B, z, h, w]
+        return self.conv_out.forward_act(a, nchw_out=True)  # [B, z, h, w] in the parameters' dtype
 
 
 class Decoder(nn.Module):
@@ -362,8 +384,9 @@ class Decoder(nn.Module):
                 nn.init.zeros_(module.bias)
 
     def forward(self, z) -> Tensor:
+        _param_dtype(self)
         a = Act(ops.to_nhwc(z), z.shape[1])
-        a = self.conv_in.forward_act(a, want_stats=True)
+        a = self.conv_in.forward_act(a, want_stats=_stats_fusion())
         a = self.mid.block_1(a)
         if not isinstance(self.mid.attn_1, nn.Identity):
             a = self.mid.attn_1(a)
@@ -376,7 +399,7 @@ class Decoder(nn.Module):
             if i_level != 0:
                 a = self.up[i_level].upsample(a)
         a = self.norm_out(a, silu=True)
-        return self.conv_out.forward_act(a, nchw_out=True)  # fp32 [B, out_ch, H, W]
+        return self.conv_out.forward_act(a, nchw_out=True)  # [B, out_ch, H, W] in the parameters' dtype
 
 
 class DiagonalGaussian(nn.Module):

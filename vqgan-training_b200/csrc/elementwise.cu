@@ -59,11 +59,11 @@ __device__ __forceinline__ float tanh_fast(float x) {
 }
 
 // ------------------------------------------------------------------ weight packing
-// out[r][slot][k] (bf16), r < R, k < Kpad:  transpose ? w[k][r][tap] : w[r][k][tap]   (w is OIHW fp32,
-// tap = tapmap[slot] indexes KH*KW), zero for k >= K.
-__global__ void pack_weights_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int Cout, int Cin,
-                                    int T, int nslots, const int* __restrict__ tapmap, int transpose, int Kpad,
-                                    int fold /* 0 none */) {
+// out[r][slot][k] (bf16), r < R, k < Kpad:  transpose ? w[k][r][tap] : w[r][k][tap]   (w is OIHW fp32 or bf16,
+// tap = tapmap[slot] indexes KH*KW), zero for k >= K. From a bf16 master the re-layout is exact.
+template <typename Src>
+__global__ void pack_weights_kernel(const Src* __restrict__ w, __nv_bfloat16* __restrict__ out, int Cout, int Cin,
+                                    int T, int nslots, const int* __restrict__ tapmap, int transpose, int Kpad) {
     const int R = transpose ? Cin : Cout;
     const int K = transpose ? Cout : Cin;
     const int64_t total = static_cast<int64_t>(R) * nslots * Kpad;
@@ -76,15 +76,17 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, __nv_bfloat16* 
         if (k < K) {
             const int tap = tapmap[slot];
             const int co = transpose ? k : r, ci = transpose ? r : k;
-            v = w[(static_cast<int64_t>(co) * Cin + ci) * T + tap];
+            v = to_f32(w[(static_cast<int64_t>(co) * Cin + ci) * T + tap]);
         }
         out[i] = __float2bfloat16(v);
     }
 }
 
 // Folded packing: out[r][slot][k] = sum over the taps in tapmask[slot] (bit t = tap t) of w[..][tap]; the fp32 sum is
-// rounded to bf16 once. Used by the nearest-2x-upsample + conv3x3 fusion (4 phase convs with 2x2 folded taps).
-__global__ void pack_weights_fold_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int Cout,
+// rounded to bf16 once (for a bf16 master too). Used by the nearest-2x-upsample + conv3x3 fusion (4 phase convs with
+// 2x2 folded taps).
+template <typename Src>
+__global__ void pack_weights_fold_kernel(const Src* __restrict__ w, __nv_bfloat16* __restrict__ out, int Cout,
                                          int Cin, int T, int nslots, const int* __restrict__ tapmask, int transpose,
                                          int Kpad) {
     const int R = transpose ? Cin : Cout;
@@ -99,9 +101,9 @@ __global__ void pack_weights_fold_kernel(const float* __restrict__ w, __nv_bfloa
         if (k < K) {
             const int mask = tapmask[slot];
             const int co = transpose ? k : r, ci = transpose ? r : k;
-            const float* wp = w + (static_cast<int64_t>(co) * Cin + ci) * T;
+            const Src* wp = w + (static_cast<int64_t>(co) * Cin + ci) * T;
             for (int t = 0; t < T; ++t)
-                if ((mask >> t) & 1) v += wp[t];
+                if ((mask >> t) & 1) v += to_f32(wp[t]);
         }
         out[i] = __float2bfloat16(v);
     }
@@ -110,7 +112,9 @@ __global__ void pack_weights_fold_kernel(const float* __restrict__ w, __nv_bfloa
 // ------------------------------------------------------------------ layout conversion
 // y[n,h,w,c] = (x[n,c,h,w] - shift[c]) * inv_scale[c]   (bf16 NHWC, channels >= C zero)
 // pad > 0: y is [N][H+2pad][W+2pad][Cpad] (pre-zeroed) and only its interior is written (W needed then)
-__global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int C, int HW,
+// x is fp32 or bf16 (a bf16 image enters without an fp32 copy; the affine math is fp32 either way)
+template <typename In>
+__global__ void nchw_to_nhwc_kernel(const In* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int C, int HW,
                                     int Cpad, const float* __restrict__ shift, const float* __restrict__ inv_scale,
                                     int W, int pad) {
     const int64_t total = static_cast<int64_t>(N) * HW;
@@ -118,7 +122,7 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __nv_bfloat16* 
     for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
          i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int64_t n = i / HW, p = i % HW;
-        const float* xp = x + n * C * HW + p;
+        const In* xp = x + n * C * HW + p;
         int64_t opix = i;
         if (pad) {
             const int h = static_cast<int>(p / W), w = static_cast<int>(p % W);
@@ -132,7 +136,7 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __nv_bfloat16* 
                 const int c = c0 + j;
                 float v = 0.f;
                 if (c < C) {
-                    v = xp[static_cast<int64_t>(c) * HW];
+                    v = to_f32(xp[static_cast<int64_t>(c) * HW]);
                     if (shift) v = (v - shift[c]) * inv_scale[c];
                 }
                 f[j] = v;
@@ -142,8 +146,9 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __nv_bfloat16* 
     }
 }
 
-// gx[n,c,h,w] = g[n,h,w,c] * inv_scale[c]   (fp32 NCHW out)
-__global__ void nhwc_to_nchw_kernel(const __nv_bfloat16* __restrict__ g, float* __restrict__ gx, int N, int C, int HW,
+// gx[n,c,h,w] = g[n,h,w,c] * inv_scale[c]   (fp32 or bf16 NCHW out; without inv_scale the bf16 copy is exact)
+template <typename Out>
+__global__ void nhwc_to_nchw_kernel(const __nv_bfloat16* __restrict__ g, Out* __restrict__ gx, int N, int C, int HW,
                                     int Cpad, const float* __restrict__ inv_scale, int W, int pad) {
     const int64_t total = static_cast<int64_t>(N) * HW;
     const int H = HW / W;
@@ -156,25 +161,25 @@ __global__ void nhwc_to_nchw_kernel(const __nv_bfloat16* __restrict__ g, float* 
             ipix = (n * (H + 2 * pad) + h + pad) * (W + 2 * pad) + w + pad;
         }
         const __nv_bfloat16* gp = g + ipix * Cpad;
-        float* xp = gx + n * C * HW + p;
+        Out* xp = gx + n * C * HW + p;
         for (int c = 0; c < C; ++c) {
             float v = __bfloat162float(gp[c]);
             if (inv_scale) v *= inv_scale[c];
-            xp[static_cast<int64_t>(c) * HW] = v;
+            from_f32(xp[static_cast<int64_t>(c) * HW], v);
         }
     }
 }
 
 // ------------------------------------------------------------------ GroupNorm forward
 // grid (chunks, N); thread t owns channel vector cv = t % V (V = C/8) and pixel rows t / V + k*R.
+// The R row partials of a block are summed in a fixed order (no shared-memory float atomics), so the fp32 chunk sums do
+// not depend on thread timing; chunks are combined in double.
 __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, double* __restrict__ sums /* [N][C][2] */, int HW,
                                 int C, int pix_per_chunk) {
-    extern __shared__ float sm[];  // [C][2]
+    extern __shared__ float sm[];  // [R][C][2]
     const int V = C >> 3, R = blockDim.x / V;
     const int cv = threadIdx.x % V, pr = threadIdx.x / V;
     const int n = blockIdx.y;
-    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sm[i] = 0.f;
-    __syncthreads();
     float s[8], q[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
@@ -209,13 +214,16 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, double* __r
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            atomicAdd(&sm[(cv * 8 + j) * 2], s[j]);
-            atomicAdd(&sm[(cv * 8 + j) * 2 + 1], q[j]);
+            sm[(pr * C + cv * 8 + j) * 2] = s[j];
+            sm[(pr * C + cv * 8 + j) * 2 + 1] = q[j];
         }
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x)
-        atomicAdd(&sums[static_cast<int64_t>(n) * 2 * C + i], static_cast<double>(sm[i]));
+    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
+        float v = 0.f;
+        for (int r = 0; r < R; ++r) v += sm[r * 2 * C + i];
+        atomicAdd(&sums[static_cast<int64_t>(n) * 2 * C + i], static_cast<double>(v));
+    }
 }
 
 // mean / rstd per (n, group) from the per-channel double sums.
@@ -866,8 +874,9 @@ __global__ void wgrad_reduce_fold_kernel(const float* __restrict__ partial, floa
 // y[n, ho, wo, c*4 + band] = sum_{i,j < 6} x[n, c, 2ho + i - 2, 2wo + j - 2] * filt[band][i][j]   (zero outside):
 // the reference's F.pad(2) + grouped 6x6 stride-2 conv, fused with the NCHW fp32 -> NHWC bf16 layout conversion the
 // encoder's first conv needs. One thread per output pixel; the 6x6 windows of neighbouring pixels overlap 9x, which the
-// L1/L2 absorbs (the whole input batch is a few tens of MB).
-__global__ void wavelet_fwd_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y,
+// L1/L2 absorbs (the whole input batch is a few tens of MB). x is fp32 or bf16; the filter sums are fp32 either way.
+template <typename In>
+__global__ void wavelet_fwd_kernel(const In* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                    const float* __restrict__ filt, int N, int C, int H, int W, int Cpad) {
     __shared__ float f[4 * 36];
     for (int i = threadIdx.x; i < 144; i += blockDim.x) f[i] = filt[i];
@@ -880,7 +889,7 @@ __global__ void wavelet_fwd_kernel(const float* __restrict__ x, __nv_bfloat16* _
         const int64_t n = p / (static_cast<int64_t>(Wo) * Ho);
         __nv_bfloat16* yp = y + p * Cpad;
         for (int c = 0; c < C; ++c) {
-            const float* xp = x + (n * C + c) * static_cast<int64_t>(H) * W;
+            const In* xp = x + (n * C + c) * static_cast<int64_t>(H) * W;
             float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
             for (int i = 0; i < 6; ++i) {
@@ -890,7 +899,7 @@ __global__ void wavelet_fwd_kernel(const float* __restrict__ x, __nv_bfloat16* _
                 for (int j = 0; j < 6; ++j) {
                     const int w = 2 * wo + j - 2;
                     if (w < 0 || w >= W) continue;
-                    const float v = __ldg(xp + static_cast<int64_t>(h) * W + w);
+                    const float v = to_f32(__ldg(xp + static_cast<int64_t>(h) * W + w));
 #pragma unroll
                     for (int b = 0; b < 4; ++b) acc[b] = fmaf(v, f[b * 36 + i * 6 + j], acc[b]);
                 }
@@ -956,8 +965,8 @@ int vqb_pack_weights(const float* w, void* out, int Cout, int Cin, int T, int ns
     VQB_CHECK(Kpad % 8 == 0 && Kpad >= (transpose ? Cout : Cin), "vqb_pack_weights: bad Kpad=%d", Kpad);
     const int R = transpose ? Cin : Cout;
     const int64_t total = static_cast<int64_t>(R) * nslots * Kpad;
-    pack_weights_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        w, static_cast<__nv_bfloat16*>(out), Cout, Cin, T, nslots, tapmap_dev, transpose, Kpad, 0);
+    pack_weights_kernel<float><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        w, static_cast<__nv_bfloat16*>(out), Cout, Cin, T, nslots, tapmap_dev, transpose, Kpad);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
@@ -969,8 +978,43 @@ int vqb_pack_weights_fold(const float* w, void* out, int Cout, int Cin, int T, i
     VQB_CHECK(Kpad % 8 == 0 && Kpad >= (transpose ? Cout : Cin) && T <= 31, "vqb_pack_weights_fold: bad Kpad/T");
     const int R = transpose ? Cin : Cout;
     const int64_t total = static_cast<int64_t>(R) * nslots * Kpad;
-    pack_weights_fold_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    pack_weights_fold_kernel<float><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         w, static_cast<__nv_bfloat16*>(out), Cout, Cin, T, nslots, tapmask_dev, transpose, Kpad);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+// bf16 OIHW masters (inference-only modules): same layouts as vqb_pack_weights / vqb_pack_weights_fold
+int vqb_pack_weights_bf16(const void* w, void* out, int Cout, int Cin, int T, int nslots, const int* tapmap_dev,
+                          int transpose, int Kpad, void* stream) {
+    VQB_CHECK(w && out && tapmap_dev, "vqb_pack_weights_bf16: null pointer");
+    VQB_CHECK(Cout > 0 && Cin > 0 && T > 0 && nslots > 0 && Kpad % 8 == 0 && Kpad >= (transpose ? Cout : Cin),
+              "vqb_pack_weights_bf16: bad shape (Cout=%d Cin=%d T=%d nslots=%d Kpad=%d)", Cout, Cin, T, nslots, Kpad);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_pack_weights_bf16: current device is not sm_90");
+    const int R = transpose ? Cin : Cout;
+    const int64_t total = static_cast<int64_t>(R) * nslots * Kpad;
+    pack_weights_kernel<__nv_bfloat16><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(w), static_cast<__nv_bfloat16*>(out), Cout, Cin, T, nslots, tapmap_dev,
+        transpose, Kpad);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+int vqb_pack_weights_fold_bf16(const void* w, void* out, int Cout, int Cin, int T, int nslots,
+                               const int* tapmask_dev, int transpose, int Kpad, void* stream) {
+    VQB_CHECK(w && out && tapmask_dev, "vqb_pack_weights_fold_bf16: null pointer");
+    VQB_CHECK(Cout > 0 && Cin > 0 && T > 0 && T <= 31 && nslots > 0 && Kpad % 8 == 0 &&
+                  Kpad >= (transpose ? Cout : Cin),
+              "vqb_pack_weights_fold_bf16: bad shape (Cout=%d Cin=%d T=%d nslots=%d Kpad=%d)", Cout, Cin, T, nslots,
+              Kpad);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_pack_weights_fold_bf16: current device is not sm_90");
+    const int R = transpose ? Cin : Cout;
+    const int64_t total = static_cast<int64_t>(R) * nslots * Kpad;
+    pack_weights_fold_kernel<__nv_bfloat16><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(w), static_cast<__nv_bfloat16*>(out), Cout, Cin, T, nslots, tapmask_dev,
+        transpose, Kpad);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
@@ -991,8 +1035,42 @@ int vqb_nchw_to_nhwc(const float* x, void* y, int N, int C, int H, int W, int Cp
                      const float* inv_scale, void* stream) {
     VQB_CHECK(x && y && Cpad % 8 == 0 && Cpad >= C, "vqb_nchw_to_nhwc: bad arguments");
     const int64_t total = static_cast<int64_t>(N) * H * W;
-    nchw_to_nhwc_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    nchw_to_nhwc_kernel<float><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         x, static_cast<__nv_bfloat16*>(y), N, C, H * W, Cpad, shift, inv_scale, W, 0);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+// bf16 NCHW input (bf16 modules / bf16 images): plain (pad = 0) or into the interior of a PRE-ZEROED framed buffer
+int vqb_nchw_to_nhwc_pad_bf16(const void* x, void* y, int N, int C, int H, int W, int Cpad, int pad,
+                              const float* shift, const float* inv_scale, void* stream) {
+    VQB_CHECK(x && y && N > 0 && C > 0 && H > 0 && W > 0 && Cpad % 8 == 0 && Cpad >= C && pad >= 0 &&
+                  (shift == nullptr) == (inv_scale == nullptr),
+              "vqb_nchw_to_nhwc_pad_bf16: bad arguments");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_nchw_to_nhwc_pad_bf16: current device is not sm_90");
+    const int64_t total = static_cast<int64_t>(N) * H * W;
+    nchw_to_nhwc_kernel<__nv_bfloat16><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), N, C, H * W, Cpad, shift, inv_scale, W,
+        pad);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+int vqb_nchw_to_nhwc_bf16(const void* x, void* y, int N, int C, int H, int W, int Cpad, const float* shift,
+                          const float* inv_scale, void* stream) {
+    return vqb_nchw_to_nhwc_pad_bf16(x, y, N, C, H, W, Cpad, 0, shift, inv_scale, stream);
+}
+
+// bf16 NHWC -> bf16 NCHW (the module-boundary output of a bf16 module; an exact copy)
+int vqb_nhwc_to_nchw_bf16(const void* y, void* x, int N, int C, int H, int W, int Cpad, void* stream) {
+    VQB_CHECK(y && x && N > 0 && C > 0 && H > 0 && W > 0 && Cpad % 8 == 0 && Cpad >= C,
+              "vqb_nhwc_to_nchw_bf16: bad arguments");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_nhwc_to_nchw_bf16: current device is not sm_90");
+    const int64_t total = static_cast<int64_t>(N) * H * W;
+    nhwc_to_nchw_kernel<__nv_bfloat16><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(y), static_cast<__nv_bfloat16*>(x), N, C, H * W, Cpad, nullptr, W, 0);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
@@ -1003,7 +1081,7 @@ int vqb_nchw_to_nhwc_pad(const float* x, void* y, int N, int C, int H, int W, in
                          const float* inv_scale, void* stream) {
     VQB_CHECK(x && y && Cpad % 8 == 0 && Cpad >= C && pad >= 0, "vqb_nchw_to_nhwc_pad: bad arguments");
     const int64_t total = static_cast<int64_t>(N) * H * W;
-    nchw_to_nhwc_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    nchw_to_nhwc_kernel<float><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         x, static_cast<__nv_bfloat16*>(y), N, C, H * W, Cpad, shift, inv_scale, W, pad);
     VQB_CUDA(cudaGetLastError());
     count_launch();
@@ -1015,7 +1093,7 @@ int vqb_nhwc_to_nchw_pad(const void* g, float* gx, int N, int C, int H, int W, i
                          const float* inv_scale, void* stream) {
     VQB_CHECK(g && gx && Cpad % 8 == 0 && Cpad >= C && pad >= 0, "vqb_nhwc_to_nchw_pad: bad arguments");
     const int64_t total = static_cast<int64_t>(N) * H * W;
-    nhwc_to_nchw_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    nhwc_to_nchw_kernel<float><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(g), gx, N, C, H * W, Cpad, inv_scale, W, pad);
     VQB_CUDA(cudaGetLastError());
     count_launch();
@@ -1026,7 +1104,7 @@ int vqb_nhwc_to_nchw(const void* g, float* gx, int N, int C, int H, int W, int C
                      void* stream) {
     VQB_CHECK(g && gx && Cpad % 8 == 0 && Cpad >= C, "vqb_nhwc_to_nchw: bad arguments");
     const int64_t total = static_cast<int64_t>(N) * H * W;
-    nhwc_to_nchw_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    nhwc_to_nchw_kernel<float><<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(g), gx, N, C, H * W, Cpad, inv_scale, W, 0);
     VQB_CUDA(cudaGetLastError());
     count_launch();
@@ -1042,8 +1120,9 @@ int vqb_gn_silu_fwd(const void* x, void* y, const float* gamma, const float* bet
     VQB_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * 2 * N * C, st));
     int chunks, ppc;
     const int T = cv_threads(C);
-    cv_grid(HW, C, N, gn_stats_kernel, 2 * C * sizeof(float), chunks, ppc);
-    gn_stats_kernel<<<dim3(chunks, N), T, 2 * C * sizeof(float), st>>>(static_cast<const __nv_bfloat16*>(x), ws, HW, C,
+    const size_t stats_smem = static_cast<size_t>(T / (C / 8)) * 2 * C * sizeof(float);  // [R][C][2]
+    cv_grid(HW, C, N, gn_stats_kernel, stats_smem, chunks, ppc);
+    gn_stats_kernel<<<dim3(chunks, N), T, stats_smem, st>>>(static_cast<const __nv_bfloat16*>(x), ws, HW, C,
                                                                         ppc);
     gn_finalize_kernel<<<(N * G + 127) / 128, 128, 0, st>>>(ws, mr, N, C, G, HW, eps);
     cv_grid(HW, C, N, gn_apply_kernel, 0, chunks, ppc);
@@ -1199,8 +1278,22 @@ int vqb_wavelet_fwd(const float* x, void* y, const float* filt, int N, int C, in
     VQB_CHECK(x && y && filt && H % 2 == 0 && W % 2 == 0 && Cpad % 8 == 0 && Cpad >= 4 * C,
               "vqb_wavelet_fwd: bad arguments (H, W even; Cpad >= 4C, multiple of 8)");
     const int64_t total = static_cast<int64_t>(N) * (H / 2) * (W / 2);
-    wavelet_fwd_kernel<<<gs_blocks(total, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+    wavelet_fwd_kernel<float><<<gs_blocks(total, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(
         x, static_cast<__nv_bfloat16*>(y), filt, N, C, H, W, Cpad);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+int vqb_wavelet_fwd_bf16(const void* x, void* y, const float* filt, int N, int C, int H, int W, int Cpad,
+                         void* stream) {
+    VQB_CHECK(x && y && filt && N > 0 && C > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && Cpad % 8 == 0 &&
+                  Cpad >= 4 * C,
+              "vqb_wavelet_fwd_bf16: bad arguments (H, W even; Cpad >= 4C, multiple of 8)");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_wavelet_fwd_bf16: current device is not sm_90");
+    const int64_t total = static_cast<int64_t>(N) * (H / 2) * (W / 2);
+    wavelet_fwd_kernel<__nv_bfloat16><<<gs_blocks(total, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), filt, N, C, H, W, Cpad);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;

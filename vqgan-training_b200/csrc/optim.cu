@@ -66,23 +66,47 @@ __global__ void __launch_bounds__(256) adamw_flat_kernel(float* __restrict__ p, 
 //   out[r*ld_r + (slot / sg) * ld_g + (slot % sg) * Kpad + k] = bf16( transpose ? w[k][r][taps] : w[r][k][taps] ), k < K,
 //   zero for K <= k < Kpad; `taps` = tapmap[slot] (one tap) or, fold = 1, the fp32 SUM over the taps whose bit is set.
 // Normal layouts have sg = nslots (one group); the fat-pixel layout [R][3][64] has sg = 3, ld_g = 64 (columns beyond
-// 3*Kpad stay at their initial zero).
+// 3*Kpad stay at their initial zero). The master w is fp32 or (w_bf16 = 1, inference-only modules) bf16; either way the
+// tile is staged in fp32, so a bf16 master is re-laid out exactly and folded taps are summed in fp32 before one rounding.
 struct PackJob {
-    const float* w;
+    const void* w;
     __nv_bfloat16* out;
     const int* tapmap;
     int Cout, Cin, T, nslots, transpose, Kpad, fold, sg, ld_g, ld_r;
     int first_block;  // prefix sum of ceil(R/8)*ceil(Kpad/64) tile blocks over the jobs before this one
-    int _pad;
+    int w_bf16;
 };
+
 static_assert(sizeof(PackJob) == sizeof(VqbPackJob), "PackJob must mirror VqbPackJob");
+constexpr int kPackRows = 8, kPackK = 64, kPackMaxT = 16;
+
+// forward layout tile[r*64T + (k*T + t)], transposed tile[k*(8T+1) + (r*T + t)] (no runtime divisions)
+template <typename Src>
+__device__ __forceinline__ void pack_load_tile(const PackJob& jb, const Src* w, float* tile, int r0, int k0, int nr,
+                                               int nk, int warp, int lane) {
+    const int T = jb.T;
+    if (!jb.transpose) {
+        const int run = nk * T;  // contiguous elements of one row
+        for (int r = warp; r < kPackRows; r += 8) {
+            const Src* src = w + (static_cast<int64_t>(r0 + r) * jb.Cin + k0) * T;
+            for (int e = lane; e < kPackK * T; e += 32)
+                tile[r * kPackK * T + e] = (r < nr && e < run) ? to_f32(src[e]) : 0.f;
+        }
+    } else {
+        const int run = nr * T;  // contiguous elements of one k (= one output channel's rows r0..r0+7)
+        const int kstride = kPackRows * T + 1;
+        for (int k = warp; k < kPackK; k += 8) {
+            const Src* src = w + (static_cast<int64_t>(k0 + k) * jb.Cin + r0) * T;
+            for (int e = lane; e < kPackRows * T; e += 32)
+                tile[k * kstride + e] = (k < nk && e < run) ? to_f32(src[e]) : 0.f;
+        }
+    }
+}
 
 // One block = an (8 rows) x (64 k) tile of one job, all slots: the OIHW source is read in contiguous runs (64*T floats per
 // row for the forward layout, 8*T floats per k for the transposed one) into shared memory, then every slot's 64
 // consecutive bf16 (128 B) are written coalesced, so the re-pack streams HBM / L2 instead of reading with a stride of T
 // floats.
-constexpr int kPackRows = 8, kPackK = 64, kPackMaxT = 16;
-
 __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackJob* __restrict__ jobs, int njobs) {
     __shared__ float tile[kPackK * (kPackRows * kPackMaxT + 1)];
     // binary search: last job with first_block <= blockIdx.x
@@ -100,21 +124,10 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackJob* 
     const int r0 = (bid / kblocks) * kPackRows, k0 = (bid % kblocks) * kPackK;
     const int nr = min(kPackRows, R - r0), nk = max(0, min(kPackK, K - k0));
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // ---- load (no runtime divisions): forward layout tile[r*64T + (k*T + t)], transposed tile[k*(8T+1) + (r*T + t)]
-    if (!jb.transpose) {
-        const int run = nk * T;  // contiguous floats of one row
-        for (int r = warp; r < kPackRows; r += 8) {
-            const float* src = jb.w + (static_cast<int64_t>(r0 + r) * jb.Cin + k0) * T;
-            for (int e = lane; e < kPackK * T; e += 32) tile[r * kPackK * T + e] = (r < nr && e < run) ? src[e] : 0.f;
-        }
-    } else {
-        const int run = nr * T;  // contiguous floats of one k (= one output channel's rows r0..r0+7)
-        const int kstride = kPackRows * T + 1;
-        for (int k = warp; k < kPackK; k += 8) {
-            const float* src = jb.w + (static_cast<int64_t>(k0 + k) * jb.Cin + r0) * T;
-            for (int e = lane; e < kPackRows * T; e += 32) tile[k * kstride + e] = (k < nk && e < run) ? src[e] : 0.f;
-        }
-    }
+    if (jb.w_bf16)
+        pack_load_tile(jb, static_cast<const __nv_bfloat16*>(jb.w), tile, r0, k0, nr, nk, warp, lane);
+    else
+        pack_load_tile(jb, static_cast<const float*>(jb.w), tile, r0, k0, nr, nk, warp, lane);
     __syncthreads();
     // ---- store: thread = (row pair q, k); every (row, slot) writes 64 consecutive bf16
     const int k = threadIdx.x & (kPackK - 1), q = threadIdx.x >> 6;

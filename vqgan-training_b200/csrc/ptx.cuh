@@ -245,4 +245,10 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
     return __bfloat1622float2(h);
 }
 
+// element loads / stores of the kernels templated on an fp32 or bf16 global tensor (boundary conversions, packing)
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ void from_f32(float& d, float v) { d = v; }
+__device__ __forceinline__ void from_f32(__nv_bfloat16& d, float v) { d = __float2bfloat16(v); }
+
 }  // namespace vqb

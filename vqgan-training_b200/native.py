@@ -51,7 +51,7 @@ class VqbPackJob(C.Structure):
     _fields_ = [("w", C.c_void_p), ("out", C.c_void_p), ("tapmap", C.c_void_p), ("Cout", C.c_int32), ("Cin", C.c_int32),
                 ("T", C.c_int32), ("nslots", C.c_int32), ("transpose", C.c_int32), ("Kpad", C.c_int32),
                 ("fold", C.c_int32), ("sg", C.c_int32), ("ld_g", C.c_int32), ("ld_r", C.c_int32),
-                ("first_block", C.c_int32), ("_pad", C.c_int32)]
+                ("first_block", C.c_int32), ("w_bf16", C.c_int32)]
 
 
 class VqbAdamwGroup(C.Structure):
@@ -118,6 +118,12 @@ def load():
         "vqb_pack_weights_multi": (i32, [vp, i32, i32, vp]),
         "vqb_adamw_fill_record": (i32, [i32, C.POINTER(VqbAdamwGroup), vp]),
         "vqb_adamw_flat_dev": (i32, [vp, vp, vp, vp, vp, i64, vp, f32, vp]),
+        "vqb_pack_weights_bf16": (i32, [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp]),
+        "vqb_pack_weights_fold_bf16": (i32, [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp]),
+        "vqb_nchw_to_nhwc_bf16": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]),
+        "vqb_nchw_to_nhwc_pad_bf16": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
+        "vqb_nhwc_to_nchw_bf16": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
+        "vqb_wavelet_fwd_bf16": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)

@@ -2,7 +2,9 @@
 
 Internal activation format: contiguous bf16 tensors of shape [N, H, W, Cp] (NHWC, Cp = channels padded to a multiple
 of 8, pad channels zero). Master weights / gradients stay fp32 OIHW nn.Parameters (the reference's state_dict
-contract); bf16 packed copies for the tensor-core kernels are caches keyed on the parameter version.
+contract); bf16 packed copies for the tensor-core kernels are caches keyed on the parameter version. A module converted
+with `.bfloat16()` (the reference's model-card inference recipe) keeps bf16 masters: it is packed from them directly,
+returns bf16 at its boundary and is inference-only (its backward raises, see `inference_only`).
 
 Every op here launches hand-written CUDA; nothing falls back to ATen for the math.
 """
@@ -41,38 +43,66 @@ def tapmap_tensor(tapmap, device) -> torch.Tensor:
     return t
 
 
+MASTER_DTYPES = (torch.float32, torch.bfloat16)
+
+
+def check_master_dtype(t: torch.Tensor, what="parameter"):
+    """fp32 (training and inference) and bf16 (inference only) are the parameter dtypes the kernels read; anything else
+    is refused here, before a pointer reaches a kernel that would reinterpret its memory."""
+    if t.dtype not in MASTER_DTYPES:
+        raise RuntimeError(f"vqgan-training_b200: {what} has dtype {t.dtype}; supported parameter dtypes are "
+                           "torch.float32 (training and inference) and torch.bfloat16 (inference only)")
+
+
+def inference_only(*params):
+    """Backward guard of the conv / GroupNorm functions: bf16 modules are inference-only (there are no bf16-master
+    gradient kernels, and the optimizer path keeps fp32 masters)."""
+    for p in params:
+        if p is not None and p.dtype != torch.float32:
+            raise RuntimeError(
+                f"vqgan-training_b200: bf16 modules are inference-only: backward through a module with {p.dtype} "
+                "parameters is not supported. Run it under torch.no_grad() / torch.inference_mode(), or train the "
+                "float32 module (`.float()`).")
+
+
 def pack_weights(weight: torch.Tensor, tapmap, transpose: bool, Kpad: int, fold: bool = False) -> torch.Tensor:
-    """OIHW fp32 -> bf16 [R][len(tapmap)][Kpad] (R = Cin if transpose else Cout). fold: tapmap holds bit masks of taps
-    whose weights are summed (fp32) before the single bf16 rounding."""
+    """OIHW fp32 or bf16 -> bf16 [R][len(tapmap)][Kpad] (R = Cin if transpose else Cout). fold: tapmap holds bit masks
+    of taps whose weights are summed (fp32) before the single bf16 rounding."""
     Cout, Cin, KH, KW = weight.shape
     R = Cin if transpose else Cout
     out = torch.empty(R, len(tapmap), Kpad, device=weight.device, dtype=torch.bfloat16)
     tm = tapmap_tensor(tapmap, weight.device)
     w = weight.detach()
-    if w.dtype != torch.float32 or not w.is_contiguous():
-        w = w.float().contiguous()
-    fn = _L().vqb_pack_weights_fold if fold else _L().vqb_pack_weights
+    if w.dtype == torch.bfloat16:
+        w = w.contiguous()
+        fn = _L().vqb_pack_weights_fold_bf16 if fold else _L().vqb_pack_weights_bf16
+    else:
+        if w.dtype != torch.float32 or not w.is_contiguous():
+            w = w.float().contiguous()
+        fn = _L().vqb_pack_weights_fold if fold else _L().vqb_pack_weights
     check(fn(ptr(w), ptr(out), Cout, Cin, KH * KW, len(tapmap), ptr(tm), 1 if transpose else 0, Kpad, stream_ptr()),
           "pack_weights")
     return out
 
 
 class _PackEntry:
-    """One cached bf16 GEMM operand of one fp32 OIHW parameter + the recipe to rebuild it in place."""
+    """One cached bf16 GEMM operand of one fp32 or bf16 OIHW parameter + the recipe to rebuild it in place."""
 
-    __slots__ = ("wref", "out", "tm", "spec", "ver", "__weakref__")
+    __slots__ = ("wref", "out", "tm", "spec", "ver", "dtype", "__weakref__")
 
     def __init__(self, weight, out, tm, spec):
         self.wref = weakref.ref(weight)
         self.out, self.tm, self.spec = out, tm, spec
         self.ver = (weight._version, weight.data_ptr())
+        self.dtype = weight.dtype  # the master's dtype selects the kernel's source type (VqbPackJob.w_bf16)
 
     def job(self, first_block):
         w = self.wref()
         Cout, Cin, T, nslots, transpose, Kpad, fold, sg, ld_g, ld_r = self.spec
         return native.VqbPackJob(w=w.data_ptr(), out=self.out.data_ptr(), tapmap=self.tm.data_ptr(), Cout=Cout, Cin=Cin,
                                  T=T, nslots=nslots, transpose=transpose, Kpad=Kpad, fold=fold, sg=sg, ld_g=ld_g,
-                                 ld_r=ld_r, first_block=first_block, _pad=0)
+                                 ld_r=ld_r, first_block=first_block,
+                                 w_bf16=1 if self.dtype == torch.bfloat16 else 0)
 
     def blocks(self):  # one block = an 8-row x 64-k tile, all slots (csrc/optim.cu)
         Cout, Cin, T, nslots, transpose, Kpad = self.spec[:6]
@@ -80,7 +110,7 @@ class _PackEntry:
         return -(-(Cin if transpose else Cout) // 8) * -(-Kpad // 64)
 
 
-# every live pack entry, by the data_ptr of the fp32 master weight it was packed from (weak: caches own the entries)
+# every live pack entry, by the data_ptr of the master weight it was packed from (weak: caches own the entries)
 _pack_registry = {}
 _pack_tables = {}
 
@@ -96,15 +126,17 @@ def _new_pack_entry(weight, tapmap, transpose, Kpad, fold, fat=False) -> _PackEn
     else:
         out = torch.empty(R, nslots, Kpad, device=weight.device, dtype=torch.bfloat16)
         spec = (Cout, Cin, KH * KW, nslots, 1 if transpose else 0, Kpad, 1 if fold else 0, nslots, 0, nslots * Kpad)
-    if weight.dtype != torch.float32 or not weight.is_contiguous():
-        raise RuntimeError("vqgan-training_b200: conv master weights must be contiguous fp32 OIHW tensors")
+    check_master_dtype(weight, "conv master weight")
+    if not weight.is_contiguous():
+        raise RuntimeError("vqgan-training_b200: conv master weights must be contiguous OIHW tensors")
     ent = _PackEntry(weight, out, tapmap_tensor(tapmap, weight.device), spec)
     _pack_registry.setdefault(weight.data_ptr(), weakref.WeakSet()).add(ent)
     return ent
 
 
 def _run_pack(entries):
-    """Re-packs `entries` (in place) with ONE vqb_pack_weights_multi launch; the device job table is cached per entry set."""
+    """Re-packs `entries` (in place) with ONE vqb_pack_weights_multi launch (fp32 and bf16 masters may be mixed: each
+    job carries its source dtype); the device job table is cached per entry set."""
     if not entries:
         return
     key = tuple(id(e) for e in entries)
@@ -142,7 +174,7 @@ def weights_updated(params=None):
             continue
         for e in list(ws):
             w = e.wref()
-            if w is None or w.data_ptr() != dp:
+            if w is None or w.data_ptr() != dp or w.dtype != e.dtype:
                 ws.discard(e)
                 continue
             entries.append(e)
@@ -172,7 +204,8 @@ except Exception:  # pragma: no cover
 
 
 class PackedCache:
-    """Per-conv-layer caches: bf16 packed copies of the fp32 OIHW parameter and the shape-dependent geometry objects /
+    """Per-conv-layer caches: bf16 packed copies of the OIHW parameter (fp32 or bf16) and the shape-dependent geometry
+    objects /
     C descriptors (built once per input shape). A packed copy is valid while (parameter version, data_ptr) are unchanged;
     updates that bypass the version counter are announced through `weights_updated` (global optimizer post-step hook)."""
 
@@ -189,7 +222,7 @@ class PackedCache:
 
     def get(self, weight: torch.Tensor, key, tapmap, transpose, Kpad, fold=False, fat=False):
         ent = self._store.get(key)
-        if ent is None or ent.wref() is None or ent.ver[1] != weight.data_ptr() or \
+        if ent is None or ent.wref() is None or ent.ver[1] != weight.data_ptr() or ent.dtype != weight.dtype or \
                 tuple(ent.out.shape[:1]) != ((weight.shape[1] if transpose else weight.shape[0]),):
             ent = _new_pack_entry(weight, tapmap, transpose, Kpad, fold, fat)
             self._store[key] = ent
@@ -415,25 +448,28 @@ def colsum(x2d_rows: int, x: torch.Tensor, C: int, out=None) -> torch.Tensor:
 
 # ----------------------------------------------------------------------------------------------------------------------
 class ToNHWC(torch.autograd.Function):
-    """[N,C,H,W] fp32 -> [N,H,W,Cp] bf16, optional per-channel (x - shift) * inv_scale (LPIPS ScalingLayer,
-    utils.py:70-71). Backward: NHWC bf16 grad -> NCHW fp32 (* inv_scale)."""
+    """[N,C,H,W] fp32 or bf16 -> [N,H,W,Cp] bf16, optional per-channel (x - shift) * inv_scale (LPIPS ScalingLayer,
+    utils.py:70-71). A bf16 input is read directly (no fp32 copy). Backward: NHWC bf16 grad -> NCHW fp32 (* inv_scale)."""
 
     @staticmethod
     def forward(ctx, x, shift, inv_scale, frame):
         require_cuda(x)
         x = x.detach()
-        if x.dtype != torch.float32 or not x.is_contiguous():
+        bf16 = x.dtype == torch.bfloat16
+        if bf16:
+            x = x.contiguous()
+        elif x.dtype != torch.float32 or not x.is_contiguous():
             x = x.float().contiguous()
         N, C, H, W = x.shape
         Cp = plans.cpad(C)
         if frame:  # zero-framed [N, H+2, W+2, Cp] for the "fat pixel" first-layer conv
             y = alloc_framed(N, H, W, Cp, x.device)
-            check(_L().vqb_nchw_to_nhwc_pad(ptr(x), ptr(y), N, C, H, W, Cp, 1, ptr(shift), ptr(inv_scale),
-                                            stream_ptr()), "nchw_to_nhwc_pad")
+            fn = _L().vqb_nchw_to_nhwc_pad_bf16 if bf16 else _L().vqb_nchw_to_nhwc_pad
+            check(fn(ptr(x), ptr(y), N, C, H, W, Cp, 1, ptr(shift), ptr(inv_scale), stream_ptr()), "nchw_to_nhwc_pad")
         else:
             y = torch.empty(N, H, W, Cp, device=x.device, dtype=torch.bfloat16)
-            check(_L().vqb_nchw_to_nhwc(ptr(x), ptr(y), N, C, H, W, Cp, ptr(shift), ptr(inv_scale), stream_ptr()),
-                  "nchw_to_nhwc")
+            fn = _L().vqb_nchw_to_nhwc_bf16 if bf16 else _L().vqb_nchw_to_nhwc
+            check(fn(ptr(x), ptr(y), N, C, H, W, Cp, ptr(shift), ptr(inv_scale), stream_ptr()), "nchw_to_nhwc")
         ctx.shape = (N, C, H, W, Cp)
         ctx.inv_scale, ctx.frame = inv_scale, frame
         return y
@@ -476,32 +512,36 @@ def fat_conv_enabled() -> bool:
         return False
     if _fat_state["ok"] is None:
         _fat_state["ok"] = False
+        # normal tensors even when the first caller runs under torch.inference_mode() (the pack cache reads _version)
         try:
-            g = torch.Generator(device="cuda").manual_seed(1)
-            x = torch.rand(2, 3, 16, 24, device="cuda", generator=g) - 0.5
-            w = torch.rand(64, 3, 3, 3, device="cuda", generator=g) - 0.5
-            c1, c2 = PackedCache(), PackedCache()
-            a = conv(ToNHWC.apply(x, None, None, False), w, None, c1, "s1")
-            b = conv(ToNHWC.apply(x, None, None, True), w, None, c2, "fat3")
-            torch.cuda.synchronize()
-            _fat_state["ok"] = bool(torch.allclose(a.float(), b.float(), rtol=2e-2, atol=2e-2))
+            with torch.inference_mode(False):
+                g = torch.Generator(device="cuda").manual_seed(1)
+                x = torch.rand(2, 3, 16, 24, device="cuda", generator=g) - 0.5
+                w = torch.rand(64, 3, 3, 3, device="cuda", generator=g) - 0.5
+                c1, c2 = PackedCache(), PackedCache()
+                a = conv(ToNHWC.apply(x, None, None, False), w, None, c1, "s1")
+                b = conv(ToNHWC.apply(x, None, None, True), w, None, c2, "fat3")
+                torch.cuda.synchronize()
+                _fat_state["ok"] = bool(torch.allclose(a.float(), b.float(), rtol=2e-2, atol=2e-2))
         except Exception:
             _fat_state["ok"] = False
     return _fat_state["ok"]
 
 
 def wavelet_to_nhwc(x: torch.Tensor, filt: torch.Tensor) -> torch.Tensor:
-    """[N,C,H,W] fp32 image -> [N,H/2,W/2,cpad(4C)] bf16: the wavelet front-end (utils.py:229-247) fused with the layout
-    conversion. Input-side op: the image is data, so there is no backward."""
+    """[N,C,H,W] fp32 or bf16 image -> [N,H/2,W/2,cpad(4C)] bf16: the wavelet front-end (utils.py:229-247) fused with the
+    layout conversion. Input-side op: the image is data, so there is no backward."""
     require_cuda(x)
     if x.requires_grad:
         raise RuntimeError("wavelet front-end: the input image must not require grad (input-side op without backward)")
-    x = x.detach().float().contiguous()
+    bf16 = x.dtype == torch.bfloat16
+    x = x.detach().contiguous() if bf16 else x.detach().float().contiguous()
     N, C, H, W = x.shape
     Cp = plans.cpad(4 * C)
     y = torch.empty(N, H // 2, W // 2, Cp, device=x.device, dtype=torch.bfloat16)
     f = filt.detach().to(device=x.device, dtype=torch.float32).reshape(4, 36).contiguous()
-    check(_L().vqb_wavelet_fwd(ptr(x), ptr(y), ptr(f), N, C, H, W, Cp, stream_ptr()), "wavelet_fwd")
+    fn = _L().vqb_wavelet_fwd_bf16 if bf16 else _L().vqb_wavelet_fwd
+    check(fn(ptr(x), ptr(y), ptr(f), N, C, H, W, Cp, stream_ptr()), "wavelet_fwd")
     return y
 
 
@@ -510,14 +550,19 @@ def to_nhwc(x, shift=None, inv_scale=None, frame=False):
 
 
 class ToNCHW(torch.autograd.Function):
-    """[N,H,W,Cp] bf16 -> [N,C,H,W] fp32 (module-boundary output when a caller wants the reference layout)."""
+    """[N,H,W,Cp] bf16 -> [N,C,H,W] fp32, or bf16 for a bf16 module (module-boundary output when a caller wants the
+    reference layout)."""
 
     @staticmethod
-    def forward(ctx, y, C):
+    def forward(ctx, y, C, dtype=torch.float32):
         N, H, W, Cp = y.shape
         y = y.contiguous()
-        x = torch.empty(N, C, H, W, device=y.device, dtype=torch.float32)
-        check(_L().vqb_nhwc_to_nchw(ptr(y), ptr(x), N, C, H, W, Cp, 0, stream_ptr()), "nhwc_to_nchw")
+        if dtype == torch.bfloat16:
+            x = torch.empty(N, C, H, W, device=y.device, dtype=torch.bfloat16)
+            check(_L().vqb_nhwc_to_nchw_bf16(ptr(y), ptr(x), N, C, H, W, Cp, stream_ptr()), "nhwc_to_nchw_bf16")
+        else:
+            x = torch.empty(N, C, H, W, device=y.device, dtype=torch.float32)
+            check(_L().vqb_nhwc_to_nchw(ptr(y), ptr(x), N, C, H, W, Cp, 0, stream_ptr()), "nhwc_to_nchw")
         ctx.shape = (N, C, H, W, Cp)
         return x
 
@@ -527,11 +572,12 @@ class ToNCHW(torch.autograd.Function):
         gx = gx.float().contiguous()
         gy = torch.empty(N, H, W, Cp, device=gx.device, dtype=torch.bfloat16)
         check(_L().vqb_nchw_to_nhwc(ptr(gx), ptr(gy), N, C, H, W, Cp, 0, 0, stream_ptr()), "nchw_to_nhwc")
-        return gy, None
+        return gy, None, None
 
 
-def to_nchw(y, C):
-    return ToNCHW.apply(y, C)
+def to_nchw(y, C, dtype=torch.float32):
+    """dtype: the dtype of the module's parameters (fp32 or bf16), which is what the reference returns."""
+    return ToNCHW.apply(y, C, dtype)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -541,7 +587,7 @@ class ConvFn(torch.autograd.Function):
     kind: "s1" (k x k stride 1 same), "s2" (Downsample: pad (0,1,0,1) + 3x3 stride 2), "patch" (k x k stride k).
     opts: relu (fused ReLU epilogue; the incoming gradient is then expected to be already gated by out > 0, which every
     consumer of a ReLU output in this package does), input_is_relu (gate the data gradient by x > 0 in the dgrad
-    epilogue), nchw_out (write fp32 [N,Cout,H,W] directly: encoder z / decoder image)."""
+    epilogue), nchw_out (write [N,Cout,H,W] in the weight's dtype, fp32 or bf16, directly: encoder z / decoder image)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, residual, cache, kind, relu, input_is_relu, nchw_out, want_stats=False,
@@ -574,9 +620,10 @@ class ConvFn(torch.autograd.Function):
             b = bias.detach()
             if b.dtype != torch.float32:
                 b = b.float()
-        if nchw_out:
-            out = torch.empty(N, Cout, g.Ho, g.Wo, device=x.device, dtype=torch.float32)
-            run_conv_gemm(g, x, wp, Cout, out, plans.nchw_strides(Cout, g.Ho, g.Wo), bias=b, relu=relu, out_f32=True)
+        if nchw_out:  # a bf16 module's z / image: the epilogue's strided bf16 store (out_f32 = 0, oc = H*W)
+            f32 = weight.dtype == torch.float32
+            out = torch.empty(N, Cout, g.Ho, g.Wo, device=x.device, dtype=torch.float32 if f32 else torch.bfloat16)
+            run_conv_gemm(g, x, wp, Cout, out, plans.nchw_strides(Cout, g.Ho, g.Wo), bias=b, relu=relu, out_f32=f32)
         else:
             alloc = torch.empty if Cop == Cout else torch.zeros
             out = alloc(N, g.Ho, g.Wo, Cop, device=x.device, dtype=torch.bfloat16)
@@ -601,6 +648,7 @@ class ConvFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout, _gstats=None):
         x, weight = ctx.saved_tensors
+        inference_only(weight)
         g, kind, cache = ctx.g, ctx.kind, ctx.cache
         N, _, _, Cp = x.shape
         H, W = ctx.HW
@@ -741,6 +789,7 @@ class UpConvFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout, _gstats=None):
         x, weight = ctx.saved_tensors
+        inference_only(weight)
         cache = ctx.cache
         N, h, w, Cp = x.shape
         Cout, Cin, KH, KW = weight.shape
@@ -828,6 +877,7 @@ class GroupNormSiLUFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gy, gskip=None):
         x, gamma, beta, mr = ctx.saved_tensors
+        inference_only(gamma, beta)
         N, H, W, C = x.shape
         if gy is None:  # only the skip output was used
             return (gskip, None, None, None, None, None, None, None, None)
