@@ -221,6 +221,75 @@ int vqb_wavelet_fwd_bf16(const void* x, void* y, const float* filt, int N, int C
 /* The encoder z / decoder image of a bf16 module come straight out of conv_out's epilogue as bf16 NCHW through
  * vqb_conv_gemm with out_f32 = 0 and NCHW output strides (oc = H*W): no separate conversion. */
 
+/*
+ * Video autoencoder (tae.py, TVAE), no-grad inference in fp32 or bf16 modules. Activations are NTHWC bf16 with C a
+ * multiple of 8; module-boundary tensors are NCTHW (the same memory as NCHW with H' = T*H, so the NCHW <-> NHWC
+ * conversions and the GroupNorm kernels above serve it unchanged, as do 1x1x1 convs through vqb_conv_gemm on the
+ * [N][T*H][W][C] view). Every entry point below validates its arguments (VQB_EINVAL) and fails with VQB_ENODEVICE
+ * without an sm_90 device.
+ */
+#define VQB_MAX_VIEWS_3D 8
+#define VQB_MAX_TAPS_3D 27
+
+/* A strided 5-D view [Nv][Tv][Hv][Wv][C] (channel stride 1) of an NTHWC bf16 tensor. */
+typedef struct VqbView3d {
+    int64_t offset;         /* element offset from the tensor base pointer */
+    int32_t Wv, Hv, Tv, Nv; /* extents */
+    int64_t sw, sh, st, sn; /* strides in elements (multiples of 8) */
+} VqbView3d;
+
+/* One filter tap: reads view `view` at (w + dw, h + dh, t + dt); out-of-range reads are zero. */
+typedef struct VqbTap3d {
+    int32_t view, dw, dh, dt;
+} VqbTap3d;
+
+/*
+ * 5-D implicit-GEMM convolution
+ *   out[n,t,h,w,co] = epi( sum_tap sum_c A_view(tap)[n, t+dt, h+dh, w+dw, c] * Wp[co][tap][c] ),
+ * epi = (+ bias[co] if VQB_EPI_BIAS) (+ res[voxel][co] if VQB_EPI_RES; bf16, same addressing as out). Other VQB_EPI_*
+ * flags are refused (inference takes the separate, deterministic GroupNorm statistics pass). Output stores:
+ *   out_f32 = 0, oc = 1: bf16 NTHWC with any voxel strides (on, ot, oh, ow multiples of 8; the folded up-sampling
+ *                        writes phase sub-grids this way);
+ *   otherwise          : strided fp32 (out_f32 = 1) or bf16 at out + n*on + t*ot + h*oh + w*ow + c*oc (NCTHW module
+ *                        boundary).
+ * Covers the 27-tap 3x3x3 stride-1 conv, the (0,1,0,1,0,1)-padded 3x3x3 stride-2 Downsample conv (8 parity views; the
+ * pad is the TMA zero fill), and one phase of the nearest-x2 up-sampling folded into its 3x3x3 conv (8 taps of
+ * pre-summed weights over the low-resolution input). Replaces nn.Conv3d at tae.py:66-78 (ResnetBlock conv1 / conv2),
+ * :96-104 (Downsample), :110-116 (Upsample, with the F.interpolate), :136-138 and :165-167 (Encoder conv_in /
+ * conv_out), :208-210 and :233 (Decoder conv_in / conv_out). The 1x1x1 convs (tae.py:22-23 qkv / proj_out,
+ * :76-78 nin_shortcut) run through vqb_conv_gemm on the [N][T*H][W][C] view.
+ */
+typedef struct VqbConv3dDesc {
+    int32_t C;          /* channels of the A tensor = K per tap (multiple of 8)     */
+    int32_t Cout;       /* GEMM N                                                   */
+    int32_t N, T, H, W; /* output voxel grid, GEMM M = N*T*H*W                      */
+    int32_t nviews, ntaps;
+    int32_t flags;   /* VQB_EPI_BIAS | VQB_EPI_RES                               */
+    int32_t out_f32; /* 0: out is bf16, 1: out is fp32                           */
+    int64_t on, ot, oh, ow, oc; /* out element address = out + n*on + t*ot + h*oh + w*ow + c*oc */
+    VqbView3d views[VQB_MAX_VIEWS_3D];
+    VqbTap3d taps[VQB_MAX_TAPS_3D];
+} VqbConv3dDesc;
+
+int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void* w_packed /* bf16 [Cout][ntaps*C] */,
+                    const float* bias, const void* res, void* out, void* stream);
+
+/*
+ * Attention core of tae.AttnBlock (tae.py:26-51: 8 heads of C/8 channels, F.scaled_dot_product_attention with its
+ * default scale 1/sqrt(head_dim)): qkv [N][T][3C] bf16 (q | k | v channel blocks, head h owns channels
+ * h*head_dim .. of each block) -> out [N][T][C] bf16; lse [N][C/head_dim][T] fp32. head_dim is 32 or 64; any other
+ * value is refused with a message naming it. vqb_attn_fwd is this with head_dim = 64.
+ */
+int vqb_attn_fwd_hd(const void* qkv, void* out, float* lse, int N, int T, int C, int head_dim, void* stream);
+
+/*
+ * Reparameterisation of tae.DiagonalGaussian (tae.py:259-264): z [N][2Z][S] (NCTHW, S = T*H*W; mean = channels 0..Z-1,
+ * logvar = Z..2Z-1) and eps [N][Z][S] -> out [N][Z][S] = mean + exp(0.5 * max(logvar, -3)) * eps, computed in fp32 and
+ * rounded once. bf16 = 1: z, eps and out are bf16, else fp32. eps is drawn by the caller (torch.randn_like(mean), the
+ * reference's own call, so a seeded run consumes the same CUDA RNG stream).
+ */
+int vqb_gauss_reparam(const void* z, const void* eps, void* out, int N, int Z, int64_t S, int bf16, void* stream);
+
 /* nearest-neighbour x2 up-sampling (ae.py:165) and its backward (2x2 sum), bf16 NHWC */
 int vqb_upsample2x_fwd(const void* x, void* y, int N, int H, int W, int C, void* stream);
 int vqb_upsample2x_bwd(const void* dy, void* dx, int N, int H, int W, int C, void* stream);

@@ -11,6 +11,17 @@ checkpoint), eagerly launched and replayed as one CUDA graph, beside the eager P
 encoder_forward / decoder_forward in bf16 with cuDNN (cudnn.benchmark on): the model card's `.bfloat16()` arithmetic.
 Prints one JSON line: images/s graphed and eagerly launched, peak allocated memory, the peer, and the card's name and
 power limit read in the same run. --dump-outputs DIR writes the graphed run's outputs as float32 DIR/<name>.npy.
+
+--frames T times the video autoencoder (tae.TVAE, ch_mult 1,2,4,4, num_res_blocks 2, z_channels 16) on a
+(batch, 3, T, res, res) clip instead, for example
+
+    python tools/infer_bench.py --frames 48 --res 256 --ch 64 --infer reconstruct --dtype bf16
+
+T, H and W must be divisible by 8. reconstruct is TVAE.forward (encoder, the sampling DiagonalGaussian, decoder); the
+CUDA graph captures its torch.randn_like too. The peer is oracle/tae_oracle.py in bf16 with cuDNN (cudnn.benchmark on).
+The line reports videos/s and frames/s, and the forward's algorithmic FLOPs counted from the plan shapes
+(tae_oracle.flops: convs with the folded up-sampling, attention matmuls), so that "tflops_per_s" is a whole-forward
+rate, not a kernel's.
 """
 from __future__ import annotations
 
@@ -74,8 +85,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--no-eager", action="store_true", help="skip the PyTorch peer")
     ap.add_argument("--dump-outputs", default=None, metavar="DIR")
+    ap.add_argument("--frames", type=int, default=0, help="time the video autoencoder (tae.TVAE) on T frames")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "infer_bench.py needs a CUDA (sm_90a) device: there is no CPU path"
+    if args.frames:
+        return video_main(args)
 
     import ae
     import ops
@@ -156,6 +170,91 @@ def main():
             line["eager_peer"] = {"value": B / (ms_p * 1e-3), "ms_per_call": ms_p, "peak_mem_gib": peak_p / 2 ** 30,
                                   "impl": "oracle encoder_forward / decoder_forward (reference arithmetic) in bf16, "
                                           "cuDNN, cudnn.benchmark=True, no autocast"}
+            line["vs_eager_peer"] = line["value"] / line["eager_peer"]["value"]
+        except torch.OutOfMemoryError:
+            line["eager_peer"] = {"unavailable": "out of memory"}
+    print(json.dumps(line), flush=True)
+
+
+def video_main(args):
+    import tae
+    from oracle import seeded
+    from oracle import tae_oracle as TO
+
+    H, W = parse_res(args.res)
+    T, B = args.frames, args.batch
+    cfg = TO.TAEConfig(ch=args.ch, ch_mult=(1, 2, 4, 4), num_res_blocks=2, z_channels=16, resolution=256)
+    f = 2 ** (len(cfg.ch_mult) - 1)
+    if T % f or H % f or W % f:
+        raise SystemExit(f"--frames {T} --res {H}x{W}: T, H and W must be divisible by {f}")
+    dtype = torch.bfloat16 if args.dtype == "bf16" else torch.float32
+    vae = tae.TVAE(**cfg.kwargs())
+    tag = f"infer_bench/tae_ch{cfg.ch}"
+    sd = seeded.fill_state_dict(vae.state_dict(), tag)
+    vae.load_state_dict(sd)
+    vae = vae.cuda().to(dtype).eval()
+    x = seeded.tensor(tag + "/x", (B, 3, T, H, W), 1.0, "uniform").cuda().to(dtype)
+    zin = seeded.tensor(tag + "/z", (B, cfg.z_channels, T // f, H // f, W // f), 1.0).cuda().to(dtype)
+
+    def ours():
+        if args.infer == "encode":
+            return {"z": vae.encoder(x)}
+        if args.infer == "decode":
+            return {"video": vae.decoder(zin)}
+        decz, z = vae(x)
+        return {"z": z, "video": decz}
+
+    base = torch.cuda.memory_allocated()
+    with torch.no_grad():
+        ms_eager, peak_eager, _ = timed(ours, args.steps, args.warmup)  # also fills the pack caches
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            ours()
+        torch.cuda.current_stream().wait_stream(s)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            static = ours()
+        ms_graph, _, _ = timed(lambda: graph.replay(), args.steps, args.warmup)
+    if args.dump_outputs:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k, v in static.items():
+            np.save(os.path.join(args.dump_outputs, k + ".npy"), v.detach().float().cpu().numpy())
+    flops = TO.flops(cfg, B, T, H, W, args.infer)
+    line = {"metric": "videos/sec", "unit": "videos/s", "model": "tae.TVAE", "infer": args.infer, "dtype": args.dtype,
+            "config": {"ch": cfg.ch, "ch_mult": list(cfg.ch_mult), "num_res_blocks": cfg.num_res_blocks,
+                       "z_channels": cfg.z_channels, "frames": T, "res": [H, W], "batch": B},
+            "value": B / (ms_graph * 1e-3), "frames_per_s": B * T / (ms_graph * 1e-3), "ms_per_call_graph": ms_graph,
+            "eager_launch": {"value": B / (ms_eager * 1e-3), "frames_per_s": B * T / (ms_eager * 1e-3),
+                             "ms_per_call": ms_eager},
+            "algorithmic_tflop": flops / 1e12, "tflops_per_s_graph": flops / (ms_graph * 1e-3) / 1e12,
+            "peak_mem_gib": peak_eager / 2 ** 30, "weights_and_inputs_gib": base / 2 ** 30,
+            "gpu": card()}
+    del graph, static
+    if not args.no_eager:
+        sdb = {k: v.cuda().bfloat16() for k, v in sd.items()}
+        xb, zb = x.bfloat16(), zin.bfloat16()
+        torch.backends.cudnn.benchmark = True
+
+        def peer():
+            if args.infer == "encode":
+                return TO.encoder_forward(sdb, xb, cfg)
+            if args.infer == "decode":
+                return TO.decoder_forward(sdb, zb, cfg)
+            z = TO.encoder_forward(sdb, xb, cfg)
+            return TO.decoder_forward(sdb, TO.reg(z, torch.randn_like(z.chunk(2, 1)[0])), cfg), z
+
+        try:
+            with torch.no_grad():
+                ms_p, peak_p, _ = timed(peer, args.steps, args.warmup)
+            line["eager_peer"] = {"value": B / (ms_p * 1e-3), "frames_per_s": B * T / (ms_p * 1e-3),
+                                  "ms_per_call": ms_p, "peak_mem_gib": peak_p / 2 ** 30,
+                                  "tflops_per_s": flops / (ms_p * 1e-3) / 1e12,
+                                  "impl": "oracle tae_oracle encoder_forward / reg / decoder_forward (reference "
+                                          "arithmetic: literal nearest-x2 + conv3d) in bf16, cuDNN, "
+                                          "cudnn.benchmark=True, no autocast"}
             line["vs_eager_peer"] = line["value"] / line["eager_peer"]["value"]
         except torch.OutOfMemoryError:
             line["eager_peer"] = {"unavailable": "out of memory"}

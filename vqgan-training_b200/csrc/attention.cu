@@ -25,19 +25,24 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], 
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// 64 x 64 bf16 tile: rows row0.. of a [T][ld] matrix (column offset already applied to src) -> dst[64][kLD]; rows >= T zero.
+// 64 x COLS bf16 tile: rows row0.. of a [T][ld] matrix (column offset already applied to src) -> dst[64][kLD]; rows >= T
+// zero.
+template <int COLS = 64>
 __device__ __forceinline__ void load_tile(__nv_bfloat16* dst, const __nv_bfloat16* src, int64_t ld, int row0, int T) {
-    for (int i = threadIdx.x; i < 64 * 8; i += blockDim.x) {
-        const int r = i >> 3, v = i & 7;
+    constexpr int kV = COLS / 8;  // 16-byte vectors per row
+    for (int i = threadIdx.x; i < 64 * kV; i += blockDim.x) {
+        const int r = i / kV, v = i % kV;
         uint4 u = make_uint4(0, 0, 0, 0);
         if (row0 + r < T) u = __ldg(reinterpret_cast<const uint4*>(src + static_cast<int64_t>(row0 + r) * ld + v * 8));
         *reinterpret_cast<uint4*>(dst + r * kLD + v * 8) = u;
     }
 }
 // same tile stored transposed: dst[col][row]
+template <int COLS = 64>
 __device__ __forceinline__ void load_tile_t(__nv_bfloat16* dst, const __nv_bfloat16* src, int64_t ld, int row0, int T) {
-    for (int i = threadIdx.x; i < 64 * 8; i += blockDim.x) {
-        const int r = i >> 3, v = i & 7;
+    constexpr int kV = COLS / 8;
+    for (int i = threadIdx.x; i < 64 * kV; i += blockDim.x) {
+        const int r = i / kV, v = i % kV;
         uint4 u = make_uint4(0, 0, 0, 0);
         if (row0 + r < T) u = __ldg(reinterpret_cast<const uint4*>(src + static_cast<int64_t>(row0 + r) * ld + v * 8));
         const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(&u);
@@ -45,24 +50,27 @@ __device__ __forceinline__ void load_tile_t(__nv_bfloat16* dst, const __nv_bfloa
         for (int j = 0; j < 8; ++j) dst[(v * 8 + j) * kLD + r] = e[j];
     }
 }
-// A fragments (16 rows of this warp x 64 cols) of a [64][kLD] smem tile
-__device__ __forceinline__ void load_a_frags(const __nv_bfloat16* s, int warp, int lane, uint32_t (&a)[4][4]) {
+// A fragments (16 rows of this warp x 16*KS cols) of a [64][kLD] smem tile
+template <int KS = 4>
+__device__ __forceinline__ void load_a_frags(const __nv_bfloat16* s, int warp, int lane, uint32_t (&a)[KS][4]) {
     const int r = warp * 16 + (lane >> 2), c = (lane & 3) * 2;
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
+    for (int ks = 0; ks < KS; ++ks) {
         a[ks][0] = *reinterpret_cast<const uint32_t*>(s + r * kLD + ks * 16 + c);
         a[ks][1] = *reinterpret_cast<const uint32_t*>(s + (r + 8) * kLD + ks * 16 + c);
         a[ks][2] = *reinterpret_cast<const uint32_t*>(s + r * kLD + ks * 16 + c + 8);
         a[ks][3] = *reinterpret_cast<const uint32_t*>(s + (r + 8) * kLD + ks * 16 + c + 8);
     }
 }
-// acc[nt] += A(16 x 64) * B where B[k][n] = s[n][k] (s is a [64 n][kLD] smem tile, k contiguous)
-__device__ __forceinline__ void mma_a_bT(float (&acc)[8][4], const uint32_t (&a)[4][4], const __nv_bfloat16* s, int lane) {
+// acc[nt] += A(16 x 16*KS) * B where B[k][n] = s[n][k] (s is a [8*NT n][kLD] smem tile, k contiguous)
+template <int KS = 4, int NT = 8>
+__device__ __forceinline__ void mma_a_bT(float (&acc)[NT][4], const uint32_t (&a)[KS][4], const __nv_bfloat16* s,
+                                         int lane) {
     const int n = lane >> 2, c = (lane & 3) * 2;
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
+    for (int ks = 0; ks < KS; ++ks)
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
+        for (int nt = 0; nt < NT; ++nt) {
             const uint32_t b0 = *reinterpret_cast<const uint32_t*>(s + (nt * 8 + n) * kLD + ks * 16 + c);
             const uint32_t b1 = *reinterpret_cast<const uint32_t*>(s + (nt * 8 + n) * kLD + ks * 16 + c + 8);
             mma16816(acc[nt], a[ks], b0, b1);
@@ -80,9 +88,13 @@ __device__ __forceinline__ void acc_to_a(const float (&p)[8][4], uint32_t (&a)[4
 }
 
 // ------------------------------------------------------------------------------------------------ forward
+// HD: head dim (64: ae.AttnBlock and tae heads of 64; 32: tae.AttnBlock at ch = 64). Q.K^T runs HD/16 k-steps over
+// 8 key n-tiles; P.V runs 4 key k-steps over HD/8 output n-tiles.
+template <int HD>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __restrict__ qkv,
                                                        __nv_bfloat16* __restrict__ out, float* __restrict__ lse, int T,
                                                        int C, float scale) {
+    constexpr int kKS = HD / 16, kNO = HD / 8;
     __shared__ __align__(16) __nv_bfloat16 sQ[64 * kLD];
     __shared__ __align__(16) __nv_bfloat16 sK[64 * kLD];
     __shared__ __align__(16) __nv_bfloat16 sVt[64 * kLD];
@@ -90,28 +102,28 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __re
     const int q0 = blockIdx.x * kTQ, h = blockIdx.y, n = blockIdx.z, heads = gridDim.y;
     const int64_t ld = 3 * static_cast<int64_t>(C);
     const __nv_bfloat16* base = qkv + static_cast<int64_t>(n) * T * ld;
-    load_tile(sQ, base + h * kHD, ld, q0, T);
+    load_tile<HD>(sQ, base + h * HD, ld, q0, T);
     __syncthreads();
-    uint32_t qa[4][4];
-    load_a_frags(sQ, warp, lane, qa);
+    uint32_t qa[kKS][4];
+    load_a_frags<kKS>(sQ, warp, lane, qa);
     float m_i[2] = {-INFINITY, -INFINITY}, l_i[2] = {0.f, 0.f};
-    float o[8][4];
+    float o[kNO][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < kNO; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) o[i][j] = 0.f;
     const int nkt = (T + 63) / 64;
     for (int kt = 0; kt < nkt; ++kt) {
         __syncthreads();
-        load_tile(sK, base + C + h * kHD, ld, kt * 64, T);
-        load_tile_t(sVt, base + 2 * C + h * kHD, ld, kt * 64, T);
+        load_tile<HD>(sK, base + C + h * HD, ld, kt * 64, T);
+        load_tile_t<HD>(sVt, base + 2 * C + h * HD, ld, kt * 64, T);
         __syncthreads();
         float s[8][4];
 #pragma unroll
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-        mma_a_bT(s, qa, sK, lane);
+        mma_a_bT<kKS, 8>(s, qa, sK, lane);
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt)
@@ -148,12 +160,12 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __re
             l_i[r] = l_i[r] * alpha[r] + rs[r];
         }
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
+        for (int nt = 0; nt < kNO; ++nt)
 #pragma unroll
             for (int j = 0; j < 4; ++j) o[nt][j] *= alpha[j >> 1];
         uint32_t pa[4][4];
         acc_to_a(s, pa);
-        mma_a_bT(o, pa, sVt, lane);  // B[k=key][n=d] = Vt[d][key]
+        mma_a_bT<4, kNO>(o, pa, sVt, lane);  // B[k=key][n=d] = Vt[d][key]
     }
     const int r0 = q0 + warp * 16 + (lane >> 2);
 #pragma unroll
@@ -161,9 +173,9 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __re
         const int q = r0 + r * 8;
         if (q < T) {
             const float inv = 1.f / l_i[r];
-            __nv_bfloat16* op = out + (static_cast<int64_t>(n) * T + q) * C + h * kHD + (lane & 3) * 2;
+            __nv_bfloat16* op = out + (static_cast<int64_t>(n) * T + q) * C + h * HD + (lane & 3) * 2;
 #pragma unroll
-            for (int nt = 0; nt < 8; ++nt)
+            for (int nt = 0; nt < kNO; ++nt)
                 *reinterpret_cast<uint32_t*>(op + nt * 8) = pack_bf16x2(o[nt][2 * r] * inv, o[nt][2 * r + 1] * inv);
             if ((lane & 3) == 0) lse[(static_cast<int64_t>(n) * heads + h) * T + q] = m_i[r] + __logf(l_i[r]);
         }
@@ -357,8 +369,34 @@ int vqb_attn_fwd(const void* qkv, void* out, float* lse, int N, int T, int C, vo
     VQB_CHECK(qkv && out && lse, "vqb_attn_fwd: null pointer");
     VQB_CHECK(C % 64 == 0 && T > 0 && N > 0, "vqb_attn_fwd: C=%d must be a multiple of the head dim 64", C);
     dim3 grid((T + 63) / 64, C / 64, N);
-    attn_fwd_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+    attn_fwd_kernel<64><<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(qkv), static_cast<__nv_bfloat16*>(out), lse, T, C, 0.125f);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+// tae.AttnBlock (tae.py:26-51): heads of head_dim = C/8 channels, SDPA's default scale 1/sqrt(head_dim). Replaces
+// F.scaled_dot_product_attention + the einops rearranges at tae.py:31-50.
+int vqb_attn_fwd_hd(const void* qkv, void* out, float* lse, int N, int T, int C, int head_dim, void* stream) {
+    VQB_CHECK(qkv && out && lse, "vqb_attn_fwd_hd: null pointer");
+    VQB_CHECK(head_dim == 32 || head_dim == 64,
+              "vqb_attn_fwd_hd: head_dim=%d is not supported (heads of 32 or 64 channels only)", head_dim);
+    VQB_CHECK(C > 0 && C % head_dim == 0 && T > 0 && N > 0,
+              "vqb_attn_fwd_hd: C=%d must be a positive multiple of head_dim %d (T=%d N=%d)", C, head_dim, T, N);
+    VQB_CHECK(((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out)) & 15u) == 0 &&
+                  (reinterpret_cast<uintptr_t>(lse) & 3u) == 0,
+              "vqb_attn_fwd_hd: qkv / out must be 16-byte aligned");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_attn_fwd_hd: current device is not sm_90");
+    dim3 grid((T + 63) / 64, C / head_dim, N);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (head_dim == 64)
+        attn_fwd_kernel<64><<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv),
+                                                   static_cast<__nv_bfloat16*>(out), lse, T, C, 0.125f);
+    else
+        attn_fwd_kernel<32><<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv),
+                                                   static_cast<__nv_bfloat16*>(out), lse, T, C,
+                                                   0.17677669529663687f);  // 1/sqrt(32)
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;

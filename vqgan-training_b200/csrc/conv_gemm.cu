@@ -16,6 +16,8 @@
 #include "common.cuh"
 #include "ptx.cuh"
 
+#include <cstring>
+
 namespace vqb {
 
 constexpr int kBlockM = 128;
@@ -26,6 +28,8 @@ constexpr int kMaxStages = 8;
 constexpr int kConsumerWarps = 8;
 
 struct alignas(64) ConvParams {
+    static constexpr int kRank = 4;  // NHWC activations, 4-D TMA boxes [64 ch][bw][bh][bn]
+    static constexpr int kViews = VQB_MAX_VIEWS;
     CUtensorMap amap[VQB_MAX_VIEWS];
     CUtensorMap bmap;
     int32_t tap_view[VQB_MAX_TAPS];
@@ -56,8 +60,42 @@ struct alignas(64) ConvParams {
     int32_t gn_G, gn_lcpg;  // groups, log2(channels per group)
 };
 
-template <int BN>
-__global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
+// The 3-D (video) form: NTHWC activations, 5-D TMA boxes [64 ch][bw][bh][bt][bn], up to 27 taps over up to 8 views.
+// Inference only: the epilogue has bias and residual; the statistics / GroupNorm-backward / ReLU / mask fields exist so
+// that the kernel body compiles for both ranks, and are always zero here (the kernel tests kRank before reading them).
+struct alignas(64) Conv3dParams {
+    static constexpr int kRank = 5;
+    static constexpr int kViews = VQB_MAX_VIEWS_3D;
+    CUtensorMap amap[VQB_MAX_VIEWS_3D];
+    CUtensorMap bmap;
+    int32_t tap_view[VQB_MAX_TAPS_3D];
+    int32_t tap_dw[VQB_MAX_TAPS_3D];
+    int32_t tap_dh[VQB_MAX_TAPS_3D];
+    int32_t tap_dt[VQB_MAX_TAPS_3D];
+    int32_t ntaps, kchunks, C, Cout;
+    int32_t N, T, H, W;
+    int32_t lbw, lbh, lbt, lbn;
+    int32_t tiles_w, tiles_h, tiles_t;
+    int32_t n_tiles, total_tiles;
+    int32_t stages, do_stats;
+    int32_t flags, out_f32;
+    int64_t on, ot, oh, ow, oc;
+    void* out;
+    const void* res;
+    const void* mask;
+    const float* bias;
+    float* stats;
+    const __nv_bfloat16* gn_x;
+    const float* gn_mr;
+    const float* gn_gamma;
+    const float* gn_beta;
+    float* gn_cs;
+    int32_t gn_G, gn_lcpg;
+};
+
+template <int BN, class P>
+__global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ P p) {
+    constexpr bool kR5 = P::kRank == 5;
     extern __shared__ uint8_t smem_raw[];
     constexpr uint32_t kBBytes = BN * kBlockK * 2;
     constexpr uint32_t kStageBytes = kABytes + kBBytes;  // a multiple of 2 KB: every tile stays 1024-B aligned
@@ -72,7 +110,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const uint32_t lane = threadIdx.x & 31u;
 
     if (threadIdx.x == 0) {
-        for (int v = 0; v < VQB_MAX_VIEWS; ++v) {
+        for (int v = 0; v < P::kViews; ++v) {
             bool used = false;
             for (int t = 0; t < p.ntaps; ++t) used |= (p.tap_view[t] == v);
             if (used) tma_prefetch_desc(&p.amap[v]);
@@ -96,7 +134,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                 const int m_tile = tile / p.n_tiles;
                 const int tw = m_tile % p.tiles_w;
                 const int th = (m_tile / p.tiles_w) % p.tiles_h;
-                const int tn = m_tile / (p.tiles_w * p.tiles_h);
+                int tt = 0, tn;
+                if constexpr (kR5) {
+                    tt = (m_tile / (p.tiles_w * p.tiles_h)) % p.tiles_t;
+                    tn = m_tile / (p.tiles_w * p.tiles_h * p.tiles_t);
+                } else {
+                    tn = m_tile / (p.tiles_w * p.tiles_h);
+                }
                 const int w0 = tw << p.lbw, h0 = th << p.lbh, n0 = tn << p.lbn;
                 const int ncol0 = n_tile * BN;
                 for (int t = 0; t < p.ntaps; ++t) {
@@ -104,8 +148,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                         mbar_wait(&empty[stage], phase ^ 1);
                         uint8_t* a_dst = base + stage * kStageBytes;
                         mbar_arrive_expect_tx(&full[stage], kStageBytes);
-                        tma_load_4d(&p.amap[p.tap_view[t]], &full[stage], a_dst, kc * kBlockK, w0 + p.tap_dw[t],
-                                    h0 + p.tap_dh[t], n0);
+                        if constexpr (kR5)
+                            tma_load_5d(&p.amap[p.tap_view[t]], &full[stage], a_dst, kc * kBlockK, w0 + p.tap_dw[t],
+                                        h0 + p.tap_dh[t], (tt << p.lbt) + p.tap_dt[t], n0);
+                        else
+                            tma_load_4d(&p.amap[p.tap_view[t]], &full[stage], a_dst, kc * kBlockK, w0 + p.tap_dw[t],
+                                        h0 + p.tap_dh[t], n0);
                         tma_load_2d(&p.bmap, &full[stage], a_dst + kABytes, t * p.C + kc * kBlockK, ncol0);
                         if (++stage == stages) {
                             stage = 0;
@@ -124,10 +172,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const uint32_t ctid = threadIdx.x - 128;  // 0..255
     const uint32_t ring = smem_u32(base);
     const bool has_bias = p.flags & VQB_EPI_BIAS, has_res = p.flags & VQB_EPI_RES;
-    const bool do_relu = p.flags & VQB_EPI_RELU, has_mask = p.flags & VQB_EPI_MASK;
+    const bool do_relu = !kR5 && (p.flags & VQB_EPI_RELU), has_mask = !kR5 && (p.flags & VQB_EPI_MASK);
     const bool vec_path = (p.oc == 1) && (p.out_f32 == 0);
-    const bool do_gn = p.gn_cs != nullptr;
-    const bool reduce = p.do_stats || do_gn;
+    const bool do_gn = !kR5 && p.gn_cs != nullptr;
+    const bool reduce = !kR5 && (p.do_stats || do_gn);
     const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.res);
     const __nv_bfloat16* mask = reinterpret_cast<const __nv_bfloat16*>(p.mask);
     float acc[BN / 2];
@@ -166,7 +214,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         const int m_tile = tile / p.n_tiles;
         const int tw = m_tile % p.tiles_w;
         const int th = (m_tile / p.tiles_w) % p.tiles_h;
-        const int tn = m_tile / (p.tiles_w * p.tiles_h);
+        int tt = 0, tn;
+        if constexpr (kR5) {
+            tt = (m_tile / (p.tiles_w * p.tiles_h)) % p.tiles_t;
+            tn = m_tile / (p.tiles_w * p.tiles_h * p.tiles_t);
+        } else {
+            tn = m_tile / (p.tiles_w * p.tiles_h);
+        }
         const int col0 = n_tile * BN;
         int64_t pix[2];
         bool valid[2];
@@ -176,10 +230,20 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             const uint32_t row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;  // row of the 128-pixel box
             const int w = (tw << p.lbw) + static_cast<int>(row & ((1u << p.lbw) - 1));
             const int h = (th << p.lbh) + static_cast<int>((row >> p.lbw) & ((1u << p.lbh) - 1));
-            const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh));
-            valid[i] = (w < p.W) && (h < p.H) && (n < p.N);
-            img[i] = n;
-            pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh + static_cast<int64_t>(w) * p.ow;
+            if constexpr (kR5) {  // row = w + bw * (h + bh * (t + bt * n)) of the 128-voxel box
+                const int t = (tt << p.lbt) + static_cast<int>((row >> (p.lbw + p.lbh)) & ((1u << p.lbt) - 1));
+                const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh + p.lbt));
+                valid[i] = (w < p.W) && (h < p.H) && (t < p.T) && (n < p.N);
+                img[i] = n;
+                pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(t) * p.ot +
+                         static_cast<int64_t>(h) * p.oh + static_cast<int64_t>(w) * p.ow;
+            } else {
+                const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh));
+                valid[i] = (w < p.W) && (h < p.H) && (n < p.N);
+                img[i] = n;
+                pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh +
+                         static_cast<int64_t>(w) * p.ow;
+            }
         }
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
@@ -303,17 +367,18 @@ static int fill_views(const VqbView* views, int nviews, const void* a, int C, in
     return VQB_OK;
 }
 
-template <int BN>
-static int launch_conv(const ConvParams& p, void* stream) {
+template <int BN, class P>
+static int launch_conv(const P& p, void* stream) {
     constexpr size_t stage_bytes = kABytes + BN * kBlockK * 2;
     const size_t smem = 1024 + p.stages * stage_bytes + kConsumerWarps * BN * 2 * sizeof(float) + 2 * 8 * p.stages;
     static bool attr_set = false;
     if (!attr_set) {
-        VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      227 * 1024));
         attr_set = true;
     }
     const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-    conv_gemm_kernel<BN><<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
+    conv_gemm_kernel<BN, P><<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
     VQB_CUDA(cudaGetLastError());
     return VQB_OK;
 }
@@ -462,6 +527,126 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     }
     int rc = fill_views(d->views, d->nviews, a, d->C, p.lbw, p.lbh, p.lbn, p.amap);
     if (rc != VQB_OK) return rc;
+    {
+        const uint64_t ktot = static_cast<uint64_t>(d->ntaps) * d->C;
+        uint64_t dims[2] = {ktot, static_cast<uint64_t>(d->Cout)};
+        uint64_t str[1] = {ktot * 2};
+        uint32_t box[2] = {kBlockK, static_cast<uint32_t>(block_n)};
+        rc = encode_tmap_bf16(&p.bmap, w_packed, 2, dims, str, box, 128);
+        if (rc != VQB_OK) return rc;
+    }
+    switch (block_n) {
+        case 16: rc = launch_conv<16>(p, stream); break;
+        case 32: rc = launch_conv<32>(p, stream); break;
+        case 64: rc = launch_conv<64>(p, stream); break;
+        default: rc = launch_conv<128>(p, stream); break;
+    }
+    if (rc != VQB_OK) return rc;
+    count_launch();
+    return VQB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// 3-D (video) convolution: the same kernel over NTHWC activations with 5-D TMA boxes (tae.py call sites in vqb200.h).
+extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void* w_packed, const float* bias,
+                               const void* res, void* out, void* stream) {
+    VQB_CHECK(d && a && w_packed && out, "vqb_conv3d_gemm: null pointer");
+    VQB_CHECK(d->C > 0 && d->C % 8 == 0, "vqb_conv3d_gemm: C=%d must be a positive multiple of 8", d->C);
+    VQB_CHECK(d->Cout > 0 && d->N > 0 && d->T > 0 && d->H > 0 && d->W > 0, "vqb_conv3d_gemm: bad extents");
+    VQB_CHECK(d->ntaps >= 1 && d->ntaps <= VQB_MAX_TAPS_3D && d->nviews >= 1 && d->nviews <= VQB_MAX_VIEWS_3D,
+              "vqb_conv3d_gemm: ntaps=%d nviews=%d out of range", d->ntaps, d->nviews);
+    VQB_CHECK((d->flags & ~(VQB_EPI_BIAS | VQB_EPI_RES)) == 0,
+              "vqb_conv3d_gemm: flags 0x%x: only VQB_EPI_BIAS and VQB_EPI_RES are supported", d->flags);
+    VQB_CHECK(d->out_f32 == 0 || d->out_f32 == 1, "vqb_conv3d_gemm: out_f32 must be 0 or 1");
+    if (d->flags & VQB_EPI_BIAS)
+        VQB_CHECK(bias != nullptr && (reinterpret_cast<uintptr_t>(bias) & 15u) == 0,
+                  "vqb_conv3d_gemm: VQB_EPI_BIAS needs a 16-byte aligned bias pointer");
+    if (d->flags & VQB_EPI_RES) VQB_CHECK(res != nullptr, "vqb_conv3d_gemm: VQB_EPI_RES without res");
+    VQB_CHECK(d->on >= 0 && d->ot >= 0 && d->oh >= 0 && d->ow >= 0 && d->oc > 0,
+              "vqb_conv3d_gemm: output strides must be non-negative (oc > 0)");
+    if (d->oc == 1 && !d->out_f32) {
+        VQB_CHECK(d->on % 8 == 0 && d->ot % 8 == 0 && d->oh % 8 == 0 && d->ow % 8 == 0 &&
+                      (reinterpret_cast<uintptr_t>(out) & 15u) == 0 && (reinterpret_cast<uintptr_t>(res) & 3u) == 0,
+                  "vqb_conv3d_gemm: NTHWC bf16 output needs 16-byte aligned voxel rows");
+    } else {
+        VQB_CHECK((reinterpret_cast<uintptr_t>(out) & (d->out_f32 ? 3u : 1u)) == 0 &&
+                      (reinterpret_cast<uintptr_t>(res) & 1u) == 0,
+                  "vqb_conv3d_gemm: misaligned output / residual");
+    }
+    for (int v = 0; v < d->nviews; ++v) {
+        const VqbView3d& vw = d->views[v];
+        VQB_CHECK(vw.offset >= 0 && vw.Wv > 0 && vw.Hv > 0 && vw.Tv > 0 && vw.Nv > 0 && vw.sw > 0 && vw.sw % 8 == 0 &&
+                      vw.sh > 0 && vw.sh % 8 == 0 && vw.st > 0 && vw.st % 8 == 0 && vw.sn > 0 && vw.sn % 8 == 0,
+                  "vqb_conv3d_gemm: view %d has bad extents / strides (strides must be positive multiples of 8)", v);
+    }
+    for (int t = 0; t < d->ntaps; ++t)
+        VQB_CHECK(d->taps[t].view >= 0 && d->taps[t].view < d->nviews, "vqb_conv3d_gemm: tap %d view out of range", t);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_conv3d_gemm: current device is not sm_90");
+
+    Conv3dParams p;
+    memset(&p, 0, sizeof(p));  // statistics / GroupNorm / mask fields stay zero (rank-5 epilogue: bias + residual)
+    const int block_n = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : (d->Cout > 16 ? 32 : 16));
+    p.n_tiles = (d->Cout + block_n - 1) / block_n;
+    // voxel box per CTA tile: 128 output voxels, as wide as the video (<= 128), then as tall, then as deep, then across
+    // videos
+    uint32_t bw = next_pow2(d->W);
+    if (bw > 128) bw = 128;
+    uint32_t bh = next_pow2(d->H);
+    if (bh > 128 / bw) bh = 128 / bw;
+    uint32_t bt = next_pow2(d->T);
+    if (bt > 128 / (bw * bh)) bt = 128 / (bw * bh);
+    const uint32_t bn = 128 / (bw * bh * bt);
+    p.lbw = ilog2(bw);
+    p.lbh = ilog2(bh);
+    p.lbt = ilog2(bt);
+    p.lbn = ilog2(bn);
+    p.tiles_w = (d->W + bw - 1) / bw;
+    p.tiles_h = (d->H + bh - 1) / bh;
+    p.tiles_t = (d->T + bt - 1) / bt;
+    const int64_t total = static_cast<int64_t>(p.tiles_w) * p.tiles_h * p.tiles_t * ((d->N + bn - 1) / bn) * p.n_tiles;
+    VQB_CHECK(total < (1ll << 31), "vqb_conv3d_gemm: too many tiles");
+    p.total_tiles = static_cast<int32_t>(total);
+    const int stage_bytes = kABytes + block_n * kBlockK * 2;
+    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages;
+    int stages = (227 * 1024 - fixed) / stage_bytes;
+    if (stages > kMaxStages) stages = kMaxStages;
+    p.stages = stages;
+    p.ntaps = d->ntaps;
+    p.kchunks = (d->C + kBlockK - 1) / kBlockK;
+    p.C = d->C;
+    p.Cout = d->Cout;
+    p.N = d->N;
+    p.T = d->T;
+    p.H = d->H;
+    p.W = d->W;
+    p.flags = d->flags;
+    p.out_f32 = d->out_f32;
+    p.on = d->on;
+    p.ot = d->ot;
+    p.oh = d->oh;
+    p.ow = d->ow;
+    p.oc = d->oc;
+    p.out = out;
+    p.res = res;
+    p.bias = bias;
+    for (int t = 0; t < d->ntaps; ++t) {
+        p.tap_view[t] = d->taps[t].view;
+        p.tap_dw[t] = d->taps[t].dw;
+        p.tap_dh[t] = d->taps[t].dh;
+        p.tap_dt[t] = d->taps[t].dt;
+    }
+    for (int v = 0; v < d->nviews; ++v) {
+        const VqbView3d& vw = d->views[v];
+        uint64_t dims[5] = {static_cast<uint64_t>(d->C), static_cast<uint64_t>(vw.Wv), static_cast<uint64_t>(vw.Hv),
+                            static_cast<uint64_t>(vw.Tv), static_cast<uint64_t>(vw.Nv)};
+        uint64_t str[4] = {static_cast<uint64_t>(vw.sw) * 2, static_cast<uint64_t>(vw.sh) * 2,
+                           static_cast<uint64_t>(vw.st) * 2, static_cast<uint64_t>(vw.sn) * 2};
+        uint32_t box[5] = {kBlockK, bw, bh, bt, bn};
+        const void* vbase = static_cast<const uint8_t*>(a) + vw.offset * 2;
+        int rc = encode_tmap_bf16(&p.amap[v], vbase, 5, dims, str, box, 128);
+        if (rc != VQB_OK) return rc;
+    }
+    int rc;
     {
         const uint64_t ktot = static_cast<uint64_t>(d->ntaps) * d->C;
         uint64_t dims[2] = {ktot, static_cast<uint64_t>(d->Cout)};

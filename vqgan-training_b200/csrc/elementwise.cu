@@ -953,6 +953,22 @@ static inline void cv_grid(int HW, int C, int N, Kernel kernel, size_t smem, int
     chunks = (HW + ppc - 1) / ppc;
 }
 
+// tae.DiagonalGaussian (tae.py:259-264): out = mean + exp(0.5 * max(logvar, -3)) * eps over NCTHW z = [N][2Z][S],
+// computed in fp32 and rounded once to the module's dtype.
+template <typename T>
+__global__ void gauss_reparam_kernel(const T* __restrict__ z, const T* __restrict__ eps, T* __restrict__ out, int Z,
+                                     int64_t S, int64_t total) {
+    for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
+         i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t s = i % S, nc = i / S;  // nc = n * Z + c
+        const int64_t n = nc / Z, c = nc % Z;
+        const int64_t zm = (n * 2 * Z + c) * S + s;
+        const float mean = to_f32(z[zm]);
+        const float logvar = fmaxf(to_f32(z[zm + static_cast<int64_t>(Z) * S]), -3.f);
+        from_f32(out[i], fmaf(expf(0.5f * logvar), to_f32(eps[i]), mean));
+    }
+}
+
 }  // namespace vqb
 
 using namespace vqb;
@@ -1348,6 +1364,25 @@ int vqb_wgrad_reduce(const float* partial, float* grad, int ksplit, int Cout, in
     const int64_t total = static_cast<int64_t>(Cout) * Cin * T;
     wgrad_reduce_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         partial, grad, ksplit, Cout, CoutPad, Cin, T, nslots, C64, tapmap_dev, accumulate);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+int vqb_gauss_reparam(const void* z, const void* eps, void* out, int N, int Z, int64_t S, int bf16, void* stream) {
+    VQB_CHECK(z && eps && out, "vqb_gauss_reparam: null pointer");
+    VQB_CHECK(N > 0 && Z > 0 && S > 0 && (bf16 == 0 || bf16 == 1),
+              "vqb_gauss_reparam: bad arguments (N=%d Z=%d S=%lld bf16=%d)", N, Z, (long long)S, bf16);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_gauss_reparam: current device is not sm_90");
+    const int64_t total = static_cast<int64_t>(N) * Z * S;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (bf16)
+        gauss_reparam_kernel<__nv_bfloat16><<<gs_blocks(total, 256), 256, 0, st>>>(
+            static_cast<const __nv_bfloat16*>(z), static_cast<const __nv_bfloat16*>(eps),
+            static_cast<__nv_bfloat16*>(out), Z, S, total);
+    else
+        gauss_reparam_kernel<float><<<gs_blocks(total, 256), 256, 0, st>>>(
+            static_cast<const float*>(z), static_cast<const float*>(eps), static_cast<float*>(out), Z, S, total);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;

@@ -111,6 +111,17 @@ __device__ __forceinline__ void tma_load_4d(const void* desc, uint64_t* bar, voi
         : "memory");
 }
 
+__device__ __forceinline__ void tma_load_5d(const void* desc, uint64_t* bar, void* smem, int32_t c0, int32_t c1,
+                                            int32_t c2, int32_t c3, int32_t c4) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes"
+        " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+        :
+        : "r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+          "r"(c2), "r"(c3), "r"(c4)
+        : "memory");
+}
+
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

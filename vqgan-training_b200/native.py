@@ -16,6 +16,8 @@ _LIB_PATH = os.path.join(_HERE, "libvqb200.so")
 
 VQB_MAX_VIEWS = 16
 VQB_MAX_TAPS = 16
+VQB_MAX_VIEWS_3D = 8
+VQB_MAX_TAPS_3D = 27
 EPI_BIAS, EPI_RES, EPI_RELU, EPI_MASK, EPI_STATS = 1, 2, 4, 8, 16
 
 
@@ -52,6 +54,22 @@ class VqbPackJob(C.Structure):
                 ("T", C.c_int32), ("nslots", C.c_int32), ("transpose", C.c_int32), ("Kpad", C.c_int32),
                 ("fold", C.c_int32), ("sg", C.c_int32), ("ld_g", C.c_int32), ("ld_r", C.c_int32),
                 ("first_block", C.c_int32), ("w_bf16", C.c_int32)]
+
+
+class VqbView3d(C.Structure):
+    _fields_ = [("offset", C.c_int64), ("Wv", C.c_int32), ("Hv", C.c_int32), ("Tv", C.c_int32), ("Nv", C.c_int32),
+                ("sw", C.c_int64), ("sh", C.c_int64), ("st", C.c_int64), ("sn", C.c_int64)]
+
+
+class VqbTap3d(C.Structure):
+    _fields_ = [("view", C.c_int32), ("dw", C.c_int32), ("dh", C.c_int32), ("dt", C.c_int32)]
+
+
+class VqbConv3dDesc(C.Structure):
+    _fields_ = [("C", C.c_int32), ("Cout", C.c_int32), ("N", C.c_int32), ("T", C.c_int32), ("H", C.c_int32),
+                ("W", C.c_int32), ("nviews", C.c_int32), ("ntaps", C.c_int32), ("flags", C.c_int32),
+                ("out_f32", C.c_int32), ("on", C.c_int64), ("ot", C.c_int64), ("oh", C.c_int64), ("ow", C.c_int64),
+                ("oc", C.c_int64), ("views", VqbView3d * VQB_MAX_VIEWS_3D), ("taps", VqbTap3d * VQB_MAX_TAPS_3D)]
 
 
 class VqbAdamwGroup(C.Structure):
@@ -124,6 +142,9 @@ def load():
         "vqb_nchw_to_nhwc_pad_bf16": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
         "vqb_nhwc_to_nchw_bf16": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
         "vqb_wavelet_fwd_bf16": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+        "vqb_conv3d_gemm": (i32, [C.POINTER(VqbConv3dDesc), vp, vp, vp, vp, vp, vp]),
+        "vqb_attn_fwd_hd": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
+        "vqb_gauss_reparam": (i32, [vp, vp, vp, i32, i32, i64, i32, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)
@@ -151,6 +172,11 @@ def ptr(t) -> int:
 
 def launch_count() -> int:
     return load().vqb_kernel_launch_count()
+
+
+def dense_view3d(N: int, T: int, H: int, W: int, Cs: int) -> VqbView3d:
+    """Dense NTHWC view with channel row stride Cs."""
+    return VqbView3d(offset=0, Wv=W, Hv=H, Tv=T, Nv=N, sw=Cs, sh=W * Cs, st=H * W * Cs, sn=T * H * W * Cs)
 
 
 def dense_view(N: int, H: int, W: int, Cs: int) -> VqbView:

@@ -109,6 +109,24 @@ class _PackEntry:
         assert T <= 16
         return -(-(Cin if transpose else Cout) // 8) * -(-Kpad // 64)
 
+    def pack_alone(self):
+        """Re-packs this entry in place with the per-tensor kernel (vqb_pack_weights[_fold][_bf16], up to 31 taps): the
+        route of the 27-tap 3x3x3 weights of tae.py, which the one-launch multi-pack kernel (<= 16 taps) does not take."""
+        Cout, Cin, T, nslots, transpose, Kpad, fold = self.spec[:7]
+        assert self.spec[7] == nslots, "the fat-pixel layout is packed by the multi-pack kernel only"
+        w = self.wref().detach()
+        if self.dtype == torch.bfloat16:
+            fn = _L().vqb_pack_weights_fold_bf16 if fold else _L().vqb_pack_weights_bf16
+        else:
+            fn = _L().vqb_pack_weights_fold if fold else _L().vqb_pack_weights
+        check(fn(ptr(w), ptr(self.out), Cout, Cin, T, nslots, ptr(self.tm), transpose, Kpad, stream_ptr()),
+              "pack_weights")
+
+
+# taps per filter the one-launch multi-pack kernel takes (kPackMaxT in csrc/optim.cu); larger filters (the 27 taps of a
+# 3x3x3 conv) are packed per tensor
+PACK_MULTI_MAX_TAPS = 16
+
 
 # every live pack entry, by the data_ptr of the master weight it was packed from (weak: caches own the entries)
 _pack_registry = {}
@@ -116,16 +134,17 @@ _pack_tables = {}
 
 
 def _new_pack_entry(weight, tapmap, transpose, Kpad, fold, fat=False) -> _PackEntry:
-    Cout, Cin, KH, KW = weight.shape
+    Cout, Cin = weight.shape[:2]
+    T = math.prod(weight.shape[2:])  # OIHW or OIDHW (tae.py's Conv3d)
     R = Cin if transpose else Cout
     nslots = len(tapmap)
     if fat:  # [R][9 slots][8] -> [R][3][64]: columns kw*8 + c of each kh row, zero beyond 24 (plans.geom_fat3)
         assert nslots == 9 and Kpad == 8
         out = torch.zeros(R, 3, plans.FAT_K, device=weight.device, dtype=torch.bfloat16)
-        spec = (Cout, Cin, KH * KW, nslots, 1 if transpose else 0, Kpad, 0, 3, plans.FAT_K, 3 * plans.FAT_K)
+        spec = (Cout, Cin, T, nslots, 1 if transpose else 0, Kpad, 0, 3, plans.FAT_K, 3 * plans.FAT_K)
     else:
         out = torch.empty(R, nslots, Kpad, device=weight.device, dtype=torch.bfloat16)
-        spec = (Cout, Cin, KH * KW, nslots, 1 if transpose else 0, Kpad, 1 if fold else 0, nslots, 0, nslots * Kpad)
+        spec = (Cout, Cin, T, nslots, 1 if transpose else 0, Kpad, 1 if fold else 0, nslots, 0, nslots * Kpad)
     check_master_dtype(weight, "conv master weight")
     if not weight.is_contiguous():
         raise RuntimeError("vqgan-training_b200: conv master weights must be contiguous OIHW tensors")
@@ -136,7 +155,15 @@ def _new_pack_entry(weight, tapmap, transpose, Kpad, fold, fat=False) -> _PackEn
 
 def _run_pack(entries):
     """Re-packs `entries` (in place) with ONE vqb_pack_weights_multi launch (fp32 and bf16 masters may be mixed: each
-    job carries its source dtype); the device job table is cached per entry set."""
+    job carries its source dtype); the device job table is cached per entry set. Entries of filters with more than
+    PACK_MULTI_MAX_TAPS taps are packed per tensor instead."""
+    alone = [e for e in entries if e.spec[2] > PACK_MULTI_MAX_TAPS]
+    if alone:
+        for e in alone:
+            e.pack_alone()
+            w = e.wref()
+            e.ver = (w._version, w.data_ptr())
+        entries = [e for e in entries if e.spec[2] <= PACK_MULTI_MAX_TAPS]
     if not entries:
         return
     key = tuple(id(e) for e in entries)
@@ -1024,3 +1051,128 @@ def vq_argmin(z_flat: torch.Tensor, codebook: torch.Tensor):
     check(_L().vqb_vq_argmin(ptr(z_flat), ptr(cb), ptr(idx), ptr(zq), ptr(sq), M, cb.shape[0], D, stream_ptr()),
           "vq_argmin")
     return idx, zq, sq
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Video autoencoder (tae.py): no-grad inference ops over NTHWC bf16 activations [N, T, H, W, Cp]. There is no backward
+# here; tae.py refuses a forward that autograd would have to differentiate before anything is launched.
+def _bias_f32(bias):
+    if bias is None:
+        return None
+    b = bias.detach()
+    return b if b.dtype == torch.float32 else b.float()
+
+
+def run_conv3d(g: plans.ConvGeom3d, a, wp, Cout, out, out_strides, out_off_elems=0, bias=None, res=None,
+               out_f32=False):
+    flags = (EPI_BIAS if bias is not None else 0) | (EPI_RES if res is not None else 0)
+    dk = (Cout, tuple(out_strides), flags, out_f32)
+    descs = g.__dict__.setdefault("_descs", {})
+    d = descs.get(dk)
+    if d is None:
+        d = plans.conv3d_desc(g, Cout, out_strides, flags, out_f32)
+        descs[dk] = d
+    esz = out.element_size()
+    check(_L().vqb_conv3d_gemm(d, ptr(a), ptr(wp), ptr(bias), (ptr(res) + out_off_elems * 2) if res is not None else 0,
+                               ptr(out) + out_off_elems * esz, stream_ptr()), "conv3d_gemm")
+
+
+def conv3d(x, weight, bias, cache, kind="s1", residual=None, ncthw_out=False):
+    """3-D convolution of the NTHWC bf16 activation x [N, T, H, W, Cp] with an OIDHW fp32 or bf16 weight.
+    kind: "s1" (3x3x3, stride 1, padding 1), "s2" (Downsample: F.pad(0,1,0,1,0,1) + 3x3x3 stride 2), "p1" (1x1x1, run
+    by vqb_conv_gemm on the [N][T*H][W][C] view). residual: bf16 in the output's layout (NTHWC [N, T, H, W, Cop], or
+    NCTHW with ncthw_out), summed in the epilogue. ncthw_out: write [N, Cout, T, H, W] in the weight's dtype straight
+    from the epilogue (encoder z / decoder video)."""
+    require_cuda(x)
+    N, T, H, W, Cp = x.shape
+    Cout, Cin = weight.shape[:2]
+    assert Cp == plans.cpad(Cin), f"conv input has {Cp} channels, weight expects {Cin}"
+    x = x.contiguous()
+    b = _bias_f32(bias)
+    Cop = plans.cpad(Cout)
+    res = residual.contiguous() if residual is not None else None
+    if kind == "p1":
+        assert not ncthw_out
+        g = cache.geom(("p1", N, T, H, W), lambda: plans.geom_s1(N, T * H, W, Cp, 1))
+        wp = cache.get(weight, ("fwd", kind), g.tapmap, False, Cp)
+        out = (torch.empty if Cop == Cout else torch.zeros)(N, T, H, W, Cop, device=x.device, dtype=torch.bfloat16)
+        run_conv_gemm(g, x, wp, Cout, out, plans.nhwc_strides(T * H, W, Cop), bias=b, res=res)
+        return out
+    if kind == "s1":
+        g = cache.geom(("s1", N, T, H, W), lambda: plans.geom3_s1(N, T, H, W, Cp))
+    elif kind == "s2":
+        g = cache.geom(("s2", N, T, H, W), lambda: plans.geom3_s2(N, T, H, W, Cp))
+    else:
+        raise ValueError(kind)
+    wp = cache.get(weight, ("fwd", kind), g.tapmap, False, Cp)
+    if ncthw_out:
+        f32 = weight.dtype == torch.float32
+        out = torch.empty(N, Cout, g.To, g.Ho, g.Wo, device=x.device, dtype=torch.float32 if f32 else torch.bfloat16)
+        run_conv3d(g, x, wp, Cout, out, plans.ncthw_strides(Cout, g.To, g.Ho, g.Wo), bias=b, res=res, out_f32=f32)
+        return out
+    out = (torch.empty if Cop == Cout else torch.zeros)(N, g.To, g.Ho, g.Wo, Cop, device=x.device, dtype=torch.bfloat16)
+    run_conv3d(g, x, wp, Cout, out, plans.nthwc_strides(g.To, g.Ho, g.Wo, Cop), bias=b, res=res)
+    return out
+
+
+def upsample_conv3d(x, weight, bias, cache):
+    """Upsample (tae.py:110-116: nearest x2 in T, H and W, then the 3x3x3 padding-1 conv) as eight 2x2x2-tap phase
+    convs over the low-resolution x (plans.geom3_up_fwd): 8/27 of the MACs, no 8x intermediate."""
+    require_cuda(x)
+    x = x.contiguous()
+    N, t, h, w, Cp = x.shape
+    Cout, Cin = weight.shape[:2]
+    assert tuple(weight.shape[2:]) == (3, 3, 3) and Cp == plans.cpad(Cin)
+    Cop = plans.cpad(Cout)
+    out = (torch.empty if Cop == Cout else torch.zeros)(N, 2 * t, 2 * h, 2 * w, Cop, device=x.device,
+                                                        dtype=torch.bfloat16)
+    b = _bias_f32(bias)
+    strides = plans.up3_out_strides(t, h, w, Cop)
+    for pt in range(2):
+        for ph in range(2):
+            for pw in range(2):
+                g = cache.geom(("up", N, t, h, w, pt, ph, pw), lambda: plans.geom3_up_fwd(N, t, h, w, Cp, pt, ph, pw))
+                wp = cache.get(weight, ("up", pt, ph, pw), g.tapmask, False, Cp, fold=True)
+                run_conv3d(g, x, wp, Cout, out, strides, out_off_elems=((pt * 2 * h + ph) * 2 * w + pw) * Cop, bias=b)
+    return out
+
+
+def group_norm_silu3d(x, gamma, beta, groups=32, eps=1e-6, silu=True):
+    """GroupNorm(+swish) over the T*H*W voxels of an NTHWC activation (tae.py:63-71): the 2-D kernels on the
+    [N][T*H][W][C] view, deterministic statistics pass."""
+    N, T, H, W, C = x.shape
+    y = group_norm_silu(x.reshape(N, T * H, W, C), gamma, beta, groups, eps, silu)
+    return y.view(N, T, H, W, C)
+
+
+def attention_hd(qkv, heads, head_dim):
+    """qkv [N, T, H, W, 3C] bf16 (q | k | v channel blocks) -> softmax(q k^T / sqrt(head_dim)) v as [N, T, H, W, C]
+    (tae.py:26-51). head_dim 32 or 64."""
+    if head_dim not in (32, 64):
+        raise NotImplementedError(f"vqgan-training_b200: attention heads of {head_dim} channels are not supported "
+                                  "(heads of 32 or 64 channels only)")
+    qkv = qkv.contiguous()
+    N, T, H, W, C3 = qkv.shape
+    C = C3 // 3
+    assert C == heads * head_dim
+    out = torch.empty(N, T, H, W, C, device=qkv.device, dtype=torch.bfloat16)
+    lse = torch.empty(N, heads, T * H * W, device=qkv.device, dtype=torch.float32)
+    check(_L().vqb_attn_fwd_hd(ptr(qkv), ptr(out), ptr(lse), N, T * H * W, C, head_dim, stream_ptr()), "attn_fwd_hd")
+    return out
+
+
+def gauss_reparam(z, eps):
+    """z [N, 2Z, ...] (mean | logvar channel halves), eps [N, Z, ...] -> mean + exp(0.5 * logvar.clamp(min=-3)) * eps
+    (tae.py:259-264) in z's dtype (fp32 or bf16), computed in fp32."""
+    require_cuda(z)
+    check_master_dtype(z, "latent")
+    z = z.contiguous()
+    eps = eps.to(z.dtype).contiguous()
+    N, Z2 = z.shape[:2]
+    Z = Z2 // 2
+    S = z[0, 0].numel()
+    assert Z2 == 2 * Z and eps.shape == (N, Z) + tuple(z.shape[2:])
+    out = torch.empty_like(eps)
+    check(_L().vqb_gauss_reparam(ptr(z), ptr(eps), ptr(out), N, Z, S, 1 if z.dtype == torch.bfloat16 else 0,
+                                 stream_ptr()), "gauss_reparam")
+    return out

@@ -8,13 +8,15 @@ Variants (reference call sites):
   s1      : k x k stride-1 "same" conv (3x3 p1, 1x1 p0)                ae.py:105-117, VGG utils.py:95-111
   s2      : 3x3 stride-2 conv after F.pad(0,1,0,1)  (Downsample)       ae.py:143-154
   patch   : k x k stride-k non-overlapping conv (PatchD heads)         utils.py:156-185
+  3-D     : 3x3x3 stride-1 / stride-2 / folded up-sampling convs of the video autoencoder (tae.py), see geom3_*
 """
 from __future__ import annotations
 
 from dataclasses import dataclass, field
 from typing import List, Tuple
 
-from native import VqbConvDesc, VqbTap, VqbView, VqbWgradDesc, dense_view
+from native import (VqbConv3dDesc, VqbConvDesc, VqbTap, VqbTap3d, VqbView, VqbView3d, VqbWgradDesc, dense_view,
+                    dense_view3d)
 
 
 def cpad(c: int) -> int:
@@ -210,3 +212,99 @@ def wgrad_desc(g: ConvGeom, Cout_pad: int, ksplit: int, dy_view=None, ld_overrid
     for i, (v, dw, dh) in enumerate(g.taps):
         d.taps[i] = VqbTap(view=v, dw=dw, dh=dh, _pad=0)
     return d
+
+
+# ---- 3-D (video) convolutions of tae.py on NTHWC activations (vqb_conv3d_gemm) --------------------------------------
+# Taps are (view, dw, dh, dt); tapmap / tapmask index the flattened 3x3x3 kernel, tap kt*9 + kh*3 + kw (OIDHW order).
+@dataclass
+class ConvGeom3d:
+    """Views/taps of the A operand for the output grid (N, To, Ho, Wo)."""
+    N: int
+    To: int
+    Ho: int
+    Wo: int
+    C: int  # channels of the A tensor (padded)
+    views: List[VqbView3d] = field(default_factory=list)
+    taps: List[Tuple[int, int, int, int]] = field(default_factory=list)  # (view, dw, dh, dt)
+    tapmap: List[int] = field(default_factory=list)
+    tapmask: List[int] = field(default_factory=list)
+
+
+def geom3_s1(N, T, H, W, C) -> ConvGeom3d:
+    """3x3x3 stride-1 conv, padding 1 (tae.py:66-78, :136-138, :165-167, :208-210, :233): 27 taps of one view."""
+    g = ConvGeom3d(N, T, H, W, C, [dense_view3d(N, T, H, W, C)])
+    for kt in range(3):
+        for kh in range(3):
+            for kw in range(3):
+                g.taps.append((0, kw - 1, kh - 1, kt - 1))
+                g.tapmap.append(kt * 9 + kh * 3 + kw)
+    return g
+
+
+def geom3_s2(N, T, H, W, C) -> ConvGeom3d:
+    """Downsample (tae.py:96-104): F.pad(x, (0,1,0,1,0,1)) + 3x3x3 stride-2 conv, out (T/2, H/2, W/2). Tap (kt,kh,kw)
+    reads x[2to+kt, 2ho+kh, 2wo+kw] = parity view (kt&1, kh&1, kw&1) at (to + kt//2, ho + kh//2, wo + kw//2); the pad
+    plane is the view's zero fill."""
+    assert T % 2 == 0 and H % 2 == 0 and W % 2 == 0, "Downsample needs even T, H, W"
+    g = ConvGeom3d(N, T // 2, H // 2, W // 2, C)
+    for pt in range(2):
+        for ph in range(2):
+            for pw in range(2):
+                g.views.append(VqbView3d(offset=((pt * H + ph) * W + pw) * C, Wv=W // 2, Hv=H // 2, Tv=T // 2, Nv=N,
+                                         sw=2 * C, sh=2 * W * C, st=2 * H * W * C, sn=T * H * W * C))
+    for kt in range(3):
+        for kh in range(3):
+            for kw in range(3):
+                g.taps.append(((kt & 1) * 4 + (kh & 1) * 2 + (kw & 1), kw // 2, kh // 2, kt // 2))
+                g.tapmap.append(kt * 9 + kh * 3 + kw)
+    return g
+
+
+def _up_mask3(pt, ph, pw, i, j, k) -> int:
+    m = 0
+    for kt in _UP_SET[pt][i]:
+        for kh in _UP_SET[ph][j]:
+            for kw in _UP_SET[pw][k]:
+                m |= 1 << (kt * 9 + kh * 3 + kw)
+    return m
+
+
+def geom3_up_fwd(N, t, h, w, C, pt, ph, pw) -> ConvGeom3d:
+    """Phase (pt,ph,pw) of Upsample (tae.py:110-116: nearest x2 in T, H, W + 3x3x3 conv, padding 1): a 2x2x2-tap conv
+    over the LOW-RES x writing the (pt,ph,pw) sub-grid of the output, with folded weights
+    Wf[i][j][k] = sum over kt in SET[pt][i], kh in SET[ph][j], kw in SET[pw][k] of W[kt,kh,kw]. The eight phases do 8/27
+    of the MACs of the literal form and never materialise the 8x tensor."""
+    g = ConvGeom3d(N, t, h, w, C, [dense_view3d(N, t, h, w, C)])
+    for i in range(2):
+        for j in range(2):
+            for k in range(2):
+                g.taps.append((0, _UP_OFF[pw][k], _UP_OFF[ph][j], _UP_OFF[pt][i]))
+                g.tapmask.append(_up_mask3(pt, ph, pw, i, j, k))
+    return g
+
+
+def up3_out_strides(t, h, w, Cop):
+    """(on, ot, oh, ow, oc) of one phase sub-grid of the [N, 2t, 2h, 2w, Cop] output, and the element offset of phase
+    (pt, ph, pw) is ((pt * 2h + ph) * 2w + pw) * Cop."""
+    return (8 * t * h * w * Cop, 2 * 4 * h * w * Cop, 2 * 2 * w * Cop, 2 * Cop, 1)
+
+
+def conv3d_desc(g: ConvGeom3d, Cout: int, out_strides, flags=0, out_f32=False) -> VqbConv3dDesc:
+    """out_strides = (on, ot, oh, ow, oc) in elements."""
+    d = VqbConv3dDesc()
+    d.C, d.Cout, d.N, d.T, d.H, d.W = g.C, Cout, g.N, g.To, g.Ho, g.Wo
+    d.nviews, d.ntaps, d.flags, d.out_f32 = len(g.views), len(g.taps), flags, 1 if out_f32 else 0
+    d.on, d.ot, d.oh, d.ow, d.oc = out_strides
+    for i, v in enumerate(g.views):
+        d.views[i] = v
+    for i, (v, dw, dh, dt) in enumerate(g.taps):
+        d.taps[i] = VqbTap3d(view=v, dw=dw, dh=dh, dt=dt)
+    return d
+
+
+def ncthw_strides(C, T, H, W):
+    return (C * T * H * W, H * W, W, 1, T * H * W)
+
+
+def nthwc_strides(T, H, W, Cs):
+    return (T * H * W * Cs, H * W * Cs, W * Cs, Cs, 1)
