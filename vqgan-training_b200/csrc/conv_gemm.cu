@@ -42,6 +42,7 @@ struct alignas(64) ConvParams {
     int32_t n_tiles, total_tiles;
     int32_t stages, do_stats;
     int32_t flags, out_f32;
+    int32_t vec_store, _pad0;  // 1: paired bf16 stores (oc == 1, 16-byte aligned pixel rows), else per element
     int64_t on, oh, ow, oc;
     void* out;
     const void* res;
@@ -79,6 +80,7 @@ struct alignas(64) Conv3dParams {
     int32_t n_tiles, total_tiles;
     int32_t stages, do_stats;
     int32_t flags, out_f32;
+    int32_t vec_store, _pad0;
     int64_t on, ot, oh, ow, oc;
     void* out;
     const void* res;
@@ -173,7 +175,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const uint32_t ring = smem_u32(base);
     const bool has_bias = p.flags & VQB_EPI_BIAS, has_res = p.flags & VQB_EPI_RES;
     const bool do_relu = !kR5 && (p.flags & VQB_EPI_RELU), has_mask = !kR5 && (p.flags & VQB_EPI_MASK);
-    const bool vec_path = (p.oc == 1) && (p.out_f32 == 0);
+    const bool vec_path = p.vec_store != 0;
     const bool do_gn = !kR5 && p.gn_cs != nullptr;
     const bool reduce = !kR5 && (p.do_stats || do_gn);
     const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.res);
@@ -418,9 +420,10 @@ extern "C" int vqb_conv_stats_ok(const VqbConvDesc* d) {
     if (!d) return 0;
     VqbConvDesc q = *d;
     q.flags &= ~VQB_EPI_STATS;
-    static const uint64_t dummy_aligned[4] = {0, 0, 0, 0};
+    alignas(16) static const uint64_t dummy_aligned[4] = {0, 0, 0, 0};
     const void* dp = dummy_aligned;
-    const int r = conv_gemm_impl(&q, dp, dp, nullptr, dp, dp, const_cast<void*>(dp), nullptr, nullptr, true);
+    const int r = conv_gemm_impl(&q, dp, dp, static_cast<const float*>(dp), dp, dp, const_cast<void*>(dp), nullptr,
+                                 nullptr, true);
     return r == 1 ? 1 : 0;
 }
 
@@ -439,15 +442,15 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     if ((d->flags & VQB_EPI_RES)) VQB_CHECK(res != nullptr, "vqb_conv_gemm: VQB_EPI_RES without res");
     if ((d->flags & VQB_EPI_MASK)) VQB_CHECK(mask != nullptr, "vqb_conv_gemm: VQB_EPI_MASK without mask");
     if ((d->flags & VQB_EPI_STATS)) VQB_CHECK(stats != nullptr, "vqb_conv_gemm: VQB_EPI_STATS without stats");
-    const bool nhwc_bf16 = d->oc == 1 && !d->out_f32;
-    if (nhwc_bf16) {
-        VQB_CHECK(d->on % 8 == 0 && d->oh % 8 == 0 && d->ow % 8 == 0 &&
-                      (reinterpret_cast<uintptr_t>(out) & 15u) == 0,
-                  "vqb_conv_gemm: NHWC bf16 output needs 16-byte aligned pixel rows");
-        const uintptr_t ops = reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(mask) |
-                              reinterpret_cast<uintptr_t>(gn ? gn->x : nullptr);
-        VQB_CHECK((ops & 3u) == 0, "vqb_conv_gemm: residual / mask / GroupNorm input must be 4-byte aligned");
-    }
+    // Paired bf16 stores need 16-byte aligned pixel rows. A channel-contiguous output without them (e.g. NCHW bf16 of
+    // 1x1 images: oc = H*W = 1, on = Cout) takes the per-element store instead.
+    const uintptr_t ops = reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(mask) |
+                          reinterpret_cast<uintptr_t>(gn ? gn->x : nullptr);
+    const bool nhwc_bf16 = d->oc == 1 && !d->out_f32 && d->on % 8 == 0 && d->oh % 8 == 0 && d->ow % 8 == 0 &&
+                           (reinterpret_cast<uintptr_t>(out) & 15u) == 0 && (ops & 3u) == 0;
+    if (!nhwc_bf16)
+        VQB_CHECK((reinterpret_cast<uintptr_t>(out) & (d->out_f32 ? 3u : 1u)) == 0 && (ops & 1u) == 0,
+                  "vqb_conv_gemm: misaligned output / residual / mask");
     for (int t = 0; t < d->ntaps; ++t)
         VQB_CHECK(d->taps[t].view >= 0 && d->taps[t].view < d->nviews, "vqb_conv_gemm: tap %d view out of range", t);
     if (!query_only && !device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_conv_gemm: current device is not sm_90");
@@ -511,6 +514,8 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     p.W = d->W;
     p.flags = d->flags;
     p.out_f32 = d->out_f32;
+    p.vec_store = nhwc_bf16 ? 1 : 0;
+    p._pad0 = 0;
     p.on = d->on;
     p.oh = d->oh;
     p.ow = d->ow;
@@ -564,15 +569,15 @@ extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void
     if (d->flags & VQB_EPI_RES) VQB_CHECK(res != nullptr, "vqb_conv3d_gemm: VQB_EPI_RES without res");
     VQB_CHECK(d->on >= 0 && d->ot >= 0 && d->oh >= 0 && d->ow >= 0 && d->oc > 0,
               "vqb_conv3d_gemm: output strides must be non-negative (oc > 0)");
-    if (d->oc == 1 && !d->out_f32) {
-        VQB_CHECK(d->on % 8 == 0 && d->ot % 8 == 0 && d->oh % 8 == 0 && d->ow % 8 == 0 &&
-                      (reinterpret_cast<uintptr_t>(out) & 15u) == 0 && (reinterpret_cast<uintptr_t>(res) & 3u) == 0,
-                  "vqb_conv3d_gemm: NTHWC bf16 output needs 16-byte aligned voxel rows");
-    } else {
+    // paired bf16 stores need 16-byte aligned voxel rows; otherwise (e.g. NCTHW bf16 of 1x1x1 videos: oc = 1) the
+    // per-element store
+    const bool vec3 = d->oc == 1 && !d->out_f32 && d->on % 8 == 0 && d->ot % 8 == 0 && d->oh % 8 == 0 &&
+                      d->ow % 8 == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0 &&
+                      (reinterpret_cast<uintptr_t>(res) & 3u) == 0;
+    if (!vec3)
         VQB_CHECK((reinterpret_cast<uintptr_t>(out) & (d->out_f32 ? 3u : 1u)) == 0 &&
                       (reinterpret_cast<uintptr_t>(res) & 1u) == 0,
                   "vqb_conv3d_gemm: misaligned output / residual");
-    }
     for (int v = 0; v < d->nviews; ++v) {
         const VqbView3d& vw = d->views[v];
         VQB_CHECK(vw.offset >= 0 && vw.Wv > 0 && vw.Hv > 0 && vw.Tv > 0 && vw.Nv > 0 && vw.sw > 0 && vw.sw % 8 == 0 &&
@@ -621,6 +626,7 @@ extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void
     p.W = d->W;
     p.flags = d->flags;
     p.out_f32 = d->out_f32;
+    p.vec_store = vec3 ? 1 : 0;
     p.on = d->on;
     p.ot = d->ot;
     p.oh = d->oh;
