@@ -99,27 +99,6 @@ typedef struct VqbWgradDesc {
     VqbTap taps[VQB_MAX_TAPS];
 } VqbWgradDesc;
 
-/*
- * Data-gradient launch fused with the statistics pass of a GroupNorm(+swish) backward. When the conv being
- * differentiated consumed y = swish(GroupNorm(x)) (ae.py:124-131: norm1 -> conv1, norm2 -> conv2), its data gradient IS
- * the dy of that GroupNorm; the epilogue reads the matching x tile (TMA-prefetched, same addressing as `out`) and
- * accumulates cs[n][c] = (sum_p du, sum_p du * xhat), du = dy * swish'(gamma*xhat + beta), into the pre-zeroed
- * cs[N][Cout][2] with fp32 atomics. vqb_gn_silu_bwd_pre then only finalises and applies (x, dy are not read a second
- * time for the reduction: 10 -> 6 bytes per element for the GroupNorm backward).
- */
-typedef struct VqbGnBwdFuse {
-    const void* x;      /* bf16 NHWC input of the GroupNorm, same geometry as `out` */
-    const float* mr;    /* [N][groups][2] mean, rstd saved by the forward */
-    const float* gamma; /* [Cout] */
-    const float* beta;  /* [Cout] */
-    float* cs;          /* [N][Cout][2], pre-zeroed */
-    int32_t groups;
-    int32_t _pad;
-} VqbGnBwdFuse;
-int vqb_conv_gemm_gnbwd(const VqbConvDesc* d, const void* a, const void* w_packed, const float* bias, void* out,
-                        const VqbGnBwdFuse* gn, void* stream);
-int vqb_conv_gnbwd_ok(const VqbConvDesc* d, int groups);
-
 /* 1 if vqb_conv_gemm supports VQB_EPI_STATS for this descriptor (staged epilogue, whole sub-tiles inside one image) */
 int vqb_conv_stats_ok(const VqbConvDesc* d);
 
@@ -180,11 +159,6 @@ int vqb_gn_silu_fwd_pre(const void* x, void* y, const float* gamma, const float*
 int vqb_gn_silu_bwd(const void* x, const void* dy, const void* add, void* dx, const float* gamma, const float* beta,
                     const float* mr, float* dgamma, float* dbeta, float* ws, int N, int HW, int C, int G, int silu,
                     float* dx_colsum, void* stream);
-/* same, when cs[N][C][2] = (sum du, sum du*xhat) was already accumulated by vqb_conv_gemm_gnbwd: finalise + apply only
- * (ws: N*G*2 floats) */
-int vqb_gn_silu_bwd_pre(const void* x, const void* dy, const void* add, void* dx, const float* gamma, const float* beta,
-                        const float* mr, const float* cs, float* dgamma, float* dbeta, float* ws, int N, int HW, int C,
-                        int G, int silu, float* dx_colsum, void* stream);
 
 /*
  * Wavelet front-end of the encoder (--use_wavelet; utils.py:229-247): F.pad(x, 2) + grouped 6x6 stride-2 conv with the
@@ -289,10 +263,6 @@ int vqb_attn_fwd_hd(const void* qkv, void* out, float* lse, int N, int T, int C,
  * reference's own call, so a seeded run consumes the same CUDA RNG stream).
  */
 int vqb_gauss_reparam(const void* z, const void* eps, void* out, int N, int Z, int64_t S, int bf16, void* stream);
-
-/* nearest-neighbour x2 up-sampling (ae.py:165) and its backward (2x2 sum), bf16 NHWC */
-int vqb_upsample2x_fwd(const void* x, void* y, int N, int H, int W, int C, void* stream);
-int vqb_upsample2x_bwd(const void* dy, void* dx, int N, int H, int W, int C, void* stream);
 
 /* out[c] = sum over P pixels of x[p][c] : Conv2d bias gradient */
 int vqb_colsum(const void* x, float* out, int64_t P, int C, void* stream);

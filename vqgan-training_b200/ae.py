@@ -5,7 +5,7 @@ state_dict keys / fp32 OIHW shapes — but every forward/backward runs hand-writ
   conv 3x3/1x1 s1, Downsample (pad(0,1,0,1)+s2), dgrad, wgrad  -> wgmma implicit-GEMM kernels (csrc/conv_gemm.cu,
                                                                   csrc/wgrad_gemm.cu), TMA-staged, register accumulators
   FP32GroupNorm + swish                                          -> fused stats/apply kernels (csrc/elementwise.cu)
-  Upsample (nearest x2)                                          -> vector copy kernel + conv
+  Upsample (nearest x2) + conv3x3                                -> four 2x2-tap phase convs over the low-res input
   AttnBlock                                                      -> GN kernel + 1x1 conv kernels + flash-style core
 
 Internally activations are bf16 NHWC (`Act`); modules accept either an `Act` (internal) or a plain NCHW tensor
@@ -42,13 +42,11 @@ from utils import wavelet_transform_multi_channel
 class Act:
     """Internal activation: bf16 NHWC tensor `t` [N,H,W,Cp] carrying its true channel count `C`."""
 
-    __slots__ = ("t", "C", "stats", "framed", "link")
+    __slots__ = ("t", "C", "stats", "framed")
 
-    def __init__(self, t: Tensor, C: int, stats=None, framed=False, link=None):
+    def __init__(self, t: Tensor, C: int, stats=None, framed=False):
         self.t = t
         self.C = C
-        self.link = link  # ops.GnLink when t is the output of a GroupNorm(+swish): lets the consuming conv's data-gradient
-        # epilogue accumulate that GroupNorm's backward statistics
         self.stats = stats  # per-(n, channel) sum / sum of squares [N, C, 2] when the producing conv computed them
         self.framed = framed  # t is a zero-framed [N, H+2, W+2, 8] image (input of a "fat pixel" first-layer conv)
 
@@ -85,7 +83,7 @@ def _stats_fusion() -> bool:
     the last bits of every later activation, vary between launches. That is what training pays for one read pass less
     per GroupNorm; without autograd (inference) the statistics come from the GroupNorm's own fixed-order pass instead,
     so the forward is deterministic and a CUDA-graph replay equals the eager run bit for bit."""
-    return torch.is_grad_enabled() and os.environ.get("VQB_GN_STATS_FUSION", "1") == "1"
+    return torch.is_grad_enabled()
 
 
 def swish(x):
@@ -115,11 +113,10 @@ class StandardizedC2d(nn.Conv2d):
     def forward_act(self, a: Act, residual: Act = None, relu=False, input_is_relu=False, nchw_out=False,
                     want_stats=False):
         """want_stats: also accumulate the GroupNorm statistics of the output in the conv epilogue (Act.stats)."""
-        want_stats = want_stats and not nchw_out and os.environ.get("VQB_GN_STATS_FUSION", "1") == "1"
+        want_stats = want_stats and not nchw_out
         kind = "fat3" if a.framed else self._kind()
         out = ops.conv(a.t, self.weight, self.bias, self._packed, kind,
-                       residual.t if residual is not None else None, relu, input_is_relu, nchw_out, want_stats,
-                       gn_link=a.link)
+                       residual.t if residual is not None else None, relu, input_is_relu, nchw_out, want_stats)
         if nchw_out:
             return out
         if want_stats:
@@ -143,17 +140,15 @@ class FP32GroupNorm(nn.GroupNorm):
 
     def forward(self, input, silu: bool = False):
         a, ext = _enter(input, self)
-        link = ops.GnLink() if (silu and not ext and torch.is_grad_enabled()) else None
-        y = ops.group_norm_silu(a.t, self.weight, self.bias, self.num_groups, self.eps, silu, chsums=a.stats, link=link)
-        return _exit(Act(y, a.C, link=link), ext, self)
+        y = ops.group_norm_silu(a.t, self.weight, self.bias, self.num_groups, self.eps, silu, chsums=a.stats)
+        return _exit(Act(y, a.C), ext, self)
 
     def forward_with_skip(self, a: "Act", silu: bool = True):
         """-> (normalised activation, the input again). Consumers of the second output (the residual path) get their
         gradient summed inside the GroupNorm backward kernel (no separate accumulation pass)."""
-        link = ops.GnLink() if (silu and torch.is_grad_enabled()) else None  # backward-only state
         y, skip = ops.group_norm_silu(a.t, self.weight, self.bias, self.num_groups, self.eps, silu, with_skip=True,
-                                      chsums=a.stats, link=link)
-        return Act(y, a.C, link=link), Act(skip, a.C)
+                                      chsums=a.stats)
+        return Act(y, a.C), Act(skip, a.C)
 
 
 class AttnBlock(nn.Module):
@@ -232,17 +227,13 @@ class Upsample(nn.Module):
         self.conv = StandardizedC2d(in_channels, in_channels, kernel_size=3, stride=1, padding=1)
 
     def forward(self, x):
-        # nearest x2 + conv3x3 as four 2x2-tap phase convs over the low-res tensor (no 4x intermediate, 4/9 of the MACs);
-        # VQB_UPSAMPLE_FOLD=0 selects the literal form (copy kernel + conv), kept for A/B measurements
+        # nearest x2 + conv3x3 as four 2x2-tap phase convs over the low-res tensor (no 4x intermediate, 4/9 of the MACs)
         a, ext = _enter(x, self)
-        if os.environ.get("VQB_UPSAMPLE_FOLD", "1") == "1":
-            fuse = _stats_fusion()
-            y = ops.upsample_conv(a.t, self.conv.weight, self.conv.bias, self.conv._packed, want_stats=fuse)
-            if fuse:
-                return _exit(Act(y[0], self.conv.out_channels, y[1]), ext, self)
-            return _exit(Act(y, self.conv.out_channels), ext, self)
-        up = Act(ops.upsample2x(a.t), a.C)
-        return _exit(self.conv.forward_act(up, want_stats=_stats_fusion()), ext, self)
+        fuse = _stats_fusion()
+        y = ops.upsample_conv(a.t, self.conv.weight, self.conv.bias, self.conv._packed, want_stats=fuse)
+        if fuse:
+            return _exit(Act(y[0], self.conv.out_channels, y[1]), ext, self)
+        return _exit(Act(y, self.conv.out_channels), ext, self)
 
 
 class Encoder(nn.Module):

@@ -49,21 +49,11 @@ struct alignas(64) ConvParams {
     const void* mask;
     const float* bias;
     float* stats;
-    // fused GroupNorm(+SiLU)-backward statistics (vqb_conv_gemm_gnbwd): this launch is the data gradient of the conv
-    // that consumed y = silu(GN(x)); its output IS dy of that GroupNorm, so the epilogue also reads x (same layout as
-    // the output) and accumulates cs[n][c] = (sum_p du, sum_p du * xhat), du = dy * silu'(gamma*xhat + beta) — the
-    // whole "reduce" pass of the GroupNorm backward (x and dy read once more from HBM) disappears.
-    const __nv_bfloat16* gn_x;
-    const float* gn_mr;     // [N][G][2] mean, rstd
-    const float* gn_gamma;  // [C]
-    const float* gn_beta;   // [C]
-    float* gn_cs;           // [N][C][2], pre-zeroed
-    int32_t gn_G, gn_lcpg;  // groups, log2(channels per group)
 };
 
 // The 3-D (video) form: NTHWC activations, 5-D TMA boxes [64 ch][bw][bh][bt][bn], up to 27 taps over up to 8 views.
-// Inference only: the epilogue has bias and residual; the statistics / GroupNorm-backward / ReLU / mask fields exist so
-// that the kernel body compiles for both ranks, and are always zero here (the kernel tests kRank before reading them).
+// Inference only: the epilogue has bias and residual; the statistics / ReLU / mask fields exist so that the kernel
+// body compiles for both ranks, and are always zero here (the kernel tests kRank before reading them).
 struct alignas(64) Conv3dParams {
     static constexpr int kRank = 5;
     static constexpr int kViews = VQB_MAX_VIEWS_3D;
@@ -87,12 +77,6 @@ struct alignas(64) Conv3dParams {
     const void* mask;
     const float* bias;
     float* stats;
-    const __nv_bfloat16* gn_x;
-    const float* gn_mr;
-    const float* gn_gamma;
-    const float* gn_beta;
-    float* gn_cs;
-    int32_t gn_G, gn_lcpg;
 };
 
 template <int BN, class P>
@@ -176,8 +160,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const bool has_bias = p.flags & VQB_EPI_BIAS, has_res = p.flags & VQB_EPI_RES;
     const bool do_relu = !kR5 && (p.flags & VQB_EPI_RELU), has_mask = !kR5 && (p.flags & VQB_EPI_MASK);
     const bool vec_path = p.vec_store != 0;
-    const bool do_gn = !kR5 && p.gn_cs != nullptr;
-    const bool reduce = !kR5 && (p.do_stats || do_gn);
+    const bool reduce = !kR5 && p.do_stats;
     const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.res);
     const __nv_bfloat16* mask = reinterpret_cast<const __nv_bfloat16*>(p.mask);
     float acc[BN / 2];
@@ -226,7 +209,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         const int col0 = n_tile * BN;
         int64_t pix[2];
         bool valid[2];
-        int img[2];
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const uint32_t row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;  // row of the 128-pixel box
@@ -236,13 +218,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                 const int t = (tt << p.lbt) + static_cast<int>((row >> (p.lbw + p.lbh)) & ((1u << p.lbt) - 1));
                 const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh + p.lbt));
                 valid[i] = (w < p.W) && (h < p.H) && (t < p.T) && (n < p.N);
-                img[i] = n;
                 pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(t) * p.ot +
                          static_cast<int64_t>(h) * p.oh + static_cast<int64_t>(w) * p.ow;
             } else {
                 const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh));
                 valid[i] = (w < p.W) && (h < p.H) && (n < p.N);
-                img[i] = n;
                 pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh +
                          static_cast<int64_t>(w) * p.ow;
             }
@@ -281,28 +261,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                     *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.out) + o) = ob;
                     if (reduce) {
                         const float2 v = __bfloat1622float2(ob);  // the bf16 values the consumer will read
-                        if (do_gn) {
-                            const float2 xv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.gn_x + o));
-                            const float* mr = p.gn_mr + static_cast<int64_t>(img[i]) * p.gn_G * 2;
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int c = col + e;
-                                const int g = c >> p.gn_lcpg;
-                                const float xh = ((e ? xv.y : xv.x) - __ldg(mr + 2 * g)) * __ldg(mr + 2 * g + 1);
-                                const float u = fmaf(xh, __ldg(p.gn_gamma + c), __ldg(p.gn_beta + c));
-                                float sg;
-                                asm("tanh.approx.f32 %0, %1;" : "=f"(sg) : "f"(0.5f * u));
-                                sg = fmaf(0.5f, sg, 0.5f);
-                                const float du = (e ? v.y : v.x) * (sg * (1.f + u * (1.f - sg)));
-                                r1[e] += du;
-                                r2[e] = fmaf(du, xh, r2[e]);
-                            }
-                        } else {
-                            r1[0] += v.x;
-                            r2[0] = fmaf(v.x, v.x, r2[0]);
-                            r1[1] += v.y;
-                            r2[1] = fmaf(v.y, v.y, r2[1]);
-                        }
+                        r1[0] += v.x;
+                        r2[0] = fmaf(v.x, v.x, r2[0]);
+                        r1[1] += v.y;
+                        r2[1] = fmaf(v.y, v.y, r2[1]);
                     }
                 } else {
                     // generic strided / ragged path (small or odd Cout, NCHW fp32 outputs)
@@ -339,14 +301,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         if (reduce) {
             // the statistics need every row of the tile inside one image (checked on the host: vqb_conv_stats_ok)
             named_bar_sync(1, 256);
-            float* dst = do_gn ? p.gn_cs : p.stats;
             const int n_img = tn << p.lbn;
             for (uint32_t idx = ctid; idx < BN * 2u; idx += 256u) {
                 const int c = col0 + static_cast<int>(idx >> 1);
                 float v = 0.f;
 #pragma unroll
                 for (int w8 = 0; w8 < kConsumerWarps; ++w8) v += sStat[w8 * BN * 2 + idx];
-                if (c < p.Cout) atomicAdd(dst + (static_cast<int64_t>(n_img) * p.Cout + c) * 2 + (idx & 1u), v);
+                if (c < p.Cout) atomicAdd(p.stats + (static_cast<int64_t>(n_img) * p.Cout + c) * 2 + (idx & 1u), v);
             }
             named_bar_sync(1, 256);  // sStat is reused by the next tile
         }
@@ -390,29 +351,11 @@ static int launch_conv(const P& p, void* stream) {
 using namespace vqb;
 
 static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_packed, const float* bias, const void* res,
-                          const void* mask, void* out, float* stats, void* stream, bool query_only,
-                          const VqbGnBwdFuse* gn = nullptr);
+                          const void* mask, void* out, float* stats, void* stream, bool query_only);
 
 extern "C" int vqb_conv_gemm(const VqbConvDesc* d, const void* a, const void* w_packed, const float* bias,
                              const void* res, const void* mask, void* out, float* stats, void* stream) {
     return conv_gemm_impl(d, a, w_packed, bias, res, mask, out, stats, stream, false);
-}
-
-// Data-gradient launch that also accumulates the statistics of the GroupNorm(+SiLU) backward whose dy it produces.
-extern "C" int vqb_conv_gemm_gnbwd(const VqbConvDesc* d, const void* a, const void* w_packed, const float* bias, void* out,
-                                   const VqbGnBwdFuse* gn, void* stream) {
-    VQB_CHECK(gn && gn->x && gn->mr && gn->gamma && gn->beta && gn->cs && gn->groups > 0,
-              "vqb_conv_gemm_gnbwd: incomplete VqbGnBwdFuse");
-    return conv_gemm_impl(d, a, w_packed, bias, nullptr, nullptr, out, nullptr, stream, false, gn);
-}
-
-// 1 if vqb_conv_gemm_gnbwd supports this descriptor with `groups` GroupNorm groups, else 0.
-extern "C" int vqb_conv_gnbwd_ok(const VqbConvDesc* d, int groups) {
-    if (!d || groups <= 0 || d->Cout % groups != 0) return 0;
-    const int cpg = d->Cout / groups;
-    if ((cpg & (cpg - 1)) != 0) return 0;
-    if (d->flags & (VQB_EPI_RES | VQB_EPI_MASK | VQB_EPI_STATS | VQB_EPI_RELU)) return 0;
-    return vqb_conv_stats_ok(d);  // same geometry conditions: NHWC bf16 output, whole tiles inside one image
 }
 
 // 1 if vqb_conv_gemm can produce GroupNorm statistics (VQB_EPI_STATS) for this descriptor, else 0.
@@ -428,8 +371,7 @@ extern "C" int vqb_conv_stats_ok(const VqbConvDesc* d) {
 }
 
 static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_packed, const float* bias, const void* res,
-                          const void* mask, void* out, float* stats, void* stream, bool query_only,
-                          const VqbGnBwdFuse* gn) {
+                          const void* mask, void* out, float* stats, void* stream, bool query_only) {
     VQB_CHECK(d && a && w_packed && out, "vqb_conv_gemm: null pointer");
     VQB_CHECK(d->C > 0 && d->C % 8 == 0, "vqb_conv_gemm: C=%d must be a positive multiple of 8", d->C);
     VQB_CHECK(d->Cout > 0 && d->N > 0 && d->H > 0 && d->W > 0, "vqb_conv_gemm: bad extents");
@@ -444,8 +386,7 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     if ((d->flags & VQB_EPI_STATS)) VQB_CHECK(stats != nullptr, "vqb_conv_gemm: VQB_EPI_STATS without stats");
     // Paired bf16 stores need 16-byte aligned pixel rows. A channel-contiguous output without them (e.g. NCHW bf16 of
     // 1x1 images: oc = H*W = 1, on = Cout) takes the per-element store instead.
-    const uintptr_t ops = reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(mask) |
-                          reinterpret_cast<uintptr_t>(gn ? gn->x : nullptr);
+    const uintptr_t ops = reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(mask);
     const bool nhwc_bf16 = d->oc == 1 && !d->out_f32 && d->on % 8 == 0 && d->oh % 8 == 0 && d->ow % 8 == 0 &&
                            (reinterpret_cast<uintptr_t>(out) & 15u) == 0 && (ops & 3u) == 0;
     if (!nhwc_bf16)
@@ -482,24 +423,6 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     }
     p.do_stats = (d->flags & VQB_EPI_STATS) ? 1 : 0;
     if (query_only) return stats_ok ? 1 : 0;
-    p.gn_x = nullptr;
-    p.gn_mr = p.gn_gamma = p.gn_beta = nullptr;
-    p.gn_cs = nullptr;
-    p.gn_G = p.gn_lcpg = 0;
-    if (gn) {
-        const int cpg = d->Cout / gn->groups;
-        VQB_CHECK(stats_ok && d->Cout % gn->groups == 0 && (cpg & (cpg - 1)) == 0 &&
-                      !(d->flags & (VQB_EPI_RES | VQB_EPI_MASK | VQB_EPI_STATS | VQB_EPI_RELU)),
-                  "vqb_conv_gemm_gnbwd: unsupported shape / flags (N=%d H=%d W=%d Cout=%d groups=%d)", d->N, d->H, d->W,
-                  d->Cout, gn->groups);
-        p.gn_x = static_cast<const __nv_bfloat16*>(gn->x);
-        p.gn_mr = gn->mr;
-        p.gn_gamma = gn->gamma;
-        p.gn_beta = gn->beta;
-        p.gn_cs = gn->cs;
-        p.gn_G = gn->groups;
-        p.gn_lcpg = ilog2(static_cast<uint32_t>(cpg));
-    }
     const int stage_bytes = kABytes + block_n * kBlockK * 2;
     const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages;
     int stages = (227 * 1024 - fixed) / stage_bytes;
@@ -589,7 +512,7 @@ extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void
     if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_conv3d_gemm: current device is not sm_90");
 
     Conv3dParams p;
-    memset(&p, 0, sizeof(p));  // statistics / GroupNorm / mask fields stay zero (rank-5 epilogue: bias + residual)
+    memset(&p, 0, sizeof(p));  // statistics / mask fields stay zero (rank-5 epilogue: bias + residual)
     const int block_n = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : (d->Cout > 16 ? 32 : 16));
     p.n_tiles = (d->Cout + block_n - 1) / block_n;
     // voxel box per CTA tile: 128 output voxels, as wide as the video (<= 128), then as tall, then as deep, then across

@@ -1,5 +1,5 @@
 // HBM-bound kernels of the VAE path: layout conversion at the module boundary, weight packing,
-// fused GroupNorm(+SiLU) forward / backward, nearest-2x up-sampling, bias gradients, wgrad split
+// fused GroupNorm(+SiLU) forward / backward, bias gradients, wgrad split
 // reduction. All activations are NHWC bf16 with C % 8 == 0; every thread moves 16-byte vectors and
 // owns a FIXED 8-channel slot (its channel vector index never changes while it strides over pixels),
 // so per-channel affine terms / reductions stay in registers.
@@ -11,8 +11,6 @@
 #endif
 #include "common.cuh"
 #include "ptx.cuh"
-
-#include <cstdlib>
 
 namespace vqb {
 
@@ -313,7 +311,6 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat
 
 // ------------------------------------------------------------------ GroupNorm backward
 // per-(n,channel) sums of du and du*xhat, du = dy * silu'(u), u = xhat*gamma + beta
-template <int U>
 __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
                                      const float* __restrict__ mr, const float* __restrict__ gamma,
                                      const float* __restrict__ beta, float* __restrict__ cs /* [N][C][2] */, int HW,
@@ -343,6 +340,7 @@ __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, const 
         const int64_t base = (static_cast<int64_t>(n) * HW) * C + cv * 8;
         // 4 pixel rows (8 x 16-byte loads) in flight per thread: with few warps per SM, fewer rows leave the kernel
         // waiting on load latency instead of streaming HBM
+        constexpr int U = 4;
         for (int p = p0 + pr; p < p1; p += U * R) {
             uint4 ux[U], ud[U];
 #pragma unroll
@@ -487,297 +485,6 @@ gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
     if (colsum) {
         __syncthreads();
         for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(&colsum[i], sm[i]);
-    }
-}
-
-
-// ------------------------------------------------------------------ GroupNorm backward, persistent L2-pipelined form
-// One persistent launch does reduce AND apply. The two-kernel form reads x and dy twice from HBM (10 B/element, 12 with
-// the skip gradient). Here the work is ordered  R(0) R(1) A(0) R(2) A(1) ... A(N-1)  (R(n) = statistics of sample n,
-// A(n) = dx of sample n): when A(n) re-reads x, dy of sample n they were streamed at most one sample ago and (for layers
-// whose x + dy of one sample fit VQB_GNP_MB, default 20 MB: two samples within the H100's 50 MB L2) are still L2 resident
-// — HBM traffic drops to read-once + write-once = 6 (8) B/element. R loads carry an L2 evict_last policy, A loads / dx stores evict_first.
-// Sync: R units add their per-channel partials to cs[n] (fp32 atomics) and bump done[n]; A units spin (acquire) until
-// done[n] == units. Every CTA walks the same global order and only ever waits on work that precedes its own position in
-// every CTA's list, and the grid is sized to be fully co-resident, so the wait cannot deadlock.
-//
-// Per element (trimmed: the reduce kernel sat on the FP32-issue / SFU limit):  h = x*a2 + b2 (= u/2), t = tanh(h),
-// 2*silu'(u) = (1 + t) * (1 + h - h*t);  du2 = dy * that;  S_du = sum du2 / 2,  S_duxh = rstd/2 * sum du2*(x - mean);
-// dx = du2*(gamma*rstd/2) - rstd*gS1 - (x - mean)*rstd^2*gS2 (+ add).
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ uint4 ldg16_hint(const __nv_bfloat16* ptr, uint64_t pol) {
-    uint4 v;
-    asm volatile("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
-                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-                 : "l"(ptr), "l"(pol));
-    return v;
-}
-__device__ __forceinline__ void stg16_hint(__nv_bfloat16* ptr, const uint4& v, uint64_t pol) {
-    asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(ptr), "r"(v.x), "r"(v.y), "r"(v.z),
-                 "r"(v.w), "l"(pol)
-                 : "memory");
-}
-__device__ __forceinline__ float tanh_approx(float x) {
-    float t;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(x));
-    return t;
-}
-
-template <bool ADD, bool SILU>
-__global__ void __launch_bounds__(256, 2)
-gn_bwd_persistent_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
-                         const __nv_bfloat16* __restrict__ add, __nv_bfloat16* __restrict__ dx,
-                         const float* __restrict__ mr, const float* __restrict__ gamma, const float* __restrict__ beta,
-                         float* cs /* [N][C][2], zeroed */, int* done /* [groups], zeroed */,
-                         float* __restrict__ colsum, int N, int HW, int C, int G, int S /* samples per group */,
-                         int ups /* units per sample */, int pix_per_unit, int depth, int hints) {
-    extern __shared__ float sm[];  // [2C] partial sums | [C] dx column sums ; then [2G] group sums
-    float* sm_gs = sm + 2 * C;
-    const int V = C >> 3, R = blockDim.x / V;
-    const int cv = threadIdx.x % V, pr = threadIdx.x / V;
-    const int cpg = C / G;
-    const uint64_t pol_keep = l2_policy_evict_last(), pol_drop = l2_policy_evict_first();
-    const int ngroups = (N + S - 1) / S;
-    float csum[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) csum[j] = 0.f;
-
-    for (int step = 0; step < ngroups + depth; ++step) {
-        // ---------------------------------------------------------------- R(step): statistics of sample group `step`
-        if (step < ngroups) {
-            const int n0 = step * S, ns = min(S, N - n0), units = ns * ups;
-            for (int u = blockIdx.x; u < units; u += gridDim.x) {
-                const int n = n0 + u / ups, ch = u % ups;
-                float mean[8], a2[8], b2[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int g = (cv * 8 + j) / cpg;
-                    mean[j] = mr[(n * G + g) * 2];
-                    const float a = __ldg(gamma + cv * 8 + j) * mr[(n * G + g) * 2 + 1];
-                    a2[j] = 0.5f * a;
-                    b2[j] = 0.5f * (__ldg(beta + cv * 8 + j) - mean[j] * a);
-                }
-                const int64_t base = (static_cast<int64_t>(n) * HW) * C + cv * 8;
-                for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sm[i] = 0.f;
-                __syncthreads();
-                float s1[8], s2[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) s1[j] = s2[j] = 0.f;
-                const int p0 = ch * pix_per_unit, p1 = min(HW, p0 + pix_per_unit);
-                for (int p = p0 + pr; p < p1; p += 3 * R) {
-                    uint4 ux[3], ud[3];
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        const bool in = (p + k * R) < p1;
-                        const __nv_bfloat16* xp = x + base + static_cast<int64_t>(p + k * R) * C;
-                        const __nv_bfloat16* dp = dy + base + static_cast<int64_t>(p + k * R) * C;
-                        ux[k] = in ? (hints ? ldg16_hint(xp, pol_keep) : ldg16(xp)) : make_uint4(0, 0, 0, 0);
-                        ud[k] = in ? (hints ? ldg16_hint(dp, pol_keep) : ldg16(dp)) : make_uint4(0, 0, 0, 0);
-                    }
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        if ((p + k * R) >= p1) break;
-                        float f[8], d[8];
-                        cvt8(ux[k], f);
-                        cvt8(ud[k], d);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            float du2 = 2.f * d[j];
-                            if (SILU) {
-                                const float h = fmaf(f[j], a2[j], b2[j]);
-                                const float t = tanh_approx(h);
-                                const float r = fmaf(-h, t, h + 1.f);
-                                du2 = d[j] * fmaf(t, r, r);
-                            }
-                            s1[j] += du2;
-                            s2[j] = fmaf(du2, f[j] - mean[j], s2[j]);
-                        }
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    atomicAdd(&sm[(cv * 8 + j) * 2], s1[j]);
-                    atomicAdd(&sm[(cv * 8 + j) * 2 + 1], s2[j]);
-                }
-                __syncthreads();
-                for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
-                    const int g = (i >> 1) / cpg;
-                    const float rstd = mr[(n * G + g) * 2 + 1];
-                    // cs[n][c] = (sum du, sum du*xhat)
-                    atomicAdd(&cs[static_cast<int64_t>(n) * 2 * C + i], sm[i] * ((i & 1) ? 0.5f * rstd : 0.5f));
-                }
-                __threadfence();
-                __syncthreads();
-                if (threadIdx.x == 0) atomicAdd(&done[step], 1);
-            }
-        }
-        // ---------------------------------------------------------------- A(step - depth): dx of that sample group
-        if (step >= depth) {
-            const int gi = step - depth;
-            const int n0 = gi * S, ns = min(S, N - n0), units = ns * ups;
-            if (static_cast<int>(blockIdx.x) < units) {
-                if (threadIdx.x == 0) {
-                    int v;
-                    do {
-                        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(done + gi) : "memory");
-                    } while (v < units);
-                }
-                __syncthreads();
-                int cur_n = -1;
-                float mean[8], a2[8], b2[8], k0[8], k2[8];  // (du2 * a2 = du * gamma * rstd)
-                for (int u = blockIdx.x; u < units; u += gridDim.x) {
-                    const int n = n0 + u / ups, ch = u % ups;
-                    if (n != cur_n) {
-                        cur_n = n;
-                        __syncthreads();
-                        // group sums gs[g] = (sum_c gamma_c cs0, sum_c gamma_c cs1) / m from the complete cs[n]
-                        for (int g = threadIdx.x; g < G; g += blockDim.x) {
-                            float a = 0.f, b = 0.f;
-                            for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
-                                a = fmaf(gamma[c], __ldcg(&cs[(static_cast<int64_t>(n) * C + c) * 2]), a);
-                                b = fmaf(gamma[c], __ldcg(&cs[(static_cast<int64_t>(n) * C + c) * 2 + 1]), b);
-                            }
-                            const float m = static_cast<float>(cpg) * HW;
-                            sm_gs[g * 2] = a / m;
-                            sm_gs[g * 2 + 1] = b / m;
-                        }
-                        __syncthreads();
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int g = (cv * 8 + j) / cpg;
-                            mean[j] = mr[(n * G + g) * 2];
-                            const float rstd = mr[(n * G + g) * 2 + 1];
-                            const float a = __ldg(gamma + cv * 8 + j) * rstd;
-                            a2[j] = 0.5f * a;
-                            b2[j] = 0.5f * (__ldg(beta + cv * 8 + j) - mean[j] * a);
-                            k0[j] = -rstd * sm_gs[g * 2];
-                            k2[j] = -rstd * rstd * sm_gs[g * 2 + 1];
-                        }
-                    }
-                    const int64_t base = (static_cast<int64_t>(n) * HW) * C + cv * 8;
-                    const int p0 = ch * pix_per_unit, p1 = min(HW, p0 + pix_per_unit);
-                    constexpr int U = 2;
-                    for (int pp = p0 + pr; pp < p1; pp += U * R) {
-                        uint4 ux[U], ud[U], ua[U];
-#pragma unroll
-                        for (int k = 0; k < U; ++k) {
-                            const bool in = (pp + k * R) < p1;
-                            const int64_t off = base + static_cast<int64_t>(pp + k * R) * C;
-                            ux[k] = in ? (hints ? ldg16_hint(x + off, pol_drop) : ldg16(x + off)) : make_uint4(0, 0, 0, 0);
-                            ud[k] = in ? (hints ? ldg16_hint(dy + off, pol_drop) : ldg16(dy + off)) : make_uint4(0, 0, 0, 0);
-                            if (ADD) ua[k] = in ? ldg16(add + off) : make_uint4(0, 0, 0, 0);
-                        }
-#pragma unroll
-                        for (int k = 0; k < U; ++k) {
-                            if ((pp + k * R) >= p1) break;
-                            float f[8], d[8], r8[8];
-                            cvt8(ux[k], f);
-                            cvt8(ud[k], d);
-                            if (ADD) cvt8(ua[k], r8);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                float du2 = 2.f * d[j];
-                                if (SILU) {
-                                    const float h = fmaf(f[j], a2[j], b2[j]);
-                                    const float t = tanh_approx(h);
-                                    const float r = fmaf(-h, t, h + 1.f);
-                                    du2 = d[j] * fmaf(t, r, r);
-                                }
-                                float v = fmaf(du2, a2[j], fmaf(f[j] - mean[j], k2[j], k0[j]));
-                                if (ADD) v += r8[j];
-                                f[j] = v;
-                                csum[j] += __bfloat162float(__float2bfloat16(v));
-                            }
-                            uint4 o;
-                            o.x = pack_bf16x2(f[0], f[1]);
-                            o.y = pack_bf16x2(f[2], f[3]);
-                            o.z = pack_bf16x2(f[4], f[5]);
-                            o.w = pack_bf16x2(f[6], f[7]);
-                            __nv_bfloat16* op = dx + base + static_cast<int64_t>(pp + k * R) * C;
-                            if (hints) stg16_hint(op, o, pol_drop); else *reinterpret_cast<uint4*>(op) = o;
-                        }
-                    }
-                }
-                __syncthreads();
-            }
-        }
-    }
-    // dx column sums (= bias gradient of the conv that produced x): once per CTA
-    if (colsum) {
-        for (int i = threadIdx.x; i < C; i += blockDim.x) sm[i] = 0.f;
-        __syncthreads();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) atomicAdd(&sm[cv * 8 + j], csum[j]);
-        __syncthreads();
-        for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(&colsum[i], sm[i]);
-    }
-}
-
-// dgamma[c] = sum_n cs[n][c][1], dbeta[c] = sum_n cs[n][c][0]
-__global__ void gn_bwd_param_grads_kernel(const float* __restrict__ cs, float* __restrict__ dgamma,
-                                          float* __restrict__ dbeta, int N, int C) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= C) return;
-    float a = 0.f, b = 0.f;
-    for (int n = 0; n < N; ++n) {
-        a += cs[(static_cast<int64_t>(n) * C + i) * 2];
-        b += cs[(static_cast<int64_t>(n) * C + i) * 2 + 1];
-    }
-    dbeta[i] = a;
-    dgamma[i] = b;
-}
-
-// ------------------------------------------------------------------ nearest 2x up-sampling
-__global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H,
-                                  int W, int C) {
-    const int V = C >> 3;
-    const int64_t total = static_cast<int64_t>(N) * H * W * V;
-    for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
-         i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int cv = static_cast<int>(i % V);
-        const int64_t pix = i / V;
-        const int w = static_cast<int>(pix % W);
-        const int h = static_cast<int>((pix / W) % H);
-        const int64_t n = pix / (static_cast<int64_t>(W) * H);
-        const uint4 u = *reinterpret_cast<const uint4*>(x + pix * C + cv * 8);
-        __nv_bfloat16* o = y + ((n * 2 * H + 2 * h) * 2 * W + 2 * w) * C + cv * 8;
-        *reinterpret_cast<uint4*>(o) = u;
-        *reinterpret_cast<uint4*>(o + C) = u;
-        *reinterpret_cast<uint4*>(o + static_cast<int64_t>(2) * W * C) = u;
-        *reinterpret_cast<uint4*>(o + static_cast<int64_t>(2) * W * C + C) = u;
-    }
-}
-
-// dx[n,h,w,c] = sum of the 2x2 block of dy (fp32 add, one rounding)
-__global__ void upsample2x_bwd_kernel(const __nv_bfloat16* __restrict__ dy, __nv_bfloat16* __restrict__ dx, int N,
-                                      int H, int W, int C) {
-    const int V = C >> 3;
-    const int64_t total = static_cast<int64_t>(N) * H * W * V;
-    for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
-         i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int cv = static_cast<int>(i % V);
-        const int64_t pix = i / V;
-        const int w = static_cast<int>(pix % W);
-        const int h = static_cast<int>((pix / W) % H);
-        const int64_t n = pix / (static_cast<int64_t>(W) * H);
-        const __nv_bfloat16* s = dy + ((n * 2 * H + 2 * h) * 2 * W + 2 * w) * C + cv * 8;
-        float a[8], b[8], c[8], d[8];
-        load8(s, a);
-        load8(s + C, b);
-        load8(s + static_cast<int64_t>(2) * W * C, c);
-        load8(s + static_cast<int64_t>(2) * W * C + C, d);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) a[j] = (a[j] + b[j]) + (c[j] + d[j]);
-        store8(dx + pix * C + cv * 8, a);
     }
 }
 
@@ -1172,89 +879,22 @@ int vqb_gn_silu_fwd_pre(const void* x, void* y, const float* gamma, const float*
 // GroupNorm(+SiLU) backward. ws: >= N*C*2 + N*G*2 floats. dx may alias dy. add (optional) is summed into dx.
 // dx_colsum (optional, [C] fp32, overwritten): per-channel sums of dx over all N*HW pixels, i.e. the bias gradient of the
 // convolution whose output this GroupNorm normalised, produced in the same pass instead of by vqb_colsum.
-static int gn_silu_bwd_impl(const void* x, const void* dy, const void* add, void* dx, const float* gamma,
-                           const float* beta, const float* mr, const float* cs_pre, float* dgamma, float* dbeta, float* ws,
-                           int N, int HW, int C, int G, int silu, float* dx_colsum, void* stream) {
+int vqb_gn_silu_bwd(const void* x, const void* dy, const void* add, void* dx, const float* gamma, const float* beta,
+                    const float* mr, float* dgamma, float* dbeta, float* ws, int N, int HW, int C, int G, int silu,
+                    float* dx_colsum, void* stream) {
     VQB_CHECK(x && dy && dx && gamma && beta && mr && dgamma && dbeta && ws, "vqb_gn_silu_bwd: null pointer");
     VQB_CHECK(C % 8 == 0 && C % G == 0 && C <= 2048, "vqb_gn_silu_bwd: C=%d G=%d unsupported", C, G);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int chunks, ppc;
     const int T = cv_threads(C);
-    const float* cs = cs_pre;
-    float* gsum = ws;
-    // Persistent L2-pipelined form (reduce + apply in one launch, x / dy read from HBM once): used when one sample's
-    // x + dy (+ add) comfortably fits the L2 next to the following sample's, and there is enough work to pipeline.
-    // VQB_GN_BWD_PERSISTENT=1 opts into the persistent form; it has not been measured on the H100 (tools/gn_bwd_bench.py
-    // compares the two), so the default stays the two-kernel form: two 128-register CTAs per SM keep fewer loads in
-    // flight, and every unit pays barrier + fence + atomics.
-    static const int gnp_mode = [] {
-        const char* e = getenv("VQB_GN_BWD_PERSISTENT");
-        return e ? atoi(e) : 0;
-    }();
-    static const int gnp_depth = [] { const char* e = getenv("VQB_GNP_DEPTH"); return e ? atoi(e) : 1; }();
-    static const int gnp_hints = [] { const char* e = getenv("VQB_GNP_HINTS"); return e ? atoi(e) : 1; }();
-    static const int gnp_mb = [] { const char* e = getenv("VQB_GNP_MB"); return e ? atoi(e) : 20; }();
-    const int64_t sample_bytes = static_cast<int64_t>(HW) * C * 2 * (add ? 3 : 2);
-    if (!cs_pre && gnp_mode && T <= 256 && T % (C / 8) == 0 && sample_bytes <= (static_cast<int64_t>(gnp_mb) << 20) &&
-        static_cast<int64_t>(N) * HW * C >= (1 << 18)) {
-        const int V = C / 8, R = T / V;
-        float* csw = ws;                                                   // [N][C][2]
-        int* done = reinterpret_cast<int*>(ws + static_cast<int64_t>(N) * C * 2);  // [<= N] (ws has N*G*2 floats there)
-        VQB_CUDA(cudaMemsetAsync(csw, 0, sizeof(float) * (2 * N * C + N), st));
-        if (dx_colsum) VQB_CUDA(cudaMemsetAsync(dx_colsum, 0, sizeof(float) * C, st));
-        const size_t smem = (2 * C + 2 * G) * sizeof(float);
-        auto launch = [&](auto kern) -> int {
-            int bpsm = 0;
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bpsm, kern, T, smem) != cudaSuccess || bpsm < 1)
-                return set_error(VQB_ECUDA, "vqb_gn_silu_bwd: occupancy query failed");
-            if (bpsm > 2) bpsm = 2;
-            const int grid = (num_sms() > 0 ? num_sms() : 132) * bpsm;
-            // sample groups of S samples whose x + dy (+ add) fit the L2 budget; each group is cut into ~grid units
-            int S = static_cast<int>((static_cast<int64_t>(gnp_mb) << 20) / sample_bytes);
-            if (S < 1) S = 1;
-            if (S > N) S = N;
-            const int min_ppu = R * 4;
-            int ups = (grid + S - 1) / S;  // units per sample
-            if (ups < 1) ups = 1;
-            if (HW / ups < min_ppu) ups = HW / min_ppu > 0 ? HW / min_ppu : 1;
-            int ppu = (HW + ups - 1) / ups;
-            ppu = ((ppu + R - 1) / R) * R;
-            ups = (HW + ppu - 1) / ppu;
-            kern<<<grid, T, smem, st>>>(static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(dy),
-                                        static_cast<const __nv_bfloat16*>(add), static_cast<__nv_bfloat16*>(dx), mr,
-                                        gamma, beta, csw, done, dx_colsum, N, HW, C, G, S, ups, ppu, gnp_depth,
-                                        gnp_hints);
-            return VQB_OK;
-        };
-        int rc;
-        if (add)
-            rc = silu ? launch(gn_bwd_persistent_kernel<true, true>) : launch(gn_bwd_persistent_kernel<true, false>);
-        else
-            rc = silu ? launch(gn_bwd_persistent_kernel<false, true>) : launch(gn_bwd_persistent_kernel<false, false>);
-        if (rc != VQB_OK) return rc;
-        gn_bwd_param_grads_kernel<<<(C + 127) / 128, 128, 0, st>>>(csw, dgamma, dbeta, N, C);
-        VQB_CUDA(cudaGetLastError());
-        count_launch(2);
-        return VQB_OK;
-    }
-    if (!cs_pre) {  // statistics pass (skipped when the consumer conv's data-gradient epilogue produced them)
-        float* csw = ws;
-        gsum = ws + static_cast<int64_t>(N) * C * 2;
-        VQB_CUDA(cudaMemsetAsync(csw, 0, sizeof(float) * 2 * N * C, st));
-        static const int red_u = [] { const char* e = getenv("VQB_GN_RED_U"); return e ? atoi(e) : 4; }();
-        auto launch_red = [&](auto kern) {
-            cv_grid(HW, C, N, kern, 2 * C * sizeof(float), chunks, ppc);
-            kern<<<dim3(chunks, N), T, 2 * C * sizeof(float), st>>>(
-                static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(dy), mr, gamma, beta, csw, HW,
-                C, G, ppc, silu);
-        };
-        if (red_u == 6) launch_red(gn_bwd_reduce_kernel<6>);
-        else if (red_u == 8) launch_red(gn_bwd_reduce_kernel<8>);
-        else if (red_u == 2) launch_red(gn_bwd_reduce_kernel<2>);
-        else launch_red(gn_bwd_reduce_kernel<4>);
-        cs = csw;
-        count_launch();
-    }
+    float* cs = ws;                                      // [N][C][2]
+    float* gsum = ws + static_cast<int64_t>(N) * C * 2;  // [N][G][2]
+    VQB_CUDA(cudaMemsetAsync(cs, 0, sizeof(float) * 2 * N * C, st));
+    cv_grid(HW, C, N, gn_bwd_reduce_kernel, 2 * C * sizeof(float), chunks, ppc);
+    gn_bwd_reduce_kernel<<<dim3(chunks, N), T, 2 * C * sizeof(float), st>>>(
+        static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(dy), mr, gamma, beta, cs, HW, C, G,
+        ppc, silu);
+    count_launch();
     const int fin = (N * G > C ? N * G : C);
     gn_bwd_finalize_kernel<<<(fin + 127) / 128, 128, 0, st>>>(cs, gamma, gsum, dgamma, dbeta, N, C, G, HW);
     const size_t cs_smem = dx_colsum ? C * sizeof(float) : 0;
@@ -1274,20 +914,6 @@ static int gn_silu_bwd_impl(const void* x, const void* dy, const void* add, void
     VQB_CUDA(cudaGetLastError());
     count_launch(2);
     return VQB_OK;
-}
-
-int vqb_gn_silu_bwd(const void* x, const void* dy, const void* add, void* dx, const float* gamma, const float* beta,
-                    const float* mr, float* dgamma, float* dbeta, float* ws, int N, int HW, int C, int G, int silu,
-                    float* dx_colsum, void* stream) {
-    return gn_silu_bwd_impl(x, dy, add, dx, gamma, beta, mr, nullptr, dgamma, dbeta, ws, N, HW, C, G, silu, dx_colsum,
-                            stream);
-}
-
-int vqb_gn_silu_bwd_pre(const void* x, const void* dy, const void* add, void* dx, const float* gamma, const float* beta,
-                        const float* mr, const float* cs, float* dgamma, float* dbeta, float* ws, int N, int HW, int C,
-                        int G, int silu, float* dx_colsum, void* stream) {
-    VQB_CHECK(cs, "vqb_gn_silu_bwd_pre: null cs");
-    return gn_silu_bwd_impl(x, dy, add, dx, gamma, beta, mr, cs, dgamma, dbeta, ws, N, HW, C, G, silu, dx_colsum, stream);
 }
 
 int vqb_wavelet_fwd(const float* x, void* y, const float* filt, int N, int C, int H, int W, int Cpad, void* stream) {
@@ -1310,26 +936,6 @@ int vqb_wavelet_fwd_bf16(const void* x, void* y, const float* filt, int N, int C
     const int64_t total = static_cast<int64_t>(N) * (H / 2) * (W / 2);
     wavelet_fwd_kernel<__nv_bfloat16><<<gs_blocks(total, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), filt, N, C, H, W, Cpad);
-    VQB_CUDA(cudaGetLastError());
-    count_launch();
-    return VQB_OK;
-}
-
-int vqb_upsample2x_fwd(const void* x, void* y, int N, int H, int W, int C, void* stream) {
-    VQB_CHECK(x && y && C % 8 == 0, "vqb_upsample2x_fwd: bad arguments");
-    const int64_t total = static_cast<int64_t>(N) * H * W * (C / 8);
-    upsample2x_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), N, H, W, C);
-    VQB_CUDA(cudaGetLastError());
-    count_launch();
-    return VQB_OK;
-}
-
-int vqb_upsample2x_bwd(const void* dy, void* dx, int N, int H, int W, int C, void* stream) {
-    VQB_CHECK(dy && dx && C % 8 == 0, "vqb_upsample2x_bwd: bad arguments");
-    const int64_t total = static_cast<int64_t>(N) * H * W * (C / 8);
-    upsample2x_bwd_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const __nv_bfloat16*>(dy), static_cast<__nv_bfloat16*>(dx), N, H, W, C);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;

@@ -44,11 +44,6 @@ class VqbWgradDesc(C.Structure):
                 ("views", VqbView * VQB_MAX_VIEWS), ("taps", VqbTap * VQB_MAX_TAPS)]
 
 
-class VqbGnBwdFuse(C.Structure):
-    _fields_ = [("x", C.c_void_p), ("mr", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("cs", C.c_void_p),
-                ("groups", C.c_int32), ("_pad", C.c_int32)]
-
-
 class VqbPackJob(C.Structure):
     _fields_ = [("w", C.c_void_p), ("out", C.c_void_p), ("tapmap", C.c_void_p), ("Cout", C.c_int32), ("Cin", C.c_int32),
                 ("T", C.c_int32), ("nslots", C.c_int32), ("transpose", C.c_int32), ("Kpad", C.c_int32),
@@ -102,9 +97,6 @@ def load():
         "vqb_kernel_launch_count": (i32, []),
         "vqb_wgrad_cols": (i32, [i32, i32]),
         "vqb_conv_gemm": (i32, [C.POINTER(VqbConvDesc), vp, vp, vp, vp, vp, vp, vp, vp]),
-        "vqb_conv_gemm_gnbwd": (i32, [C.POINTER(VqbConvDesc), vp, vp, vp, vp, C.POINTER(VqbGnBwdFuse), vp]),
-        "vqb_conv_gnbwd_ok": (i32, [C.POINTER(VqbConvDesc), i32]),
-        "vqb_gn_silu_bwd_pre": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp]),
         "vqb_wgrad_gemm": (i32, [C.POINTER(VqbWgradDesc), vp, vp, vp, vp]),
         "vqb_pack_weights": (i32, [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp]),
         "vqb_nchw_to_nhwc": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]),
@@ -112,8 +104,6 @@ def load():
         "vqb_gn_silu_fwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, vp]),
         "vqb_gn_silu_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp]),
         "vqb_wavelet_fwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
-        "vqb_upsample2x_fwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),
-        "vqb_upsample2x_bwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),
         "vqb_colsum": (i32, [vp, vp, i64, i32, vp]),
         "vqb_wgrad_reduce": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]),
         "vqb_maxpool2_fwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),

@@ -336,53 +336,6 @@ def choose_ksplit(g: plans.ConvGeom, Cout_pad: int) -> int:
     return best
 
 
-class GnLink:
-    """Connects a GroupNorm(+swish) forward to the conv that consumes its output, so that the conv's data-gradient
-    launch can accumulate the GroupNorm-backward statistics in its epilogue (vqb_conv_gemm_gnbwd) and the GroupNorm
-    backward can skip its reduction pass. Filled by GroupNormSiLUFn.forward (x, mr, gamma, beta, groups); `sums` is set by
-    ConvFn.backward as (cs, dy data_ptr, dy version, strong ref to dy) and consumed once by GroupNormSiLUFn.backward."""
-
-    __slots__ = ("x", "mr", "gamma", "beta", "groups", "silu", "sums")
-
-    def __init__(self):
-        self.x = self.mr = self.gamma = self.beta = None
-        self.groups, self.silu, self.sums = 0, False, None
-
-
-# Opt-in (VQB_GN_BWD_FUSE=1): the extra epilogue work runs on the MMA warpgroups of the conv, and whether the saved
-# GroupNorm reduction pass pays for it has not been measured on the H100; kept, with its parity test.
-_GN_BWD_FUSE = os.environ.get("VQB_GN_BWD_FUSE", "0") == "1"
-_GN_BWD_FUSE_MIN_C = int(os.environ.get("VQB_GN_BWD_FUSE_MIN_C", "0"))
-
-
-def conv_gnbwd_supported(g: plans.ConvGeom, Cout: int, out_strides, groups: int) -> bool:
-    descs = g.__dict__.setdefault("_descs", {})
-    key = ("gnbwd_ok", Cout, tuple(out_strides), groups)
-    ok = descs.get(key)
-    if ok is None:
-        ok = bool(_L().vqb_conv_gnbwd_ok(plans.conv_desc(g, Cout, out_strides, 0, False), groups))
-        descs[key] = ok
-    return ok
-
-
-gnbwd_fused_launches = 0  # how many data-gradient launches carried fused GroupNorm-backward statistics (tests)
-
-
-def run_conv_gemm_gnbwd(g: plans.ConvGeom, a, wp, Cout, out, out_strides, link: "GnLink", cs):
-    global gnbwd_fused_launches
-    gnbwd_fused_launches += 1
-    dk = (Cout, tuple(out_strides), 0, False)
-    descs = g.__dict__.setdefault("_descs", {})
-    d = descs.get(dk)
-    if d is None:
-        d = plans.conv_desc(g, Cout, out_strides, 0, False)
-        descs[dk] = d
-    ga, be = link.gamma.detach(), link.beta.detach()
-    fuse = native.VqbGnBwdFuse(x=ptr(link.x), mr=ptr(link.mr), gamma=ptr(ga), beta=ptr(be), cs=ptr(cs),
-                               groups=link.groups, _pad=0)
-    check(_L().vqb_conv_gemm_gnbwd(d, ptr(a), ptr(wp), 0, ptr(out), fuse, stream_ptr()), "conv_gemm_gnbwd")
-
-
 def run_conv_gemm(g: plans.ConvGeom, a: torch.Tensor, wp: torch.Tensor, Cout: int, out: torch.Tensor, out_strides,
                   out_ptr_offset_bytes=0, bias=None, res=None, mask=None, relu=False, out_f32=False, stats=None):
     flags = (EPI_BIAS if bias is not None else 0) | (EPI_RES if res is not None else 0) | \
@@ -533,10 +486,6 @@ _fat_state = {"ok": None}
 def fat_conv_enabled() -> bool:
     """One-time self check of the fat-pixel first-layer path (it relies on a TMA map whose pixel stride (16 B) is smaller
     than its 48-byte inner extent): run a tiny conv both ways; disable the path on any error or mismatch."""
-    import os
-
-    if os.environ.get("VQB_FAT_CONV", "1") != "1":
-        return False
     if _fat_state["ok"] is None:
         _fat_state["ok"] = False
         # normal tensors even when the first caller runs under torch.inference_mode() (the pack cache reads _version)
@@ -617,8 +566,7 @@ class ConvFn(torch.autograd.Function):
     epilogue), nchw_out (write [N,Cout,H,W] in the weight's dtype, fp32 or bf16, directly: encoder z / decoder image)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, residual, cache, kind, relu, input_is_relu, nchw_out, want_stats=False,
-                gn_link=None):
+    def forward(ctx, x, weight, bias, residual, cache, kind, relu, input_is_relu, nchw_out, want_stats=False):
         require_cuda(x)
         N, H, W, Cp = x.shape
         Cout, Cin, KH, KW = weight.shape
@@ -664,7 +612,6 @@ class ConvFn(torch.autograd.Function):
         ctx.cache, ctx.kind, ctx.g = cache, kind, g
         ctx.has_bias, ctx.has_res = bias is not None, residual is not None
         ctx.input_is_relu, ctx.nchw_out = input_is_relu, nchw_out
-        ctx.gn_link = gn_link if _GN_BWD_FUSE else None
         if want_stats and not nchw_out:
             if stats is None:
                 stats = torch.empty(0, device=x.device)  # "not available" marker
@@ -719,18 +666,7 @@ class ConvFn(torch.autograd.Function):
             elif kind == "s1":
                 gd = cache.geom(("d", N, H, W), lambda: plans.geom_s1_dgrad(N, H, W, Cop, KH))
                 wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
-                link = ctx.gn_link
-                ostr = plans.nhwc_strides(H, W, Cp)
-                if (link is not None and mask is None and Cp == Cin and Cin >= _GN_BWD_FUSE_MIN_C and link.silu
-                        and link.x is not None
-                        and link.x.shape == gx.shape and conv_gnbwd_supported(gd, Cin, ostr, link.groups)):
-                    # this data gradient IS the dy of the GroupNorm(+swish) that produced x: its epilogue also
-                    # accumulates that GroupNorm's backward statistics (the separate reduction pass disappears)
-                    cs = torch.zeros(N, Cin, 2, device=x.device, dtype=torch.float32)
-                    run_conv_gemm_gnbwd(gd, dy, wpd, Cin, gx, ostr, link, cs)
-                    link.sums = (cs, gx.data_ptr(), gx._version, gx)
-                else:
-                    run_conv_gemm(gd, dy, wpd, Cin, gx, ostr, mask=mask)
+                run_conv_gemm(gd, dy, wpd, Cin, gx, plans.nhwc_strides(H, W, Cp), mask=mask)
             elif kind == "s2":
                 for ph, pw, gd in cache.geom(("d", N, H, W), lambda: plans.geom_s2_dgrad_classes(N, H, W, Cop)):
                     wpd = cache.get(weight, ("dgrad", kind, ph, pw), gd.tapmap, True, Cop)
@@ -763,17 +699,16 @@ class ConvFn(torch.autograd.Function):
                 gb = colsum(rows, dy, Cop)[:Cout]
         if ctx.has_res and ctx.needs_input_grad[3]:
             gres = dy
-        return gx, gw, gb, gres, None, None, None, None, None, None, None
+        return gx, gw, gb, gres, None, None, None, None, None, None
 
 
 def conv(x, weight, bias, cache, kind="s1", residual=None, relu=False, input_is_relu=False, nchw_out=False,
-         want_stats=False, gn_link=None):
-    """-> out, or (out, stats) when want_stats (stats is None if the epilogue cannot produce them for this shape).
-    gn_link: the GnLink of the GroupNorm(+swish) whose output `x` is (fused GroupNorm-backward statistics)."""
+         want_stats=False):
+    """-> out, or (out, stats) when want_stats (stats is None if the epilogue cannot produce them for this shape)."""
     if want_stats and not nchw_out:
-        out, st = ConvFn.apply(x, weight, bias, residual, cache, kind, relu, input_is_relu, nchw_out, True, gn_link)
+        out, st = ConvFn.apply(x, weight, bias, residual, cache, kind, relu, input_is_relu, nchw_out, True)
         return out, (st if st.numel() > 0 else None)
-    return ConvFn.apply(x, weight, bias, residual, cache, kind, relu, input_is_relu, nchw_out, False, gn_link)
+    return ConvFn.apply(x, weight, bias, residual, cache, kind, relu, input_is_relu, nchw_out, False)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -865,9 +800,6 @@ def upsample_conv(x, weight, bias, cache, want_stats=False):
     return UpConvFn.apply(x, weight, bias, cache, False)
 
 
-_GN_COLSUM = os.environ.get("VQB_GN_COLSUM", "1") == "1"
-
-
 class GroupNormSiLUFn(torch.autograd.Function):
     """FP32GroupNorm (32 groups, eps 1e-6, biased variance, fp32 statistics; ae.py:41-53) fused with swish
     (ae.py:13-14): one statistics pass + one apply pass over bf16 NHWC, instead of cast/GN/cast/sigmoid/mul.
@@ -877,7 +809,7 @@ class GroupNormSiLUFn(torch.autograd.Function):
     autograd accumulation kernel."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, groups, eps, silu, with_skip, chsums=None, link=None):
+    def forward(ctx, x, gamma, beta, groups, eps, silu, with_skip, chsums=None):
         require_cuda(x)
         x = x.contiguous()
         N, H, W, C = x.shape
@@ -893,9 +825,6 @@ class GroupNormSiLUFn(torch.autograd.Function):
                                        1 if silu else 0, stream_ptr()), "gn_silu_fwd")
         ctx.save_for_backward(x, gamma, beta, mr)
         ctx.groups, ctx.silu, ctx.with_skip = groups, silu, with_skip
-        ctx.link = link
-        if link is not None:
-            link.x, link.mr, link.gamma, link.beta, link.groups, link.silu = x, mr, gamma, beta, groups, bool(silu)
         ctx.set_materialize_grads(False)  # an unused output arrives as None, not as a zero tensor
         if with_skip:
             return y, x.view_as(x)
@@ -907,61 +836,23 @@ class GroupNormSiLUFn(torch.autograd.Function):
         inference_only(gamma, beta)
         N, H, W, C = x.shape
         if gy is None:  # only the skip output was used
-            return (gskip, None, None, None, None, None, None, None, None)
+            return (gskip, None, None, None, None, None, None, None)
         gy = gy.contiguous()
         add = gskip.contiguous() if gskip is not None else None
         dx = torch.empty_like(x)
         dg, db = grad_out(gamma), grad_out(beta)
         ws = torch.empty(N * C * 2 + N * ctx.groups * 2, device=x.device, dtype=torch.float32)
         ga, be = gamma.detach().float(), beta.detach().float()
-        cs = torch.empty(C, device=x.device, dtype=torch.float32) if _GN_COLSUM else None
-        pre = None
-        link = ctx.link
-        if link is not None and link.sums is not None:
-            pcs, dptr, dver, dref = link.sums
-            link.sums = None
-            if dptr == gy.data_ptr() and dref.shape == gy.shape and gy._version == dver and pcs.shape == (N, C, 2):
-                pre = pcs  # the consumer conv's data-gradient epilogue already accumulated (sum du, sum du*xhat)
-        if link is not None:
-            link.x = link.mr = link.gamma = link.beta = None  # drop the references once the backward ran
-        if pre is not None:
-            check(_L().vqb_gn_silu_bwd_pre(ptr(x), ptr(gy), ptr(add), ptr(dx), ptr(ga), ptr(be), ptr(mr), ptr(pre),
-                                           ptr(dg), ptr(db), ptr(ws), N, H * W, C, ctx.groups, 1 if ctx.silu else 0,
-                                           ptr(cs), stream_ptr()), "gn_silu_bwd_pre")
-        else:
-            check(_L().vqb_gn_silu_bwd(ptr(x), ptr(gy), ptr(add), ptr(dx), ptr(ga), ptr(be), ptr(mr), ptr(dg), ptr(db),
-                                       ptr(ws), N, H * W, C, ctx.groups, 1 if ctx.silu else 0, ptr(cs), stream_ptr()),
-                  "gn_silu_bwd")
-        _dx_colsum_slot[0] = (dx, dx._version, cs) if cs is not None else None
-        return dx, dg, db, None, None, None, None, None, None
+        cs = torch.empty(C, device=x.device, dtype=torch.float32)
+        check(_L().vqb_gn_silu_bwd(ptr(x), ptr(gy), ptr(add), ptr(dx), ptr(ga), ptr(be), ptr(mr), ptr(dg), ptr(db),
+                                   ptr(ws), N, H * W, C, ctx.groups, 1 if ctx.silu else 0, ptr(cs), stream_ptr()),
+              "gn_silu_bwd")
+        _dx_colsum_slot[0] = (dx, dx._version, cs)
+        return dx, dg, db, None, None, None, None, None
 
 
-def group_norm_silu(x, gamma, beta, groups=32, eps=1e-6, silu=True, with_skip=False, chsums=None, link=None):
-    return GroupNormSiLUFn.apply(x, gamma, beta, groups, eps, silu, with_skip, chsums, link)
-
-
-class Upsample2xFn(torch.autograd.Function):
-    """nearest x2 (ae.py:165); backward = 2x2 sum."""
-
-    @staticmethod
-    def forward(ctx, x):
-        x = x.contiguous()
-        N, H, W, C = x.shape
-        y = torch.empty(N, 2 * H, 2 * W, C, device=x.device, dtype=x.dtype)
-        check(_L().vqb_upsample2x_fwd(ptr(x), ptr(y), N, H, W, C, stream_ptr()), "upsample2x_fwd")
-        return y
-
-    @staticmethod
-    def backward(ctx, gy):
-        gy = gy.contiguous()
-        N, H2, W2, C = gy.shape
-        gx = torch.empty(N, H2 // 2, W2 // 2, C, device=gy.device, dtype=gy.dtype)
-        check(_L().vqb_upsample2x_bwd(ptr(gy), ptr(gx), N, H2 // 2, W2 // 2, C, stream_ptr()), "upsample2x_bwd")
-        return gx
-
-
-def upsample2x(x):
-    return Upsample2xFn.apply(x)
+def group_norm_silu(x, gamma, beta, groups=32, eps=1e-6, silu=True, with_skip=False, chsums=None):
+    return GroupNormSiLUFn.apply(x, gamma, beta, groups, eps, silu, with_skip, chsums)
 
 
 class MaxPool2Fn(torch.autograd.Function):
