@@ -249,12 +249,66 @@ int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void* w_packed 
                     const float* bias, const void* res, void* out, void* stream);
 
 /*
+ * Training of tae.TVAE (opt-in through tae.enable_training; fp32 master weights). The data gradients of the 3x3x3
+ * stride-1 conv (27 rotated taps over dy, transposed weights) and of the stride-2 Downsample conv (one conv of 1 to 8
+ * taps per parity class of dx, written through strided voxel addressing) run through vqb_conv3d_gemm. The data gradient
+ * of the folded nearest-x2 up-sampling (tae.py:110-116) is inherently 4 (offset, folded weight) terms per axis: 64 taps
+ * over the 8 parity views of dy, more than VqbConv3dDesc holds. VqbConv3dDgradDesc is VqbConv3dDesc with a 64-entry tap
+ * table; vqb_conv3d_dgrad_gemm runs the same rank-5 kernel with no epilogue (flags must be 0) so the 64 taps accumulate
+ * in one fp32 accumulator and are rounded once. Replaces the dgrad half of autograd's convolution_backward for
+ * nn.Conv3d at tae.py:110-116 (Upsample).
+ */
+#define VQB_MAX_TAPS_3D_DGRAD 64
+typedef struct VqbConv3dDgradDesc {
+    int32_t C;          /* channels of dy = K per tap (multiple of 8)               */
+    int32_t Cout;       /* channels of dx written                                    */
+    int32_t N, T, H, W; /* dx voxel grid                                              */
+    int32_t nviews, ntaps;
+    int32_t flags;   /* must be 0                                                */
+    int32_t out_f32; /* 0: dx is bf16, 1: dx is fp32                             */
+    int64_t on, ot, oh, ow, oc;
+    VqbView3d views[VQB_MAX_VIEWS_3D];
+    VqbTap3d taps[VQB_MAX_TAPS_3D_DGRAD];
+} VqbConv3dDgradDesc;
+
+int vqb_conv3d_dgrad_gemm(const VqbConv3dDgradDesc* d, const void* dy, const void* w_packed /* bf16 [Cout][ntaps*C] */,
+                          void* dx, void* stream);
+
+/*
+ * Rank-5 weight gradient  dWp[co][t*C64 + c] = sum_{n,t,h,w} dy[n,t,h,w,co] * X_view(tap)[n, t+dt, h+dh, w+dw, c]:
+ * the split-K wgmma GEMM of vqb_wgrad_gemm with the K walk over 64-voxel boxes [bw][bh][bt][bn] (5-D TMA loads of dy and
+ * of the tap-shifted x views). Up to 27 taps over up to 8 views (the Downsample's 8 parity views; its pad is the TMA zero
+ * fill). ld_override / col_offset as in VqbWgradDesc, so the eight up-sampling phases fill one partial buffer. The fp32
+ * partial [ksplit][Cout][ntaps*C64] is reduced to the OIDHW gradient by vqb_wgrad_reduce (T = 27) or
+ * vqb_wgrad_reduce_fold (T = 27, 64 slots). Replaces the wgrad half of convolution_backward for nn.Conv3d at
+ * tae.py:66-78, :96-104, :110-116, :136-138, :165-167, :208-210, :233.
+ */
+typedef struct VqbWgrad3dDesc {
+    int32_t C;          /* channels of x                         */
+    int32_t Cout;       /* channels of dy                        */
+    int32_t N, T, H, W; /* dy voxel grid                         */
+    int32_t nviews, ntaps;
+    int32_t ksplit, _pad;
+    int64_t ld_override; /* row pitch (floats) of partial; 0 = ntaps*roundup(C,64) */
+    int64_t col_offset;  /* first column of partial this launch writes            */
+    VqbView3d dy_view;   /* normally the dense view of dy                          */
+    VqbView3d views[VQB_MAX_VIEWS_3D];
+    VqbTap3d taps[VQB_MAX_TAPS_3D];
+} VqbWgrad3dDesc;
+
+int vqb_wgrad3d_gemm(const VqbWgrad3dDesc* d, const void* dy, const void* x, float* partial, void* stream);
+
+/*
  * Attention core of tae.AttnBlock (tae.py:26-51: 8 heads of C/8 channels, F.scaled_dot_product_attention with its
  * default scale 1/sqrt(head_dim)): qkv [N][T][3C] bf16 (q | k | v channel blocks, head h owns channels
  * h*head_dim .. of each block) -> out [N][T][C] bf16; lse [N][C/head_dim][T] fp32. head_dim is 32 or 64; any other
  * value is refused with a message naming it. vqb_attn_fwd is this with head_dim = 64.
  */
 int vqb_attn_fwd_hd(const void* qkv, void* out, float* lse, int N, int T, int C, int head_dim, void* stream);
+/* Its backward (autograd of F.scaled_dot_product_attention at tae.py:31-50): dqkv [N][T][3C] bf16 from qkv, out, dout
+ * and lse of the forward; dvec is a workspace of lse's shape. head_dim 32 or 64; vqb_attn_bwd is this with 64. */
+int vqb_attn_bwd_hd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec, void* dqkv,
+                    int N, int T, int C, int head_dim, void* stream);
 
 /*
  * Reparameterisation of tae.DiagonalGaussian (tae.py:259-264): z [N][2Z][S] (NCTHW, S = T*H*W; mean = channels 0..Z-1,
@@ -263,6 +317,11 @@ int vqb_attn_fwd_hd(const void* qkv, void* out, float* lse, int N, int T, int C,
  * reference's own call, so a seeded run consumes the same CUDA RNG stream).
  */
 int vqb_gauss_reparam(const void* z, const void* eps, void* out, int N, int Z, int64_t S, int bf16, void* stream);
+/* Its backward (autograd of tae.py:263-264, fp32 training): g = dL/dout [N][Z][S], z, eps fp32 -> dz [N][2Z][S] fp32 with
+ * dmean = g and dlogvar = g * eps * 0.5 * exp(0.5 * logvar) where logvar >= -3, else 0 (torch's clamp backward: the
+ * gradient passes at exactly -3). */
+int vqb_gauss_reparam_bwd(const float* g, const float* z, const float* eps, float* dz, int N, int Z, int64_t S,
+                          void* stream);
 
 /* out[c] = sum over P pixels of x[p][c] : Conv2d bias gradient */
 int vqb_colsum(const void* x, float* out, int64_t P, int C, void* stream);

@@ -14,7 +14,6 @@
 
 namespace vqb {
 
-constexpr int kHD = 64;   // head dim
 constexpr int kTQ = 64;   // rows per block (4 warps x 16)
 constexpr int kLD = 72;   // smem row pitch in bf16 (144 B: conflict-free 32-bit fragment loads)
 
@@ -182,7 +181,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __re
     }
 }
 
-// D[n][h][q] = sum_d dO * O
+// D[n][h][q] = sum_d dO * O   (HD: head dim, 64 or 32; lane l holds channels 2l, 2l + 1 of the head)
+template <int HD>
 __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ dout,
                                      float* __restrict__ dvec, int T, int C, int heads, int64_t total) {
     const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x / 32) + (threadIdx.x >> 5);  // one warp per (n,q,h)
@@ -190,10 +190,13 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const 
     const int lane = threadIdx.x & 31;
     const int h = static_cast<int>(i % heads);
     const int64_t nq = i / heads;
-    const int64_t off = nq * C + h * kHD + lane * 2;
-    const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(o + off));
-    const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + off));
-    float s = a.x * b.x + a.y * b.y;
+    const int64_t off = nq * C + h * HD + lane * 2;
+    float s = 0.f;
+    if (HD == 64 || lane * 2 < HD) {
+        const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(o + off));
+        const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + off));
+        s = a.x * b.x + a.y * b.y;
+    }
 #pragma unroll
     for (int k = 16; k > 0; k >>= 1) s += __shfl_xor_sync(0xffffffffu, s, k);
     if (lane == 0) {
@@ -203,6 +206,9 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const 
 }
 
 // ------------------------------------------------------------------------------------------------ backward: dK, dV
+// HD as in the forward: K.Q^T and V.dO^T run HD/16 k-steps over 8 query n-tiles; dV and dK run 4 query k-steps over HD/8
+// n-tiles.
+template <int HD>
 __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ qkv,
                                                             const __nv_bfloat16* __restrict__ dout,
                                                             const float* __restrict__ lse,
@@ -219,27 +225,28 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
     const int k0 = blockIdx.x * 64, h = blockIdx.y, n = blockIdx.z, heads = gridDim.y;
     const int64_t ld = 3 * static_cast<int64_t>(C);
     const __nv_bfloat16* base = qkv + static_cast<int64_t>(n) * T * ld;
-    const __nv_bfloat16* dob = dout + static_cast<int64_t>(n) * T * C + h * kHD;
+    constexpr int kKS = HD / 16, kNO = HD / 8;
+    const __nv_bfloat16* dob = dout + static_cast<int64_t>(n) * T * C + h * HD;
     // K and V rows of this warp as A fragments (staged through sQ / sdO once)
-    load_tile(sQ, base + C + h * kHD, ld, k0, T);
-    load_tile(sdO, base + 2 * C + h * kHD, ld, k0, T);
+    load_tile<HD>(sQ, base + C + h * HD, ld, k0, T);
+    load_tile<HD>(sdO, base + 2 * C + h * HD, ld, k0, T);
     __syncthreads();
-    uint32_t ka[4][4], va[4][4];
-    load_a_frags(sQ, warp, lane, ka);
-    load_a_frags(sdO, warp, lane, va);
-    float dk[8][4], dv[8][4];
+    uint32_t ka[kKS][4], va[kKS][4];
+    load_a_frags<kKS>(sQ, warp, lane, ka);
+    load_a_frags<kKS>(sdO, warp, lane, va);
+    float dk[kNO][4], dv[kNO][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < kNO; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) dk[i][j] = dv[i][j] = 0.f;
     const int key_r0 = k0 + warp * 16 + (lane >> 2);
     const int nqt = (T + 63) / 64;
     for (int qt = 0; qt < nqt; ++qt) {
         __syncthreads();
-        load_tile(sQ, base + h * kHD, ld, qt * 64, T);
-        load_tile_t(sQt, base + h * kHD, ld, qt * 64, T);
-        load_tile(sdO, dob, C, qt * 64, T);
-        load_tile_t(sdOt, dob, C, qt * 64, T);
+        load_tile<HD>(sQ, base + h * HD, ld, qt * 64, T);
+        load_tile_t<HD>(sQt, base + h * HD, ld, qt * 64, T);
+        load_tile<HD>(sdO, dob, C, qt * 64, T);
+        load_tile_t<HD>(sdOt, dob, C, qt * 64, T);
         if (threadIdx.x < 64) {
             const int q = qt * 64 + threadIdx.x;
             sLse[threadIdx.x] = q < T ? lse[(static_cast<int64_t>(n) * heads + h) * T + q] : 0.f;
@@ -251,8 +258,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) st[i][j] = dp[i][j] = 0.f;
-        mma_a_bT(st, ka, sQ, lane);   // S^T[key][q] = sum_d K[key][d] Q[q][d]
-        mma_a_bT(dp, va, sdO, lane);  // dP^T[key][q] = sum_d V[key][d] dO[q][d]
+        mma_a_bT<kKS, 8>(st, ka, sQ, lane);   // S^T[key][q] = sum_d K[key][d] Q[q][d]
+        mma_a_bT<kKS, 8>(dp, va, sdO, lane);  // dP^T[key][q] = sum_d V[key][d] dO[q][d]
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -267,17 +274,17 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
         uint32_t pa[4][4], dsa[4][4];
         acc_to_a(st, pa);
         acc_to_a(dp, dsa);
-        mma_a_bT(dv, pa, sdOt, lane);  // dV[key][d] += sum_q P^T[key][q] dO[q][d]
-        mma_a_bT(dk, dsa, sQt, lane);  // dK[key][d] += sum_q dS^T[key][q] Q[q][d]
+        mma_a_bT<4, kNO>(dv, pa, sdOt, lane);  // dV[key][d] += sum_q P^T[key][q] dO[q][d]
+        mma_a_bT<4, kNO>(dk, dsa, sQt, lane);  // dK[key][d] += sum_q dS^T[key][q] Q[q][d]
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int key = key_r0 + r * 8;
         if (key < T) {
-            __nv_bfloat16* kp = dqkv + (static_cast<int64_t>(n) * T + key) * ld + C + h * kHD + (lane & 3) * 2;
+            __nv_bfloat16* kp = dqkv + (static_cast<int64_t>(n) * T + key) * ld + C + h * HD + (lane & 3) * 2;
             __nv_bfloat16* vp = kp + C;
 #pragma unroll
-            for (int nt = 0; nt < 8; ++nt) {
+            for (int nt = 0; nt < kNO; ++nt) {
                 *reinterpret_cast<uint32_t*>(kp + nt * 8) = pack_bf16x2(dk[nt][2 * r], dk[nt][2 * r + 1]);
                 *reinterpret_cast<uint32_t*>(vp + nt * 8) = pack_bf16x2(dv[nt][2 * r], dv[nt][2 * r + 1]);
             }
@@ -286,7 +293,9 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
 }
 
 // ------------------------------------------------------------------------------------------------ backward: dQ
-__global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const __nv_bfloat16* __restrict__ qkv,
+// min-blocks 1 for heads of 32: without it ptxas caps the registers low and spills; heads of 64 keep the default
+template <int HD>
+__global__ void __launch_bounds__(128, HD == 32 ? 1 : 0) attn_bwd_dq_kernel(const __nv_bfloat16* __restrict__ qkv,
                                                           const __nv_bfloat16* __restrict__ dout,
                                                           const float* __restrict__ lse, const float* __restrict__ dvec,
                                                           __nv_bfloat16* __restrict__ dqkv, int T, int C, float scale) {
@@ -297,13 +306,14 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const __nv_bfloat16* _
     const int q0 = blockIdx.x * 64, h = blockIdx.y, n = blockIdx.z, heads = gridDim.y;
     const int64_t ld = 3 * static_cast<int64_t>(C);
     const __nv_bfloat16* base = qkv + static_cast<int64_t>(n) * T * ld;
-    const __nv_bfloat16* dob = dout + static_cast<int64_t>(n) * T * C + h * kHD;
-    load_tile(sK, base + h * kHD, ld, q0, T);
-    load_tile(sV, dob, C, q0, T);
+    constexpr int kKS = HD / 16, kNO = HD / 8;
+    const __nv_bfloat16* dob = dout + static_cast<int64_t>(n) * T * C + h * HD;
+    load_tile<HD>(sK, base + h * HD, ld, q0, T);
+    load_tile<HD>(sV, dob, C, q0, T);
     __syncthreads();
-    uint32_t qa[4][4], doa[4][4];
-    load_a_frags(sK, warp, lane, qa);
-    load_a_frags(sV, warp, lane, doa);
+    uint32_t qa[kKS][4], doa[kKS][4];
+    load_a_frags<kKS>(sK, warp, lane, qa);
+    load_a_frags<kKS>(sV, warp, lane, doa);
     const int qr0 = q0 + warp * 16 + (lane >> 2);
     float lse_r[2], d_r[2];
 #pragma unroll
@@ -312,25 +322,25 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const __nv_bfloat16* _
         lse_r[r] = q < T ? lse[(static_cast<int64_t>(n) * heads + h) * T + q] : 0.f;
         d_r[r] = q < T ? dvec[(static_cast<int64_t>(n) * heads + h) * T + q] : 0.f;
     }
-    float dq[8][4];
+    float dq[kNO][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < kNO; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) dq[i][j] = 0.f;
     const int nkt = (T + 63) / 64;
     for (int kt = 0; kt < nkt; ++kt) {
         __syncthreads();
-        load_tile(sK, base + C + h * kHD, ld, kt * 64, T);
-        load_tile_t(sKt, base + C + h * kHD, ld, kt * 64, T);
-        load_tile(sV, base + 2 * C + h * kHD, ld, kt * 64, T);
+        load_tile<HD>(sK, base + C + h * HD, ld, kt * 64, T);
+        load_tile_t<HD>(sKt, base + C + h * HD, ld, kt * 64, T);
+        load_tile<HD>(sV, base + 2 * C + h * HD, ld, kt * 64, T);
         __syncthreads();
         float s[8][4], dp[8][4];
 #pragma unroll
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-        mma_a_bT(s, qa, sK, lane);    // S[q][key]
-        mma_a_bT(dp, doa, sV, lane);  // dP[q][key] = sum_d dO[q][d] V[key][d]
+        mma_a_bT<kKS, 8>(s, qa, sK, lane);    // S[q][key]
+        mma_a_bT<kKS, 8>(dp, doa, sV, lane);  // dP[q][key] = sum_d dO[q][d] V[key][d]
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -343,18 +353,44 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const __nv_bfloat16* _
             }
         uint32_t dsa[4][4];
         acc_to_a(dp, dsa);
-        mma_a_bT(dq, dsa, sKt, lane);  // dQ[q][d] += sum_key dS[q][key] K[key][d]
+        mma_a_bT<4, kNO>(dq, dsa, sKt, lane);  // dQ[q][d] += sum_key dS[q][key] K[key][d]
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int q = qr0 + r * 8;
         if (q < T) {
-            __nv_bfloat16* qp = dqkv + (static_cast<int64_t>(n) * T + q) * ld + h * kHD + (lane & 3) * 2;
+            __nv_bfloat16* qp = dqkv + (static_cast<int64_t>(n) * T + q) * ld + h * HD + (lane & 3) * 2;
 #pragma unroll
-            for (int nt = 0; nt < 8; ++nt)
+            for (int nt = 0; nt < kNO; ++nt)
                 *reinterpret_cast<uint32_t*>(qp + nt * 8) = pack_bf16x2(dq[nt][2 * r], dq[nt][2 * r + 1]);
         }
     }
+}
+
+template <int HD>
+static int launch_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec,
+                           void* dqkv, int N, int T, int C, float scale, cudaStream_t st) {
+    const int heads = C / HD;
+    const int64_t total = static_cast<int64_t>(N) * T * heads;
+    attn_bwd_prep_kernel<HD><<<static_cast<int>((total + 7) / 8), 256, 0, st>>>(
+        static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), dvec, T, C, heads, total);
+    dim3 grid((T + 63) / 64, heads, N);
+    const size_t smem = 4 * 64 * kLD * sizeof(__nv_bfloat16) + 2 * 64 * sizeof(float);
+    static bool attr = false;
+    if (!attr) {
+        VQB_CUDA(cudaFuncSetAttribute(attn_bwd_dkdv_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      64 * 1024));
+        attr = true;
+    }
+    attn_bwd_dkdv_kernel<HD><<<grid, 128, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv),
+                                                       static_cast<const __nv_bfloat16*>(dout), lse, dvec,
+                                                       static_cast<__nv_bfloat16*>(dqkv), T, C, scale);
+    attn_bwd_dq_kernel<HD><<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv),
+                                                 static_cast<const __nv_bfloat16*>(dout), lse, dvec,
+                                                 static_cast<__nv_bfloat16*>(dqkv), T, C, scale);
+    VQB_CUDA(cudaGetLastError());
+    count_launch(3);
+    return VQB_OK;
 }
 
 }  // namespace vqb
@@ -407,27 +443,26 @@ int vqb_attn_bwd(const void* qkv, const void* out, const void* dout, const float
                  int T, int C, void* stream) {
     VQB_CHECK(qkv && out && dout && lse && dvec && dqkv, "vqb_attn_bwd: null pointer");
     VQB_CHECK(C % 64 == 0 && T > 0 && N > 0, "vqb_attn_bwd: C=%d must be a multiple of the head dim 64", C);
+    return launch_attn_bwd<64>(qkv, out, dout, lse, dvec, dqkv, N, T, C, 0.125f, static_cast<cudaStream_t>(stream));
+}
+
+// Backward of vqb_attn_fwd_hd (autograd of F.scaled_dot_product_attention at tae.py:31-50): heads of head_dim = C/8
+// channels, scale 1/sqrt(head_dim). dqkv [N][T][3C]; dvec: workspace [N][C/head_dim][T] floats.
+int vqb_attn_bwd_hd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec, void* dqkv,
+                    int N, int T, int C, int head_dim, void* stream) {
+    VQB_CHECK(qkv && out && dout && lse && dvec && dqkv, "vqb_attn_bwd_hd: null pointer");
+    VQB_CHECK(head_dim == 32 || head_dim == 64,
+              "vqb_attn_bwd_hd: head_dim=%d is not supported (heads of 32 or 64 channels only)", head_dim);
+    VQB_CHECK(C > 0 && C % head_dim == 0 && T > 0 && N > 0,
+              "vqb_attn_bwd_hd: C=%d must be a positive multiple of head_dim %d (T=%d N=%d)", C, head_dim, T, N);
+    VQB_CHECK(((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out) |
+                reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(dqkv)) & 15u) == 0 &&
+                  ((reinterpret_cast<uintptr_t>(lse) | reinterpret_cast<uintptr_t>(dvec)) & 3u) == 0,
+              "vqb_attn_bwd_hd: qkv / out / dout / dqkv must be 16-byte aligned");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_attn_bwd_hd: current device is not sm_90");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int heads = C / 64;
-    const int64_t total = static_cast<int64_t>(N) * T * heads;
-    attn_bwd_prep_kernel<<<static_cast<int>((total + 7) / 8), 256, 0, st>>>(
-        static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), dvec, T, C, heads, total);
-    dim3 grid((T + 63) / 64, heads, N);
-    const size_t smem = 4 * 64 * kLD * sizeof(__nv_bfloat16) + 2 * 64 * sizeof(float);
-    static bool attr = false;
-    if (!attr) {
-        VQB_CUDA(cudaFuncSetAttribute(attn_bwd_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-        attr = true;
-    }
-    attn_bwd_dkdv_kernel<<<grid, 128, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv),
-                                                   static_cast<const __nv_bfloat16*>(dout), lse, dvec,
-                                                   static_cast<__nv_bfloat16*>(dqkv), T, C, 0.125f);
-    attn_bwd_dq_kernel<<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv),
-                                             static_cast<const __nv_bfloat16*>(dout), lse, dvec,
-                                             static_cast<__nv_bfloat16*>(dqkv), T, C, 0.125f);
-    VQB_CUDA(cudaGetLastError());
-    count_launch(3);
-    return VQB_OK;
+    if (head_dim == 64) return launch_attn_bwd<64>(qkv, out, dout, lse, dvec, dqkv, N, T, C, 0.125f, st);
+    return launch_attn_bwd<32>(qkv, out, dout, lse, dvec, dqkv, N, T, C, 0.17677669529663687f, st);  // 1/sqrt(32)
 }
 
 }  // extern "C"

@@ -52,17 +52,19 @@ struct alignas(64) ConvParams {
 };
 
 // The 3-D (video) form: NTHWC activations, 5-D TMA boxes [64 ch][bw][bh][bt][bn], up to 27 taps over up to 8 views.
-// Inference only: the epilogue has bias and residual; the statistics / ReLU / mask fields exist so that the kernel
-// body compiles for both ranks, and are always zero here (the kernel tests kRank before reading them).
-struct alignas(64) Conv3dParams {
+// The epilogue has bias and residual; the statistics / ReLU / mask fields exist so that the kernel
+// body compiles for both ranks, and are always zero here (the kernel tests kRank before reading them). kTaps is the size
+// of the tap table: 27 (vqb_conv3d_gemm) or 64 (vqb_conv3d_dgrad_gemm, the data gradient of the folded up-sampling).
+template <int kTaps>
+struct alignas(64) Conv3dParamsT {
     static constexpr int kRank = 5;
     static constexpr int kViews = VQB_MAX_VIEWS_3D;
     CUtensorMap amap[VQB_MAX_VIEWS_3D];
     CUtensorMap bmap;
-    int32_t tap_view[VQB_MAX_TAPS_3D];
-    int32_t tap_dw[VQB_MAX_TAPS_3D];
-    int32_t tap_dh[VQB_MAX_TAPS_3D];
-    int32_t tap_dt[VQB_MAX_TAPS_3D];
+    int32_t tap_view[kTaps];
+    int32_t tap_dw[kTaps];
+    int32_t tap_dh[kTaps];
+    int32_t tap_dt[kTaps];
     int32_t ntaps, kchunks, C, Cout;
     int32_t N, T, H, W;
     int32_t lbw, lbh, lbt, lbn;
@@ -78,6 +80,8 @@ struct alignas(64) Conv3dParams {
     const float* bias;
     float* stats;
 };
+using Conv3dParams = Conv3dParamsT<VQB_MAX_TAPS_3D>;
+using Conv3dDgradParams = Conv3dParamsT<VQB_MAX_TAPS_3D_DGRAD>;
 
 template <int BN, class P>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ P p) {
@@ -476,22 +480,25 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
 
 // ---------------------------------------------------------------------------------------------------------------------
 // 3-D (video) convolution: the same kernel over NTHWC activations with 5-D TMA boxes (tae.py call sites in vqb200.h).
-extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void* w_packed, const float* bias,
-                               const void* res, void* out, void* stream) {
-    VQB_CHECK(d && a && w_packed && out, "vqb_conv3d_gemm: null pointer");
-    VQB_CHECK(d->C > 0 && d->C % 8 == 0, "vqb_conv3d_gemm: C=%d must be a positive multiple of 8", d->C);
-    VQB_CHECK(d->Cout > 0 && d->N > 0 && d->T > 0 && d->H > 0 && d->W > 0, "vqb_conv3d_gemm: bad extents");
-    VQB_CHECK(d->ntaps >= 1 && d->ntaps <= VQB_MAX_TAPS_3D && d->nviews >= 1 && d->nviews <= VQB_MAX_VIEWS_3D,
-              "vqb_conv3d_gemm: ntaps=%d nviews=%d out of range", d->ntaps, d->nviews);
+// D / P: VqbConv3dDesc / Conv3dParams (27 taps) or VqbConv3dDgradDesc / Conv3dDgradParams (64 taps); `fn` names the
+// entry point in error messages.
+template <class D, class P, int kMaxTaps>
+static int conv3d_impl(const char* fn, const D* d, const void* a, const void* w_packed, const float* bias,
+                       const void* res, void* out, void* stream) {
+    VQB_CHECK(d && a && w_packed && out, "%s: null pointer", fn);
+    VQB_CHECK(d->C > 0 && d->C % 8 == 0, "%s: C=%d must be a positive multiple of 8", fn, d->C);
+    VQB_CHECK(d->Cout > 0 && d->N > 0 && d->T > 0 && d->H > 0 && d->W > 0, "%s: bad extents", fn);
+    VQB_CHECK(d->ntaps >= 1 && d->ntaps <= kMaxTaps && d->nviews >= 1 && d->nviews <= VQB_MAX_VIEWS_3D,
+              "%s: ntaps=%d nviews=%d out of range", fn, d->ntaps, d->nviews);
     VQB_CHECK((d->flags & ~(VQB_EPI_BIAS | VQB_EPI_RES)) == 0,
-              "vqb_conv3d_gemm: flags 0x%x: only VQB_EPI_BIAS and VQB_EPI_RES are supported", d->flags);
-    VQB_CHECK(d->out_f32 == 0 || d->out_f32 == 1, "vqb_conv3d_gemm: out_f32 must be 0 or 1");
+              "%s: flags 0x%x: only VQB_EPI_BIAS and VQB_EPI_RES are supported", fn, d->flags);
+    VQB_CHECK(d->out_f32 == 0 || d->out_f32 == 1, "%s: out_f32 must be 0 or 1", fn);
     if (d->flags & VQB_EPI_BIAS)
         VQB_CHECK(bias != nullptr && (reinterpret_cast<uintptr_t>(bias) & 15u) == 0,
-                  "vqb_conv3d_gemm: VQB_EPI_BIAS needs a 16-byte aligned bias pointer");
-    if (d->flags & VQB_EPI_RES) VQB_CHECK(res != nullptr, "vqb_conv3d_gemm: VQB_EPI_RES without res");
+                  "%s: VQB_EPI_BIAS needs a 16-byte aligned bias pointer", fn);
+    if (d->flags & VQB_EPI_RES) VQB_CHECK(res != nullptr, "%s: VQB_EPI_RES without res", fn);
     VQB_CHECK(d->on >= 0 && d->ot >= 0 && d->oh >= 0 && d->ow >= 0 && d->oc > 0,
-              "vqb_conv3d_gemm: output strides must be non-negative (oc > 0)");
+              "%s: output strides must be non-negative (oc > 0)", fn);
     // paired bf16 stores need 16-byte aligned voxel rows; otherwise (e.g. NCTHW bf16 of 1x1x1 videos: oc = 1) the
     // per-element store
     const bool vec3 = d->oc == 1 && !d->out_f32 && d->on % 8 == 0 && d->ot % 8 == 0 && d->oh % 8 == 0 &&
@@ -500,18 +507,18 @@ extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void
     if (!vec3)
         VQB_CHECK((reinterpret_cast<uintptr_t>(out) & (d->out_f32 ? 3u : 1u)) == 0 &&
                       (reinterpret_cast<uintptr_t>(res) & 1u) == 0,
-                  "vqb_conv3d_gemm: misaligned output / residual");
+                  "%s: misaligned output / residual", fn);
     for (int v = 0; v < d->nviews; ++v) {
         const VqbView3d& vw = d->views[v];
         VQB_CHECK(vw.offset >= 0 && vw.Wv > 0 && vw.Hv > 0 && vw.Tv > 0 && vw.Nv > 0 && vw.sw > 0 && vw.sw % 8 == 0 &&
                       vw.sh > 0 && vw.sh % 8 == 0 && vw.st > 0 && vw.st % 8 == 0 && vw.sn > 0 && vw.sn % 8 == 0,
-                  "vqb_conv3d_gemm: view %d has bad extents / strides (strides must be positive multiples of 8)", v);
+                  "%s: view %d has bad extents / strides (strides must be positive multiples of 8)", fn, v);
     }
     for (int t = 0; t < d->ntaps; ++t)
-        VQB_CHECK(d->taps[t].view >= 0 && d->taps[t].view < d->nviews, "vqb_conv3d_gemm: tap %d view out of range", t);
-    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_conv3d_gemm: current device is not sm_90");
+        VQB_CHECK(d->taps[t].view >= 0 && d->taps[t].view < d->nviews, "%s: tap %d view out of range", fn, t);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "%s: current device is not sm_90", fn);
 
-    Conv3dParams p;
+    P p;
     memset(&p, 0, sizeof(p));  // statistics / mask fields stay zero (rank-5 epilogue: bias + residual)
     const int block_n = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : (d->Cout > 16 ? 32 : 16));
     p.n_tiles = (d->Cout + block_n - 1) / block_n;
@@ -532,7 +539,7 @@ extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void
     p.tiles_h = (d->H + bh - 1) / bh;
     p.tiles_t = (d->T + bt - 1) / bt;
     const int64_t total = static_cast<int64_t>(p.tiles_w) * p.tiles_h * p.tiles_t * ((d->N + bn - 1) / bn) * p.n_tiles;
-    VQB_CHECK(total < (1ll << 31), "vqb_conv3d_gemm: too many tiles");
+    VQB_CHECK(total < (1ll << 31), "%s: too many tiles", fn);
     p.total_tiles = static_cast<int32_t>(total);
     const int stage_bytes = kABytes + block_n * kBlockK * 2;
     const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages;
@@ -593,4 +600,21 @@ extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void
     if (rc != VQB_OK) return rc;
     count_launch();
     return VQB_OK;
+}
+
+extern "C" int vqb_conv3d_gemm(const VqbConv3dDesc* d, const void* a, const void* w_packed, const float* bias,
+                               const void* res, void* out, void* stream) {
+    return conv3d_impl<VqbConv3dDesc, Conv3dParams, VQB_MAX_TAPS_3D>("vqb_conv3d_gemm", d, a, w_packed, bias, res, out,
+                                                                       stream);
+}
+
+// Data gradient of the folded up-sampling (tae.py:110-116): 64 taps over the 8 parity views of dy in one launch, no
+// epilogue (include/vqb200.h).
+extern "C" int vqb_conv3d_dgrad_gemm(const VqbConv3dDgradDesc* d, const void* dy, const void* w_packed, void* dx,
+                                     void* stream) {
+    VQB_CHECK(d == nullptr || d->flags == 0, "vqb_conv3d_dgrad_gemm: flags 0x%x: the data gradient has no epilogue",
+              d->flags);
+    return conv3d_impl<VqbConv3dDgradDesc, Conv3dDgradParams, VQB_MAX_TAPS_3D_DGRAD>("vqb_conv3d_dgrad_gemm", d, dy,
+                                                                                     w_packed, nullptr, nullptr, dx,
+                                                                                     stream);
 }

@@ -676,6 +676,23 @@ __global__ void gauss_reparam_kernel(const T* __restrict__ z, const T* __restric
     }
 }
 
+// Backward of gauss_reparam_kernel (fp32 training): dz[n][c] = g (mean half), dz[n][Z + c] = g * eps * 0.5 *
+// exp(0.5 * logvar) where logvar >= -3, else 0 (torch's clamp backward passes the gradient at exactly -3).
+__global__ void gauss_reparam_bwd_kernel(const float* __restrict__ g, const float* __restrict__ z,
+                                         const float* __restrict__ eps, float* __restrict__ dz, int Z, int64_t S,
+                                         int64_t total) {
+    for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
+         i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t s = i % S, nc = i / S;
+        const int64_t n = nc / Z, c = nc % Z;
+        const int64_t zm = (n * 2 * Z + c) * S + s, zl = zm + static_cast<int64_t>(Z) * S;
+        const float gv = g[i];
+        const float lv = z[zl];
+        dz[zm] = gv;
+        dz[zl] = lv >= -3.f ? gv * eps[i] * expf(0.5f * lv) * 0.5f : 0.f;
+    }
+}
+
 }  // namespace vqb
 
 using namespace vqb;
@@ -989,6 +1006,23 @@ int vqb_gauss_reparam(const void* z, const void* eps, void* out, int N, int Z, i
     else
         gauss_reparam_kernel<float><<<gs_blocks(total, 256), 256, 0, st>>>(
             static_cast<const float*>(z), static_cast<const float*>(eps), static_cast<float*>(out), Z, S, total);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+// tae.DiagonalGaussian backward (autograd of tae.py:263-264), see include/vqb200.h.
+int vqb_gauss_reparam_bwd(const float* g, const float* z, const float* eps, float* dz, int N, int Z, int64_t S,
+                          void* stream) {
+    VQB_CHECK(g && z && eps && dz, "vqb_gauss_reparam_bwd: null pointer");
+    VQB_CHECK(N > 0 && Z > 0 && S > 0, "vqb_gauss_reparam_bwd: bad arguments (N=%d Z=%d S=%lld)", N, Z, (long long)S);
+    VQB_CHECK(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(eps) |
+                reinterpret_cast<uintptr_t>(dz)) & 3u) == 0,
+              "vqb_gauss_reparam_bwd: pointers must be 4-byte aligned (fp32)");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_gauss_reparam_bwd: current device is not sm_90");
+    const int64_t total = static_cast<int64_t>(N) * Z * S;
+    gauss_reparam_bwd_kernel<<<gs_blocks(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(g, z, eps, dz, Z, S,
+                                                                                                    total);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;

@@ -15,6 +15,8 @@
 #include "common.cuh"
 #include "ptx.cuh"
 
+#include <cstring>
+
 namespace vqb {
 
 constexpr int kWM = 128;       // Cout rows per tile
@@ -24,6 +26,7 @@ constexpr int kWPix = 64;                     // pixels per K block
 constexpr uint32_t kAtomBytes = kWPix * 128;  // [64 px][64 ch] bf16
 
 struct alignas(64) WgradParams {
+    static constexpr int kRank = 4;  // NHWC, 4-D TMA boxes [64 ch][bw][bh][bn]
     CUtensorMap ymap;
     CUtensorMap xmap[VQB_MAX_VIEWS];
     int32_t tap_view[VQB_MAX_TAPS];
@@ -38,8 +41,26 @@ struct alignas(64) WgradParams {
     float* partial;
 };
 
-template <int BN>
-__global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
+// The rank-5 (video) form: NTHWC, 5-D TMA boxes [64 ch][bw][bh][bt][bn] of 64 voxels, up to 27 taps over up to 8 views.
+struct alignas(64) Wgrad3dParams {
+    static constexpr int kRank = 5;
+    CUtensorMap ymap;
+    CUtensorMap xmap[VQB_MAX_VIEWS_3D];
+    int32_t tap_view[VQB_MAX_TAPS_3D];
+    int32_t tap_dw[VQB_MAX_TAPS_3D];
+    int32_t tap_dh[VQB_MAX_TAPS_3D];
+    int32_t tap_dt[VQB_MAX_TAPS_3D];
+    int32_t ntaps, C, C64, Cout;
+    int32_t lbw, lbh, lbt, lbn;
+    int32_t tiles_w, tiles_h, tiles_t, pixel_boxes;
+    int32_t n_tiles, ksplit, total_units;
+    int32_t stages;
+    int64_t ld;
+    float* partial;
+};
+
+template <int BN, class P>
+__global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_constant__ P p) {
     extern __shared__ uint8_t smem_raw[];
     constexpr int kAtoms = BN / 64;
     constexpr uint32_t kABytes = 2 * kAtomBytes;
@@ -87,21 +108,41 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
                 for (int kb = kb0; kb < kb1; ++kb) {
                     const int tw = kb % p.tiles_w;
                     const int th = (kb / p.tiles_w) % p.tiles_h;
-                    const int tn = kb / (p.tiles_w * p.tiles_h);
+                    int tt = 0, tn;
+                    if constexpr (P::kRank == 5) {
+                        tt = (kb / (p.tiles_w * p.tiles_h)) % p.tiles_t;
+                        tn = kb / (p.tiles_w * p.tiles_h * p.tiles_t);
+                    } else {
+                        tn = kb / (p.tiles_w * p.tiles_h);
+                    }
                     const int w0 = tw << p.lbw, h0 = th << p.lbh, n0 = tn << p.lbn;
                     mbar_wait(&empty[stage], phase ^ 1);
                     mbar_arrive_expect_tx(&full[stage], kStageBytes);
                     uint8_t* a = base + stage * kStageBytes;
                     uint8_t* b = a + kABytes;
-                    tma_load_4d(&p.ymap, &full[stage], a, co0, w0, h0, n0);
-                    tma_load_4d(&p.ymap, &full[stage], a + kAtomBytes, co0 + 64, w0, h0, n0);
+                    if constexpr (P::kRank == 5) {
+                        const int t0 = tt << p.lbt;
+                        tma_load_5d(&p.ymap, &full[stage], a, co0, w0, h0, t0, n0);
+                        tma_load_5d(&p.ymap, &full[stage], a + kAtomBytes, co0 + 64, w0, h0, t0, n0);
 #pragma unroll
-                    for (int j = 0; j < kAtoms; ++j) {
-                        const int col = colbase + 64 * j;
-                        const int t = col / p.C64;
-                        const int c0 = col - t * p.C64;
-                        tma_load_4d(&p.xmap[p.tap_view[t]], &full[stage], b + j * kAtomBytes, c0, w0 + p.tap_dw[t],
-                                    h0 + p.tap_dh[t], n0);
+                        for (int j = 0; j < kAtoms; ++j) {
+                            const int col = colbase + 64 * j;
+                            const int t = col / p.C64;
+                            const int c0 = col - t * p.C64;
+                            tma_load_5d(&p.xmap[p.tap_view[t]], &full[stage], b + j * kAtomBytes, c0, w0 + p.tap_dw[t],
+                                        h0 + p.tap_dh[t], t0 + p.tap_dt[t], n0);
+                        }
+                    } else {
+                        tma_load_4d(&p.ymap, &full[stage], a, co0, w0, h0, n0);
+                        tma_load_4d(&p.ymap, &full[stage], a + kAtomBytes, co0 + 64, w0, h0, n0);
+#pragma unroll
+                        for (int j = 0; j < kAtoms; ++j) {
+                            const int col = colbase + 64 * j;
+                            const int t = col / p.C64;
+                            const int c0 = col - t * p.C64;
+                            tma_load_4d(&p.xmap[p.tap_view[t]], &full[stage], b + j * kAtomBytes, c0, w0 + p.tap_dw[t],
+                                        h0 + p.tap_dh[t], n0);
+                        }
                     }
                     if (++stage == stages) {
                         stage = 0;
@@ -166,16 +207,16 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
     }
 }
 
-template <int BN>
-static int launch_wgrad(const WgradParams& p, void* stream) {
+template <int BN, class P>
+static int launch_wgrad(const P& p, void* stream) {
     const size_t smem = 1024 + static_cast<size_t>(p.stages) * (2 + BN / 64) * kAtomBytes + 16 * p.stages;
     static bool attr_set = false;
     if (!attr_set) {
-        VQB_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VQB_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set = true;
     }
     const int grid = p.total_units < num_sms() ? p.total_units : num_sms();
-    wgrad_gemm_kernel<BN><<<grid, kWThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
+    wgrad_gemm_kernel<BN, P><<<grid, kWThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
     VQB_CUDA(cudaGetLastError());
     return VQB_OK;
 }
@@ -248,6 +289,102 @@ extern "C" int vqb_wgrad_gemm(const VqbWgradDesc* d, const void* dy, const void*
     if (rc != VQB_OK) return rc;
     for (int v = 0; v < d->nviews; ++v) {
         rc = encode_view(d->views[v], x, d->C, p.lbw, p.lbh, p.lbn, &p.xmap[v]);
+        if (rc != VQB_OK) return rc;
+    }
+    rc = block_n == 128 ? launch_wgrad<128>(p, stream) : launch_wgrad<64>(p, stream);
+    if (rc != VQB_OK) return rc;
+    count_launch();
+    return VQB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Rank-5 weight gradient of the video autoencoder's 3x3x3 convs (tae.py call sites in include/vqb200.h).
+static int encode_view3d(const VqbView3d& vw, const void* basep, int C, uint32_t bw, uint32_t bh, uint32_t bt,
+                         uint32_t bn, CUtensorMap* m) {
+    const void* base = static_cast<const uint8_t*>(basep) + vw.offset * 2;
+    uint64_t dims[5] = {static_cast<uint64_t>(C), static_cast<uint64_t>(vw.Wv), static_cast<uint64_t>(vw.Hv),
+                        static_cast<uint64_t>(vw.Tv), static_cast<uint64_t>(vw.Nv)};
+    uint64_t str[4] = {static_cast<uint64_t>(vw.sw) * 2, static_cast<uint64_t>(vw.sh) * 2,
+                       static_cast<uint64_t>(vw.st) * 2, static_cast<uint64_t>(vw.sn) * 2};
+    uint32_t box[5] = {64, bw, bh, bt, bn};
+    return vqb::encode_tmap_bf16(m, base, 5, dims, str, box, 128);
+}
+
+static bool view3d_ok(const VqbView3d& vw) {
+    return vw.offset >= 0 && vw.Wv > 0 && vw.Hv > 0 && vw.Tv > 0 && vw.Nv > 0 && vw.sw > 0 && vw.sw % 8 == 0 &&
+           vw.sh > 0 && vw.sh % 8 == 0 && vw.st > 0 && vw.st % 8 == 0 && vw.sn > 0 && vw.sn % 8 == 0;
+}
+
+extern "C" int vqb_wgrad3d_gemm(const VqbWgrad3dDesc* d, const void* dy, const void* x, float* partial, void* stream) {
+    VQB_CHECK(d && dy && x && partial, "vqb_wgrad3d_gemm: null pointer");
+    VQB_CHECK(d->C > 0 && d->C % 8 == 0 && d->Cout > 0 && d->Cout % 8 == 0,
+              "vqb_wgrad3d_gemm: C=%d Cout=%d must be positive multiples of 8", d->C, d->Cout);
+    VQB_CHECK(d->N > 0 && d->T > 0 && d->H > 0 && d->W > 0, "vqb_wgrad3d_gemm: bad extents");
+    VQB_CHECK(d->ntaps >= 1 && d->ntaps <= VQB_MAX_TAPS_3D && d->nviews >= 1 && d->nviews <= VQB_MAX_VIEWS_3D,
+              "vqb_wgrad3d_gemm: ntaps=%d nviews=%d out of range", d->ntaps, d->nviews);
+    VQB_CHECK(d->ksplit >= 1, "vqb_wgrad3d_gemm: ksplit must be >= 1");
+    VQB_CHECK((reinterpret_cast<uintptr_t>(partial) & 15u) == 0, "vqb_wgrad3d_gemm: partial not 16-byte aligned");
+    VQB_CHECK(d->col_offset >= 0 && d->ld_override >= 0 && d->col_offset % 2 == 0 && d->ld_override % 2 == 0,
+              "vqb_wgrad3d_gemm: col_offset / ld_override must be non-negative and even (8-byte partial stores)");
+    VQB_CHECK(view3d_ok(d->dy_view), "vqb_wgrad3d_gemm: dy view has bad extents / strides");
+    for (int v = 0; v < d->nviews; ++v)
+        VQB_CHECK(view3d_ok(d->views[v]), "vqb_wgrad3d_gemm: view %d has bad extents / strides", v);
+    for (int t = 0; t < d->ntaps; ++t)
+        VQB_CHECK(d->taps[t].view >= 0 && d->taps[t].view < d->nviews, "vqb_wgrad3d_gemm: tap %d view out of range",
+                  t);
+    const int cols = vqb_wgrad_cols(d->ntaps, d->C);
+    if (d->ld_override > 0)
+        VQB_CHECK(d->col_offset + cols <= d->ld_override, "vqb_wgrad3d_gemm: columns exceed ld_override");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_wgrad3d_gemm: current device is not sm_90");
+
+    Wgrad3dParams p;
+    memset(&p, 0, sizeof(p));
+    // 64-voxel K box: as wide as the video (<= 64), then as tall, then as deep, then across videos
+    const uint32_t kp = kWPix;
+    uint32_t bw = next_pow2(d->W);
+    if (bw > kp) bw = kp;
+    uint32_t bh = next_pow2(d->H);
+    if (bh > kp / bw) bh = kp / bw;
+    uint32_t bt = next_pow2(d->T);
+    if (bt > kp / (bw * bh)) bt = kp / (bw * bh);
+    const uint32_t bn = kp / (bw * bh * bt);
+    p.lbw = ilog2(bw);
+    p.lbh = ilog2(bh);
+    p.lbt = ilog2(bt);
+    p.lbn = ilog2(bn);
+    p.tiles_w = (d->W + bw - 1) / bw;
+    p.tiles_h = (d->H + bh - 1) / bh;
+    p.tiles_t = (d->T + bt - 1) / bt;
+    const int64_t boxes = static_cast<int64_t>(p.tiles_w) * p.tiles_h * p.tiles_t * ((d->N + bn - 1) / bn);
+    VQB_CHECK(boxes < (1ll << 31), "vqb_wgrad3d_gemm: too many voxel boxes");
+    p.pixel_boxes = static_cast<int32_t>(boxes);
+    p.ntaps = d->ntaps;
+    p.C = d->C;
+    p.C64 = ((d->C + 63) / 64) * 64;
+    p.Cout = d->Cout;
+    const int block_n = (cols % 128 == 0) ? 128 : 64;
+    const int m_tiles = (d->Cout + kWM - 1) / kWM;
+    p.n_tiles = cols / block_n;
+    p.ksplit = d->ksplit;
+    const int64_t units = static_cast<int64_t>(m_tiles) * p.n_tiles * p.ksplit;
+    VQB_CHECK(units < (1ll << 31), "vqb_wgrad3d_gemm: too many work units");
+    p.total_units = static_cast<int32_t>(units);
+    p.ld = d->ld_override > 0 ? d->ld_override : cols;
+    p.partial = partial + d->col_offset;
+    const int stage_bytes = (2 + block_n / 64) * static_cast<int>(kAtomBytes);
+    int stages = (200 * 1024) / stage_bytes;
+    if (stages > kWMaxStages) stages = kWMaxStages;
+    p.stages = stages;
+    for (int t = 0; t < d->ntaps; ++t) {
+        p.tap_view[t] = d->taps[t].view;
+        p.tap_dw[t] = d->taps[t].dw;
+        p.tap_dh[t] = d->taps[t].dh;
+        p.tap_dt[t] = d->taps[t].dt;
+    }
+    int rc = encode_view3d(d->dy_view, dy, d->Cout, bw, bh, bt, bn, &p.ymap);
+    if (rc != VQB_OK) return rc;
+    for (int v = 0; v < d->nviews; ++v) {
+        rc = encode_view3d(d->views[v], x, d->C, bw, bh, bt, bn, &p.xmap[v]);
         if (rc != VQB_OK) return rc;
     }
     rc = block_n == 128 ? launch_wgrad<128>(p, stream) : launch_wgrad<64>(p, stream);

@@ -18,6 +18,7 @@ VQB_MAX_VIEWS = 16
 VQB_MAX_TAPS = 16
 VQB_MAX_VIEWS_3D = 8
 VQB_MAX_TAPS_3D = 27
+VQB_MAX_TAPS_3D_DGRAD = 64
 EPI_BIAS, EPI_RES, EPI_RELU, EPI_MASK, EPI_STATS = 1, 2, 4, 8, 16
 
 
@@ -65,6 +66,21 @@ class VqbConv3dDesc(C.Structure):
                 ("W", C.c_int32), ("nviews", C.c_int32), ("ntaps", C.c_int32), ("flags", C.c_int32),
                 ("out_f32", C.c_int32), ("on", C.c_int64), ("ot", C.c_int64), ("oh", C.c_int64), ("ow", C.c_int64),
                 ("oc", C.c_int64), ("views", VqbView3d * VQB_MAX_VIEWS_3D), ("taps", VqbTap3d * VQB_MAX_TAPS_3D)]
+
+
+class VqbConv3dDgradDesc(C.Structure):
+    _fields_ = [("C", C.c_int32), ("Cout", C.c_int32), ("N", C.c_int32), ("T", C.c_int32), ("H", C.c_int32),
+                ("W", C.c_int32), ("nviews", C.c_int32), ("ntaps", C.c_int32), ("flags", C.c_int32),
+                ("out_f32", C.c_int32), ("on", C.c_int64), ("ot", C.c_int64), ("oh", C.c_int64), ("ow", C.c_int64),
+                ("oc", C.c_int64), ("views", VqbView3d * VQB_MAX_VIEWS_3D),
+                ("taps", VqbTap3d * VQB_MAX_TAPS_3D_DGRAD)]
+
+
+class VqbWgrad3dDesc(C.Structure):
+    _fields_ = [("C", C.c_int32), ("Cout", C.c_int32), ("N", C.c_int32), ("T", C.c_int32), ("H", C.c_int32),
+                ("W", C.c_int32), ("nviews", C.c_int32), ("ntaps", C.c_int32), ("ksplit", C.c_int32),
+                ("_pad", C.c_int32), ("ld_override", C.c_int64), ("col_offset", C.c_int64), ("dy_view", VqbView3d),
+                ("views", VqbView3d * VQB_MAX_VIEWS_3D), ("taps", VqbTap3d * VQB_MAX_TAPS_3D)]
 
 
 class VqbAdamwGroup(C.Structure):
@@ -135,6 +151,10 @@ def load():
         "vqb_conv3d_gemm": (i32, [C.POINTER(VqbConv3dDesc), vp, vp, vp, vp, vp, vp]),
         "vqb_attn_fwd_hd": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "vqb_gauss_reparam": (i32, [vp, vp, vp, i32, i32, i64, i32, vp]),
+        "vqb_conv3d_dgrad_gemm": (i32, [C.POINTER(VqbConv3dDgradDesc), vp, vp, vp, vp]),
+        "vqb_wgrad3d_gemm": (i32, [C.POINTER(VqbWgrad3dDesc), vp, vp, vp, vp]),
+        "vqb_attn_bwd_hd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+        "vqb_gauss_reparam_bwd": (i32, [vp, vp, vp, vp, i32, i32, i64, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)

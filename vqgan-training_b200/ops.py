@@ -305,7 +305,7 @@ def _wgrad_block_n(cols: int) -> int:
 def choose_ksplit(g: plans.ConvGeom, Cout_pad: int) -> int:
     """Split-K factor of the weight-gradient GEMM: the split count whose (tile, split) unit count best fills whole waves
     of the persistent CTAs (one per SM of an H100 SXM), preferring one wave. Mirrors the tile shape rules of
-    csrc/wgrad_gemm.cu (128 Cout rows x 128 or 64 columns, 64-pixel K blocks)."""
+    csrc/wgrad_gemm.cu (128 Cout rows x 128 or 64 columns, 64-pixel K blocks; for a 3-D geometry, 64-voxel boxes)."""
     cols = len(g.taps) * ((g.C + 63) // 64) * 64
     rows = 128
     kpix = 64
@@ -319,8 +319,13 @@ def choose_ksplit(g: plans.ConvGeom, Cout_pad: int) -> int:
 
     bw = p2(g.Wo, kpix)
     bh = p2(g.Ho, kpix // bw)
-    bn = kpix // (bw * bh)
-    boxes = -(-g.Wo // bw) * -(-g.Ho // bh) * -(-g.N // bn)
+    if isinstance(g, plans.ConvGeom3d):  # vqb_wgrad3d_gemm: 64-voxel boxes [bw][bh][bt][bn]
+        bt = p2(g.To, kpix // (bw * bh))
+        bn = kpix // (bw * bh * bt)
+        boxes = -(-g.Wo // bw) * -(-g.Ho // bh) * -(-g.To // bt) * -(-g.N // bn)
+    else:
+        bn = kpix // (bw * bh)
+        boxes = -(-g.Wo // bw) * -(-g.Ho // bh) * -(-g.N // bn)
     # every unit pays a fixed pipeline-fill + fp32-partial-tile epilogue, and the reduction kernel reads ksplit partials:
     # each extra wave and each extra split is penalised
     sms = _num_sms()
@@ -945,8 +950,9 @@ def vq_argmin(z_flat: torch.Tensor, codebook: torch.Tensor):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# Video autoencoder (tae.py): no-grad inference ops over NTHWC bf16 activations [N, T, H, W, Cp]. There is no backward
-# here; tae.py refuses a forward that autograd would have to differentiate before anything is launched.
+# Video autoencoder (tae.py): ops over NTHWC bf16 activations [N, T, H, W, Cp]. The plain functions are the no-grad
+# inference path; the autograd functions after them (Conv3dFn, UpConv3dFn, AttentionHdFn, GaussReparamFn) are the
+# training path that tae.py takes once a module is opted in with tae.enable_training.
 def _bias_f32(bias):
     if bias is None:
         return None
@@ -1039,6 +1045,11 @@ def group_norm_silu3d(x, gamma, beta, groups=32, eps=1e-6, silu=True):
 def attention_hd(qkv, heads, head_dim):
     """qkv [N, T, H, W, 3C] bf16 (q | k | v channel blocks) -> softmax(q k^T / sqrt(head_dim)) v as [N, T, H, W, C]
     (tae.py:26-51). head_dim 32 or 64."""
+    return _attention_hd_fwd(qkv, heads, head_dim)[0]
+
+
+def _attention_hd_fwd(qkv, heads, head_dim):
+    """-> (out, lse) of attention_hd; lse [N, heads, T*H*W] is what the backward needs."""
     if head_dim not in (32, 64):
         raise NotImplementedError(f"vqgan-training_b200: attention heads of {head_dim} channels are not supported "
                                   "(heads of 32 or 64 channels only)")
@@ -1049,7 +1060,7 @@ def attention_hd(qkv, heads, head_dim):
     out = torch.empty(N, T, H, W, C, device=qkv.device, dtype=torch.bfloat16)
     lse = torch.empty(N, heads, T * H * W, device=qkv.device, dtype=torch.float32)
     check(_L().vqb_attn_fwd_hd(ptr(qkv), ptr(out), ptr(lse), N, T * H * W, C, head_dim, stream_ptr()), "attn_fwd_hd")
-    return out
+    return out, lse
 
 
 def gauss_reparam(z, eps):
@@ -1067,3 +1078,225 @@ def gauss_reparam(z, eps):
     check(_L().vqb_gauss_reparam(ptr(z), ptr(eps), ptr(out), N, Z, S, 1 if z.dtype == torch.bfloat16 else 0,
                                  stream_ptr()), "gauss_reparam")
     return out
+
+
+# ---- training path of the video autoencoder -------------------------------------------------------------------------
+def _ncthw_grad_to_nthwc(gout, Cout, Cop):
+    """fp32 NCTHW gradient of a module-boundary output -> bf16 NTHWC dy (vqb_nchw_to_nhwc on the [N][C][T*H][W] view)."""
+    N, _, T, H, W = gout.shape
+    gn = gout.float().contiguous()
+    dy = torch.empty(N, T, H, W, Cop, device=gout.device, dtype=torch.bfloat16)
+    check(_L().vqb_nchw_to_nhwc(ptr(gn), ptr(dy), N, Cout, T * H, W, Cop, 0, 0, stream_ptr()), "nchw_to_nhwc")
+    return dy
+
+
+def run_wgrad3d(g: plans.ConvGeom3d, x: torch.Tensor, dy: torch.Tensor, weight: torch.Tensor, Cout_pad: int,
+                out: torch.Tensor) -> torch.Tensor:
+    """OIDHW fp32 gradient (into `out`) of a 3x3x3 conv whose forward geometry is g: vqb_wgrad3d_gemm + the
+    deterministic split reduction."""
+    Cout, Cin = weight.shape[:2]
+    descs = g.__dict__.setdefault("_descs", {})
+    ent = descs.get(("wgrad3", Cout_pad))
+    if ent is None:
+        ksplit = choose_ksplit(g, Cout_pad)
+        ent = (ksplit, plans.wgrad3d_desc(g, Cout_pad, ksplit), _L().vqb_wgrad_cols(len(g.taps), g.C))
+        descs[("wgrad3", Cout_pad)] = ent
+    ksplit, d, cols = ent
+    partial = torch.empty(ksplit, Cout_pad, cols, device=x.device, dtype=torch.float32)
+    check(_L().vqb_wgrad3d_gemm(d, ptr(dy), ptr(x), ptr(partial), stream_ptr()), "wgrad3d_gemm")
+    assert out.shape == weight.shape and out.is_contiguous()
+    tm = tapmap_tensor(g.tapmap, x.device)
+    check(_L().vqb_wgrad_reduce(ptr(partial), ptr(out), ksplit, Cout, Cout_pad, Cin, 27, len(g.taps),
+                                cols // len(g.taps), ptr(tm), 0, stream_ptr()), "wgrad_reduce")
+    return out
+
+
+def _bias_grad(dy, rows, Cout, Cop):
+    """Bias gradient: the per-channel sums the GroupNorm backward already produced for this dy, else vqb_colsum."""
+    N, T, H, W, _ = dy.shape
+    gb = _take_dx_colsum(dy.view(N, T * H, W, Cop), Cop)
+    if gb is None:
+        gb = colsum(rows, dy, Cop)
+    return gb[:Cout]
+
+
+class Conv3dFn(torch.autograd.Function):
+    """Autograd form of conv3d (kinds "s1", "s2", "p1"). Backward: the data gradient through the rotated 27-tap plan
+    (s1), one strided conv per parity class of dx (s2, the pad plane's gradient is dropped) or the 2-D 1x1 dgrad on the
+    [N][T*H][W] view (p1); the weight gradient through vqb_wgrad3d_gemm (p1: vqb_wgrad_gemm) into grad_out(weight); the
+    bias gradient from the GroupNorm backward's column sums; the residual gradient is dy."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, cache, kind, ncthw_out):
+        x = x.contiguous()
+        out = conv3d(x, weight, bias, cache, kind, residual, ncthw_out)
+        ctx.save_for_backward(x, weight)
+        ctx.cache, ctx.kind, ctx.ncthw_out = cache, kind, ncthw_out
+        ctx.has_bias, ctx.has_res = bias is not None, residual is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, weight = ctx.saved_tensors
+        inference_only(weight)
+        cache, kind = ctx.cache, ctx.kind
+        N, T, H, W, Cp = x.shape
+        Cout, Cin = weight.shape[:2]
+        Cop = plans.cpad(Cout)
+        if kind == "p1":
+            g = cache.geom(("p1", N, T, H, W), lambda: plans.geom_s1(N, T * H, W, Cp, 1))
+            To, Ho, Wo = T, H, W
+        else:
+            g = cache.geom((kind, N, T, H, W), lambda: (plans.geom3_s1 if kind == "s1" else plans.geom3_s2)(
+                N, T, H, W, Cp))
+            To, Ho, Wo = g.To, g.Ho, g.Wo
+        dy = _ncthw_grad_to_nthwc(gout, Cout, Cop) if ctx.ncthw_out else gout.contiguous()
+        gx = gw = gb = gres = None
+        if ctx.needs_input_grad[0]:
+            gx = (torch.empty if Cp == Cin else torch.zeros)(N, T, H, W, Cp, device=x.device, dtype=torch.bfloat16)
+            if kind == "p1":
+                gd = cache.geom(("p1d", N, T, H, W), lambda: plans.geom_s1_dgrad(N, T * H, W, Cop, 1))
+                wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
+                run_conv_gemm(gd, dy, wpd, Cin, gx, plans.nhwc_strides(T * H, W, Cp))
+            elif kind == "s1":
+                gd = cache.geom(("s1d", N, T, H, W), lambda: plans.geom3_s1_dgrad(N, T, H, W, Cop))
+                wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
+                run_conv3d(gd, dy, wpd, Cin, gx, plans.nthwc_strides(T, H, W, Cp))
+            else:
+                for pt, ph, pw, gd in cache.geom(("s2d", N, T, H, W),
+                                                 lambda: plans.geom3_s2_dgrad_classes(N, T, H, W, Cop)):
+                    wpd = cache.get(weight, ("dgrad", kind, pt, ph, pw), gd.tapmap, True, Cop)
+                    strides, off = plans.s2_dgrad_out(T, H, W, Cp, pt, ph, pw)
+                    run_conv3d(gd, dy, wpd, Cin, gx, strides, out_off_elems=off)
+        if ctx.needs_input_grad[1]:
+            gw = grad_out(weight)
+            if kind == "p1":
+                run_wgrad(g, x, dy, (Cout, Cin, 1, 1), Cop, out=gw.view(Cout, Cin, 1, 1))
+            else:
+                run_wgrad3d(g, x, dy, weight, Cop, gw)
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            gb = _bias_grad(dy, N * To * Ho * Wo, Cout, Cop)
+        if ctx.has_res and ctx.needs_input_grad[3]:
+            gres = gout if ctx.ncthw_out else dy
+        return gx, gw, gb, gres, None, None, None
+
+
+def conv3d_train(x, weight, bias, cache, kind="s1", residual=None, ncthw_out=False):
+    return Conv3dFn.apply(x, weight, bias, residual, cache, kind, ncthw_out)
+
+
+class UpConv3dFn(torch.autograd.Function):
+    """Autograd form of upsample_conv3d. Backward: the data gradient is one 64-tap conv over the eight parity views of dy
+    (plans.geom3_up_dgrad, vqb_conv3d_dgrad_gemm: one fp32 accumulation, one rounding); the weight gradient is eight phase
+    GEMMs (vqb_wgrad3d_gemm) filling one partial buffer, unfolded by vqb_wgrad_reduce_fold."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, cache):
+        x = x.contiguous()
+        out = upsample_conv3d(x, weight, bias, cache)
+        ctx.save_for_backward(x, weight)
+        ctx.cache, ctx.has_bias = cache, bias is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, weight = ctx.saved_tensors
+        inference_only(weight)
+        cache = ctx.cache
+        N, t, h, w, Cp = x.shape
+        Cout, Cin = weight.shape[:2]
+        Cop = plans.cpad(Cout)
+        dy = gout.contiguous()
+        gx = gw = gb = None
+        if ctx.needs_input_grad[0]:
+            gd = cache.geom(("upd", N, t, h, w), lambda: plans.geom3_up_dgrad(N, t, h, w, Cop))
+            wpd = cache.get(weight, ("updgrad",), gd.tapmask, True, Cop, fold=True)
+            gx = (torch.empty if Cp == Cin else torch.zeros)(N, t, h, w, Cp, device=x.device, dtype=torch.bfloat16)
+            descs = gd.__dict__.setdefault("_descs", {})
+            d = descs.get(Cin)
+            if d is None:
+                d = descs[Cin] = plans.conv3d_dgrad_desc(gd, Cin, plans.nthwc_strides(t, h, w, Cp))
+            check(_L().vqb_conv3d_dgrad_gemm(d, ptr(dy), ptr(wpd), ptr(gx), stream_ptr()), "conv3d_dgrad_gemm")
+        if ctx.needs_input_grad[1]:
+            C64 = ((Cp + 63) // 64) * 64
+            g0 = cache.geom(("up", N, t, h, w, 0, 0, 0), lambda: plans.geom3_up_fwd(N, t, h, w, Cp, 0, 0, 0))
+            ksplit = choose_ksplit(g0, Cop)
+            partial = torch.empty(ksplit, Cop, 64 * C64, device=x.device, dtype=torch.float32)
+            masks = []
+            for pt in range(2):
+                for ph in range(2):
+                    for pw in range(2):
+                        g = cache.geom(("up", N, t, h, w, pt, ph, pw),
+                                       lambda: plans.geom3_up_fwd(N, t, h, w, Cp, pt, ph, pw))
+                        descs = g.__dict__.setdefault("_descs", {})
+                        d = descs.get(("upwgrad", Cop, ksplit))
+                        if d is None:
+                            d = descs[("upwgrad", Cop, ksplit)] = plans.wgrad3d_desc(
+                                g, Cop, ksplit, dy_view=plans.up3_dy_view(N, t, h, w, Cop, pt, ph, pw),
+                                ld_override=64 * C64, col_offset=(pt * 4 + ph * 2 + pw) * 8 * C64)
+                        check(_L().vqb_wgrad3d_gemm(d, ptr(dy), ptr(x), ptr(partial), stream_ptr()), "wgrad3d_gemm(up)")
+                        masks += g.tapmask
+            gw = grad_out(weight)
+            check(_L().vqb_wgrad_reduce_fold(ptr(partial), ptr(gw), ksplit, Cout, Cop, Cin, 27, 64, C64,
+                                             ptr(tapmap_tensor(masks, x.device)), stream_ptr()), "wgrad_reduce_fold")
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            gb = _bias_grad(dy, N * 8 * t * h * w, Cout, Cop)
+        return gx, gw, gb, None
+
+
+def upsample_conv3d_train(x, weight, bias, cache):
+    return UpConv3dFn.apply(x, weight, bias, cache)
+
+
+class AttentionHdFn(torch.autograd.Function):
+    """Autograd form of attention_hd; the backward is vqb_attn_bwd_hd (heads of 32 or 64)."""
+
+    @staticmethod
+    def forward(ctx, qkv, heads, head_dim):
+        qkv = qkv.contiguous()
+        out, lse = _attention_hd_fwd(qkv, heads, head_dim)
+        ctx.save_for_backward(qkv, out, lse)
+        ctx.head_dim = head_dim
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        qkv, out, lse = ctx.saved_tensors
+        N, T, H, W, C3 = qkv.shape
+        dout = gout.contiguous()
+        dvec = torch.empty_like(lse)
+        dqkv = torch.empty_like(qkv)
+        check(_L().vqb_attn_bwd_hd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dvec), ptr(dqkv), N, T * H * W, C3 // 3,
+                                   ctx.head_dim, stream_ptr()), "attn_bwd_hd")
+        return dqkv, None, None
+
+
+def attention_hd_train(qkv, heads, head_dim):
+    return AttentionHdFn.apply(qkv, heads, head_dim)
+
+
+class GaussReparamFn(torch.autograd.Function):
+    """Autograd form of gauss_reparam for fp32 latents; the backward is vqb_gauss_reparam_bwd (eps carries no
+    gradient: it is drawn noise)."""
+
+    @staticmethod
+    def forward(ctx, z, eps):
+        z = z.contiguous()
+        eps = eps.to(z.dtype).contiguous()
+        ctx.save_for_backward(z, eps)
+        return gauss_reparam(z, eps)
+
+    @staticmethod
+    def backward(ctx, g):
+        z, eps = ctx.saved_tensors
+        inference_only(z)
+        N, Z2 = z.shape[:2]
+        g = g.float().contiguous()
+        dz = torch.empty_like(z)
+        check(_L().vqb_gauss_reparam_bwd(ptr(g), ptr(z), ptr(eps), ptr(dz), N, Z2 // 2,
+                                         z[0, 0].numel(), stream_ptr()), "gauss_reparam_bwd")
+        return dz, None
+
+
+def gauss_reparam_train(z, eps):
+    return GaussReparamFn.apply(z, eps)

@@ -15,8 +15,8 @@ from __future__ import annotations
 from dataclasses import dataclass, field
 from typing import List, Tuple
 
-from native import (VqbConv3dDesc, VqbConvDesc, VqbTap, VqbTap3d, VqbView, VqbView3d, VqbWgradDesc, dense_view,
-                    dense_view3d)
+from native import (VqbConv3dDesc, VqbConv3dDgradDesc, VqbConvDesc, VqbTap, VqbTap3d, VqbView, VqbView3d,
+                    VqbWgrad3dDesc, VqbWgradDesc, dense_view, dense_view3d)
 
 
 def cpad(c: int) -> int:
@@ -308,3 +308,96 @@ def ncthw_strides(C, T, H, W):
 
 def nthwc_strides(T, H, W, Cs):
     return (T * H * W * Cs, H * W * Cs, W * Cs, Cs, 1)
+
+
+# ---- 3-D data / weight gradients (training, tae.enable_training) ---------------------------------------------------
+def geom3_s1_dgrad(N, T, H, W, Cout_pad) -> ConvGeom3d:
+    """dgrad of the 3x3x3 stride-1 conv = the same conv over dy with the 27 taps rotated (weights packed transposed)."""
+    g = ConvGeom3d(N, T, H, W, Cout_pad, [dense_view3d(N, T, H, W, Cout_pad)])
+    for kt in range(3):
+        for kh in range(3):
+            for kw in range(3):
+                g.taps.append((0, kw - 1, kh - 1, kt - 1))
+                g.tapmap.append(26 - (kt * 9 + kh * 3 + kw))
+    return g
+
+
+def geom3_s2_dgrad_classes(N, T, H, W, Cout_pad):
+    """dgrad of the Downsample conv, one small conv per parity class (pt, ph, pw) of dx (T x H x W):
+    dx[2a+pt, 2b+ph, 2c+pw] = sum over taps with kt%2==pt, kh%2==ph, kw%2==pw of
+    dy[a - (kt-pt)/2, b - (kh-ph)/2, c - (kw-pw)/2] . W[kt,kh,kw]  (1 to 8 taps). The pad plane's gradient is never
+    formed. Returns [(pt, ph, pw, ConvGeom3d over the dy grid (N, T/2, H/2, W/2))]; class (pt, ph, pw) writes the strided
+    sub-grid s2_dgrad_out of dx."""
+    out = []
+    To, Ho, Wo = T // 2, H // 2, W // 2
+    for pt in range(2):
+        for ph in range(2):
+            for pw in range(2):
+                g = ConvGeom3d(N, To, Ho, Wo, Cout_pad, [dense_view3d(N, To, Ho, Wo, Cout_pad)])
+                for kt in range(pt, 3, 2):
+                    for kh in range(ph, 3, 2):
+                        for kw in range(pw, 3, 2):
+                            g.taps.append((0, -((kw - pw) // 2), -((kh - ph) // 2), -((kt - pt) // 2)))
+                            g.tapmap.append(kt * 9 + kh * 3 + kw)
+                out.append((pt, ph, pw, g))
+    return out
+
+
+def s2_dgrad_out(T, H, W, Cp, pt, ph, pw):
+    """-> ((on, ot, oh, ow, oc), element offset) of parity class (pt, ph, pw) inside dx [N, T, H, W, Cp]."""
+    return (T * H * W * Cp, 2 * H * W * Cp, 2 * W * Cp, 2 * Cp, 1), ((pt * H + ph) * W + pw) * Cp
+
+
+def up3_dy_view(N, t, h, w, Cop, pt, ph, pw) -> VqbView3d:
+    """Parity view (pt, ph, pw) of dy / out [N, 2t, 2h, 2w, Cop]."""
+    return VqbView3d(offset=((pt * 2 * h + ph) * 2 * w + pw) * Cop, Wv=w, Hv=h, Tv=t, Nv=N, sw=2 * Cop,
+                     sh=2 * 2 * w * Cop, st=2 * 4 * h * w * Cop, sn=8 * t * h * w * Cop)
+
+
+def geom3_up_dgrad(N, t, h, w, Cop) -> ConvGeom3d:
+    """dgrad of the folded up-sampling: dx[a,b,c] = sum over the 8 phases and their 2x2x2 taps of
+    dy_phase[a - dt, b - dh, c - dw] . Wf^T, one 64-tap conv over the eight parity views of dy (the 3-D form of
+    geom_up_dgrad). Needs the 64-entry tap table of VqbConv3dDgradDesc."""
+    g = ConvGeom3d(N, t, h, w, Cop)
+    for pt in range(2):
+        for ph in range(2):
+            for pw in range(2):
+                g.views.append(up3_dy_view(N, t, h, w, Cop, pt, ph, pw))
+    for pt in range(2):
+        for ph in range(2):
+            for pw in range(2):
+                for i in range(2):
+                    for j in range(2):
+                        for k in range(2):
+                            g.taps.append((pt * 4 + ph * 2 + pw, -_UP_OFF[pw][k], -_UP_OFF[ph][j], -_UP_OFF[pt][i]))
+                            g.tapmask.append(_up_mask3(pt, ph, pw, i, j, k))
+    return g
+
+
+def conv3d_dgrad_desc(g: ConvGeom3d, Cout: int, out_strides) -> VqbConv3dDgradDesc:
+    """64-tap form of conv3d_desc (no epilogue, bf16 output)."""
+    d = VqbConv3dDgradDesc()
+    d.C, d.Cout, d.N, d.T, d.H, d.W = g.C, Cout, g.N, g.To, g.Ho, g.Wo
+    d.nviews, d.ntaps, d.flags, d.out_f32 = len(g.views), len(g.taps), 0, 0
+    d.on, d.ot, d.oh, d.ow, d.oc = out_strides
+    for i, v in enumerate(g.views):
+        d.views[i] = v
+    for i, (v, dw, dh, dt) in enumerate(g.taps):
+        d.taps[i] = VqbTap3d(view=v, dw=dw, dh=dh, dt=dt)
+    return d
+
+
+def wgrad3d_desc(g: ConvGeom3d, Cout_pad: int, ksplit: int, dy_view=None, ld_override=0,
+                 col_offset=0) -> VqbWgrad3dDesc:
+    """x operand geometry = forward geometry g; dy is the dense (N, To, Ho, Wo, Cout_pad) tensor unless dy_view is
+    given."""
+    d = VqbWgrad3dDesc()
+    d.C, d.Cout, d.N, d.T, d.H, d.W = g.C, Cout_pad, g.N, g.To, g.Ho, g.Wo
+    d.nviews, d.ntaps, d.ksplit = len(g.views), len(g.taps), ksplit
+    d.ld_override, d.col_offset = ld_override, col_offset
+    d.dy_view = dy_view if dy_view is not None else dense_view3d(g.N, g.To, g.Ho, g.Wo, Cout_pad)
+    for i, v in enumerate(g.views):
+        d.views[i] = v
+    for i, (v, dw, dh, dt) in enumerate(g.taps):
+        d.taps[i] = VqbTap3d(view=v, dw=dw, dh=dh, dt=dt)
+    return d

@@ -1,4 +1,5 @@
-"""H100-native drop-in for the reference `tae.py` (TVAE, the video autoencoder), for no-grad inference.
+"""H100-native drop-in for the reference `tae.py` (TVAE, the video autoencoder): no-grad inference, and training once
+opted in with `enable_training`.
 
 Same names, constructor signatures, parameter creation order (so `torch.manual_seed(s); TVAE(...)` yields the
 reference's initial weights bit for bit), `state_dict` keys and OIDHW shapes, and return values as the reference; no
@@ -14,16 +15,22 @@ einops. Every forward runs hand-written sm_90a kernels (libvqb200.so):
   DiagonalGaussian                                                         -> torch.randn_like(mean) + one fused kernel
 
 Internally activations are bf16 NTHWC (`Act3`); modules accept an `Act3` or an NCTHW tensor and return NCTHW in the
-dtype of their parameters (fp32 or bf16). Inference only: a forward that autograd would have to differentiate (grad
-enabled and parameters that require grad) raises before anything is launched. Deviations from the reference
-(DESIGN.md section 7): inference only; T, H and W divisible by 2^(len(ch_mult)-1) at the encoder; heads of 32 or 64
-channels.
+dtype of their parameters (fp32 or bf16).
+
+Training is opted into explicitly: `tae.enable_training(vae)` (returns vae). Then a grad-enabled forward records the
+autograd functions of ops.py (Conv3dFn, UpConv3dFn, GroupNormSiLUFn, AttentionHdFn, GaussReparamFn), whose backward runs
+the 3-D data- and weight-gradient kernels; parameters may be frozen and the input may require grad (the gradient of the
+video). Without the opt-in, a forward that autograd would have to differentiate (grad enabled and parameters that
+require grad) raises before anything is launched: a grad-enabled forward of a full clip would otherwise keep many GB of
+activations alive. Modules with bf16 parameters stay inference-only. Deviations from the reference (DESIGN.md
+section 7): training is opt-in; T, H and W divisible by 2^(len(ch_mult)-1) at the encoder; heads of 32 or 64 channels.
 
 Reference citations: tae.py:9-10 swish, :13-54 AttnBlock, :57-90 ResnetBlock, :93-104 Downsample, :107-117 Upsample,
 :120-184 Encoder, :187-250 Decoder, :253-266 DiagonalGaussian, :269-297 TVAE.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import os
 import sys
@@ -63,12 +70,48 @@ def _param_dtype(module: nn.Module):
     return p.dtype
 
 
+def enable_training(module: nn.Module, enabled: bool = True) -> nn.Module:
+    """Opts `module` and every submodule into training (enabled=False opts out again); returns `module`.
+
+    Once opted in, a grad-enabled forward records for autograd and `loss.backward()` runs the native 3-D gradient
+    kernels; no-grad forwards are unchanged. Parameters must be float32 (bf16 modules are inference-only)."""
+    for m in module.modules():
+        m._vqb_training = bool(enabled)
+    return module
+
+
+def _opted_in(module: nn.Module) -> bool:
+    return getattr(module, "_vqb_training", False)
+
+
+def _grad_path(module: nn.Module) -> bool:
+    """True when this forward records for autograd: grad enabled and the module opted in."""
+    return torch.is_grad_enabled() and _opted_in(module)
+
+
+def _mode(module: nn.Module):
+    """The forward's autograd context: recording on the training path, torch.no_grad() otherwise."""
+    return contextlib.nullcontext() if _grad_path(module) else torch.no_grad()
+
+
+def _check_trainable(module: nn.Module):
+    for p in module.parameters():
+        if p.dtype != torch.float32:
+            raise RuntimeError(
+                f"vqgan-training_b200: tae.{type(module).__name__} has {p.dtype} parameters; training needs float32 "
+                "master weights (bf16 modules are inference-only). Run it under torch.no_grad() / "
+                "torch.inference_mode(), or train the float32 module (`.float()`).")
+
+
 def _inference_only(module: nn.Module):
+    if _grad_path(module):
+        _check_trainable(module)
+        return
     if torch.is_grad_enabled() and any(p.requires_grad for p in module.parameters()):
         raise RuntimeError(
-            f"vqgan-training_b200: tae.{type(module).__name__} runs inference only (there are no 3-D gradient "
-            "kernels): run it under torch.no_grad() / torch.inference_mode(), or freeze its parameters "
-            "(requires_grad_(False)).")
+            f"vqgan-training_b200: tae.{type(module).__name__} runs inference only unless opted into training: run it "
+            "under torch.no_grad() / torch.inference_mode(), freeze its parameters (requires_grad_(False)), or call "
+            "tae.enable_training(module) to train it.")
 
 
 def _enter(x, module: nn.Module):
@@ -81,7 +124,10 @@ def _enter(x, module: nn.Module):
         raise ValueError(f"tae.{type(module).__name__}: expected an NCTHW tensor, got shape {tuple(x.shape)}")
     ops.require_cuda(x)
     N, C, T, H, W = x.shape
-    y = ops.to_nhwc(x.detach().reshape(N, C, T * H, W))
+    if _grad_path(module):  # the input may require grad (the gradient of the video)
+        y = ops.to_nhwc(x.reshape(N, C, T * H, W))
+    else:
+        y = ops.to_nhwc(x.detach().reshape(N, C, T * H, W))
     return Act3(y.view(N, T, H, W, y.shape[-1]), C), True
 
 
@@ -118,8 +164,10 @@ class Conv3d(nn.Conv3d):
         raise NotImplementedError(f"Conv3d k={k} s={s} p={p} is not on the native path")
 
     def forward_act(self, a: Act3, residual: Act3 = None, ncthw_out=False):
-        out = ops.conv3d(a.t, self.weight, self.bias, self._packed, self._kind(),
-                         residual.t if residual is not None else None, ncthw_out)
+        # grad is enabled here only on the training path (the inference path runs under torch.no_grad())
+        conv = ops.conv3d_train if torch.is_grad_enabled() else ops.conv3d
+        out = conv(a.t, self.weight, self.bias, self._packed, self._kind(),
+                   residual.t if residual is not None else None, ncthw_out)
         return out if ncthw_out else Act3(out, self.out_channels)
 
     def forward(self, x):
@@ -128,12 +176,21 @@ class Conv3d(nn.Conv3d):
         if self._kind() == "s2":
             raise RuntimeError("stride-2 Conv3d is only reachable through Downsample")
         a, ext = _enter(x, self)
-        with torch.no_grad():
+        with _mode(self):
             return _exit(self.forward_act(a), ext, self)
 
 
 def _norm(gn: nn.GroupNorm, a: Act3, silu: bool) -> Act3:
     return Act3(ops.group_norm_silu3d(a.t, gn.weight, gn.bias, gn.num_groups, gn.eps, silu), a.C)
+
+
+def _norm_skip(gn: nn.GroupNorm, a: Act3, silu: bool):
+    """Training path: GroupNorm(+swish) that also returns its input as the skip connection, so the skip's gradient is
+    summed into dx inside the GroupNorm backward kernel (GroupNormSiLUFn with_skip)."""
+    N, T, H, W, C = a.t.shape
+    y, skip = ops.group_norm_silu(a.t.reshape(N, T * H, W, C), gn.weight, gn.bias, gn.num_groups, gn.eps, silu,
+                                  with_skip=True)
+    return Act3(y.view(N, T, H, W, C), a.C), Act3(skip.view(N, T, H, W, C), a.C)
 
 
 class AttnBlock(nn.Module):
@@ -156,15 +213,21 @@ class AttnBlock(nn.Module):
     def attention(self, h_) -> Act3:
         self._check_heads()
         a, ext = _enter(h_, self)
-        with torch.no_grad():
+        with _mode(self):
             qkv = self.qkv.forward_act(_norm(self.norm, a, silu=False))
-            o = Act3(ops.attention_hd(qkv.t, self.num_heads, self.head_dim), self.in_channels)
+            attn = ops.attention_hd_train if torch.is_grad_enabled() else ops.attention_hd
+            o = Act3(attn(qkv.t, self.num_heads, self.head_dim), self.in_channels)
             return _exit(o, ext, self)
 
     def forward(self, x):
         self._check_heads()
         a, ext = _enter(x, self)
-        with torch.no_grad():
+        with _mode(self):
+            if torch.is_grad_enabled():  # training path
+                hn, skip = _norm_skip(self.norm, a, silu=False)
+                qkv = self.qkv.forward_act(hn)
+                h = Act3(ops.attention_hd_train(qkv.t, self.num_heads, self.head_dim), self.in_channels)
+                return _exit(self.proj_out.forward_act(h, residual=skip), ext, self)
             h = self.attention(a)
             out = self.proj_out.forward_act(h, residual=a)  # x + proj_out(attention(x)) fused in the conv epilogue
             return _exit(out, ext, self)
@@ -185,7 +248,13 @@ class ResnetBlock(nn.Module):
 
     def forward(self, x):
         a, ext = _enter(x, self)
-        with torch.no_grad():
+        with _mode(self):
+            if torch.is_grad_enabled():  # training path
+                hn, skip = _norm_skip(self.norm1, a, silu=True)
+                h = self.conv1.forward_act(hn)
+                h = _norm(self.norm2, h, silu=True)
+                skip = self.nin_shortcut.forward_act(skip) if self.in_channels != self.out_channels else skip
+                return _exit(self.conv2.forward_act(h, residual=skip), ext, self)
             h = self.conv1.forward_act(_norm(self.norm1, a, silu=True))
             h = _norm(self.norm2, h, silu=True)
             skip = self.nin_shortcut.forward_act(a) if self.in_channels != self.out_channels else a
@@ -209,7 +278,7 @@ class Downsample(nn.Module):
         # F.pad(x, (0,1,0,1,0,1)) + stride-2 conv (tae.py:100-104): the pad planes are the TMA unit's zero fill
         _check_even(tuple(x.shape), "Downsample")
         a, ext = _enter(x, self)
-        with torch.no_grad():
+        with _mode(self):
             return _exit(self.conv.forward_act(a), ext, self)
 
 
@@ -221,8 +290,9 @@ class Upsample(nn.Module):
     def forward(self, x: Tensor):
         # nearest x2 + 3x3x3 conv as eight 2x2x2-tap phase convs over the low-resolution tensor
         a, ext = _enter(x, self)
-        with torch.no_grad():
-            y = ops.upsample_conv3d(a.t, self.conv.weight, self.conv.bias, self.conv._packed)
+        with _mode(self):
+            up = ops.upsample_conv3d_train if torch.is_grad_enabled() else ops.upsample_conv3d
+            y = up(a.t, self.conv.weight, self.conv.bias, self.conv._packed)
             return _exit(Act3(y, self.conv.out_channels), ext, self)
 
 
@@ -276,7 +346,7 @@ class Encoder(nn.Module):
                              f"{self.num_resolutions - 1} Downsample levels); got input shape {tuple(x.shape)}")
         self.mid.attn_1._check_heads()
         a, _ = _enter(x, self)
-        with torch.no_grad():
+        with _mode(self):
             a = self.conv_in.forward_act(a)
             for i_level in range(self.num_resolutions):
                 for i_block in range(self.num_res_blocks):
@@ -339,7 +409,7 @@ class Decoder(nn.Module):
     def forward(self, z: Tensor) -> Tensor:
         self.mid.attn_1._check_heads()
         a, _ = _enter(z, self)
-        with torch.no_grad():
+        with _mode(self):
             a = self.conv_in.forward_act(a)
             a = self.mid.block_1(a)
             a = self.mid.attn_1(a)
@@ -368,8 +438,15 @@ class DiagonalGaussian(nn.Module):
         if self.chunk_dim != 1:
             raise NotImplementedError("tae.DiagonalGaussian: the native sampler takes chunk_dim=1 (channels)")
         if torch.is_grad_enabled() and z.requires_grad:
-            raise RuntimeError("vqgan-training_b200: tae.DiagonalGaussian runs inference only: run it under "
-                               "torch.no_grad() / torch.inference_mode()")
+            if not _opted_in(self):
+                raise RuntimeError("vqgan-training_b200: tae.DiagonalGaussian runs inference only unless opted into "
+                                   "training: run it under torch.no_grad() / torch.inference_mode(), or call "
+                                   "tae.enable_training(module)")
+            if z.dtype != torch.float32:
+                raise RuntimeError(f"vqgan-training_b200: tae.DiagonalGaussian: training needs a float32 latent, got "
+                                   f"{z.dtype} (bf16 modules are inference-only)")
+            eps = torch.randn_like(mean)  # the reference's own draw (tae.py:264)
+            return ops.gauss_reparam_train(z, eps)
         # the reference's own draw (tae.py:264): a seeded run consumes the same RNG stream and gets the same eps
         eps = torch.randn_like(mean)
         return ops.gauss_reparam(z, eps)
@@ -400,6 +477,8 @@ class TVAE(nn.Module):
         self.reg = DiagonalGaussian()
 
     def forward(self, x: Tensor) -> Tensor:
+        if _grad_path(self):
+            _check_trainable(self)  # a bf16 part is refused before the encoder launches anything
         z = self.encoder(x)
         z_s = self.reg(z)
         decz = self.decoder(z_s)
