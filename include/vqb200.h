@@ -155,6 +155,11 @@ int vqb_gn_silu_fwd(const void* x, void* y, const float* gamma, const float* bet
 /* forward when the producing conv already accumulated chsums[N][C][2] (VQB_EPI_STATS): finalise + apply only */
 int vqb_gn_silu_fwd_pre(const void* x, void* y, const float* gamma, const float* beta, float* mr, const float* chsums,
                         int N, int HW, int C, int G, float eps, int silu, void* stream);
+/* the apply pass alone, with the mr = [N][G][2] (mean, rstd) of an earlier vqb_gn_silu_fwd over the same x: same kernel
+ * and grid, so y is bit-identical to that call's y. Recomputes a ResnetBlock's normalised activations in its backward
+ * (tae.ResnetBlock, enable_training(..., recompute=True)). x, y 16-byte aligned; gamma, beta, mr 4-byte aligned. */
+int vqb_gn_silu_apply(const void* x, void* y, const float* gamma, const float* beta, const float* mr, int N, int HW,
+                      int C, int G, int silu, void* stream);
 /* dx_colsum (optional [C] fp32): per-channel sums of dx = bias gradient of the conv that produced x, same pass */
 int vqb_gn_silu_bwd(const void* x, const void* dy, const void* add, void* dx, const float* gamma, const float* beta,
                     const float* mr, float* dgamma, float* dbeta, float* ws, int N, int HW, int C, int G, int silu,

@@ -3,10 +3,16 @@ torch.optim.AdamW, against the same step of the reference arithmetic (oracle/tae
 softmax attention) under bf16 autocast with cuDNN on the same GPU.
 
 Usage: python tools/tae_train_bench.py [--frames 16] [--res 256] [--ch 64] [--batch 1] [--steps 5] [--warmup 2]
-           [--skip-peer]
+           [--skip-peer] [--recompute]
 
-Prints one JSON line per arm (native, peer) with steps/s, frames/s, whole-step TFLOP/s and peak allocated memory, plus
-the card's name and power limit read in the same run. FLOPs are counted from the plan shapes (step_flops): the forward
+Prints one JSON line per arm (native, native + recompute with --recompute, peer) with steps/s, frames/s, whole-step
+TFLOP/s and peak allocated memory, plus the card's name and power limit read in the same run. Every line also carries
+the arm's saved-activation bytes predicted from the shapes (saved_activation_bytes). An arm whose prediction exceeds
+3/4 of the card's memory is not run (its line says so): the rest is left for weights, optimizer state and the
+backward's transient buffers, and a run that would exhaust the card measures nothing.
+
+FLOPs are counted from the plan shapes (step_flops), the same for every arm: the recompute arm's extra conv1 forwards
+show up as a lower TFLOP/s. step_flops counts the forward
 GEMMs of oracle.tae_oracle.flops, plus for every convolution a weight-gradient GEMM and a data-gradient GEMM of the
 same size as its forward (27 rotated taps for stride 1; the 1 to 8 taps of the eight parity classes, 27 in all, over the
 Downsample's output grid; 64 taps over the low-resolution grid for the folded up-sampling, as its 8 forward phases of 8),
@@ -40,6 +46,53 @@ def step_flops(cfg, N, T, H, W):
     return 3 * TO.flops(cfg, N, T, H, W) - conv_in_dgrad
 
 
+def saved_activation_bytes(cfg, N, T, H, W, recompute):
+    """Bytes of the activations the native training forward keeps for the backward (bf16, channels padded to 8), each
+    tensor counted once, by the module that saves it: conv_in, Downsample and Upsample their input; a ResnetBlock x,
+    hn, h and h2 (recompute: x and two [N, 32, 2] fp32 GroupNorm records); an AttnBlock x, hn, qkv, the attention
+    output and its fp32 log-sum-exp; norm_out + conv_out x and hn; the reparameterisation z and eps (fp32). A lower
+    bound for the eager bf16-autocast peer, which keeps at least these tensors in at least this precision."""
+    cp = lambda c: -(-c // 8) * 8  # noqa: E731
+    tot = 0
+
+    def act(c, v):
+        return 2 * cp(c) * v * N
+
+    def block(cin, cout, v):
+        if recompute:
+            return act(cin, v) + 2 * (N * 32 * 2 * 4)
+        return act(cin, v) * 2 + act(cout, v) * 2
+
+    def mid(c, v):
+        return 2 * block(c, c, v) + act(c, v) * 6 + 4 * 8 * v * N
+
+    n = len(cfg.ch_mult)
+    ch, vox = cfg.ch, T * H * W
+    tot += act(cfg.in_channels, vox)  # encoder conv_in
+    cin = ch
+    for i in range(n):
+        cout = ch * cfg.ch_mult[i]
+        for _ in range(cfg.num_res_blocks):
+            tot += block(cin, cout, vox)
+            cin = cout
+        if i != n - 1:
+            tot += act(cin, vox)  # Downsample input
+            vox //= 8
+    tot += mid(cin, vox) + 2 * act(cin, vox)  # mid, norm_out + conv_out
+    tot += 4 * 3 * cfg.z_channels * vox * N  # z and eps
+    cin = ch * cfg.ch_mult[-1]
+    tot += act(cfg.z_channels, vox) + mid(cin, vox)  # decoder conv_in, mid
+    for i in reversed(range(n)):
+        cout = ch * cfg.ch_mult[i]
+        for _ in range(cfg.num_res_blocks + 1):
+            tot += block(cin, cout, vox)
+            cin = cout
+        if i != 0:
+            tot += act(cin, vox)  # Upsample input
+            vox *= 8
+    return tot + 2 * act(cin, vox)  # norm_out + conv_out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=16)
@@ -49,6 +102,8 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--skip-peer", action="store_true")
+    ap.add_argument("--recompute", action="store_true",
+                    help="also time the native step with tae.enable_training(vae, recompute=True)")
     a = ap.parse_args()
 
     import tae
@@ -57,32 +112,51 @@ def main():
     N, T, H, W = a.batch, a.frames, a.res, a.res
     flops = step_flops(cfg, N, T, H, W)
     info = card()
+    budget = 0.75 * torch.cuda.get_device_properties(torch.cuda.current_device()).total_memory
     torch.manual_seed(0)
     x = torch.rand(N, 3, T, H, W, device="cuda") * 2 - 1
 
-    def report(arm, ms, peak):
-        print(json.dumps({"arm": arm, "frames": T, "res": a.res, "ch": a.ch, "batch": N, "ms_per_step": round(ms, 2),
-                          "steps_per_s": round(1e3 / ms, 3), "frames_per_s": round(N * T * 1e3 / ms, 2),
-                          "tflops": round(flops / ms / 1e9, 1), "peak_alloc_gb": round(peak / 2 ** 30, 2),
-                          "gpu": info}), flush=True)
+    def report(arm, ms, peak, pred):
+        line = {"arm": arm, "frames": T, "res": a.res, "ch": a.ch, "batch": N,
+                "predicted_saved_gb": round(pred / 2 ** 30, 2)}
+        if ms is None:
+            line["skipped"] = f"predicted saved activations exceed 3/4 of the card ({budget / 2 ** 30:.1f} GB)"
+        else:
+            line.update(ms_per_step=round(ms, 2), steps_per_s=round(1e3 / ms, 3),
+                        frames_per_s=round(N * T * 1e3 / ms, 2), tflops=round(flops / ms / 1e9, 1),
+                        peak_alloc_gb=round(peak / 2 ** 30, 2))
+        print(json.dumps(dict(line, gpu=info)), flush=True)
 
-    torch.manual_seed(1)
-    vae = tae.enable_training(tae.TVAE(**cfg.kwargs()).cuda())
-    opt = torch.optim.AdamW(vae.parameters(), lr=1e-4)
+    def native(arm, recompute):
+        pred = saved_activation_bytes(cfg, N, T, H, W, recompute)
+        if pred > budget:
+            report(arm, None, None, pred)
+            return
+        torch.manual_seed(1)
+        vae = tae.enable_training(tae.TVAE(**cfg.kwargs()).cuda(), recompute=recompute)
+        opt = torch.optim.AdamW(vae.parameters(), lr=1e-4)
 
-    def native_step():
-        opt.zero_grad(set_to_none=True)
-        decz, z = vae(x)
-        loss = _loss(decz, x, z)
-        loss.backward()
-        opt.step()
-        return loss
+        def native_step():
+            opt.zero_grad(set_to_none=True)
+            decz, z = vae(x)
+            loss = _loss(decz, x, z)
+            loss.backward()
+            opt.step()
+            return loss
 
-    ms, peak, _ = timed(native_step, a.steps, a.warmup)
-    report("native", ms, peak)
-    del vae, opt
-    torch.cuda.empty_cache()
+        ms, peak, _ = timed(native_step, a.steps, a.warmup)
+        report(arm, ms, peak, pred)
+        del vae, opt
+        torch.cuda.empty_cache()
+
+    native("native", False)
+    if a.recompute:
+        native("native + recompute", True)
     if a.skip_peer:
+        return
+    pred = saved_activation_bytes(cfg, N, T, H, W, False)  # a lower bound for the peer
+    if pred > budget:
+        report("bf16-autocast cuDNN peer", None, None, pred)
         return
     torch.manual_seed(1)
     sd = {k: v.cuda().requires_grad_(True) for k, v in tae.TVAE(**cfg.kwargs()).state_dict().items()}
@@ -100,7 +174,7 @@ def main():
         return loss
 
     ms, peak, _ = timed(peer_step, a.steps, a.warmup)
-    report("bf16-autocast cuDNN peer", ms, peak)
+    report("bf16-autocast cuDNN peer", ms, peak, pred)
 
 
 if __name__ == "__main__":

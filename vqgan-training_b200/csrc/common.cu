@@ -115,7 +115,7 @@ bool device_is_sm90() {
 extern "C" {
 
 const char* vqb_last_error(void) { return vqb::g_err; }
-int vqb_version(void) { return 102; }
+int vqb_version(void) { return 103; }
 int vqb_device_ok(void) { return (vqb::device_is_sm90() && vqb::get_encode_fn() != nullptr) ? 1 : 0; }
 int vqb_kernel_launch_count(void) { return vqb::g_launches.load(std::memory_order_relaxed); }
 

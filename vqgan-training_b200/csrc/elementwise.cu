@@ -874,6 +874,28 @@ int vqb_gn_silu_fwd(const void* x, void* y, const float* gamma, const float* bet
     return VQB_OK;
 }
 
+// GroupNorm(+SiLU) apply pass alone, with the mean/rstd mr [N][G][2] of an earlier vqb_gn_silu_fwd: the same kernel and
+// grid as that call's apply pass, so y is bit-identical to its y (the ResnetBlock recompute of tae.py).
+int vqb_gn_silu_apply(const void* x, void* y, const float* gamma, const float* beta, const float* mr, int N, int HW,
+                      int C, int G, int silu, void* stream) {
+    VQB_CHECK(x && y && gamma && beta && mr, "vqb_gn_silu_apply: null pointer");
+    VQB_CHECK(N > 0 && HW > 0 && G > 0 && C % 8 == 0 && C % G == 0 && C <= 2048 && (silu == 0 || silu == 1),
+              "vqb_gn_silu_apply: N=%d HW=%d C=%d G=%d silu=%d unsupported", N, HW, C, G, silu);
+    VQB_CHECK(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15u) == 0 &&
+                  ((reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta) |
+                    reinterpret_cast<uintptr_t>(mr)) & 3u) == 0,
+              "vqb_gn_silu_apply: x and y must be 16-byte aligned, gamma, beta and mr 4-byte aligned");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_gn_silu_apply: current device is not sm_90");
+    int chunks, ppc;
+    const int T = cv_threads(C);
+    cv_grid(HW, C, N, gn_apply_kernel, 0, chunks, ppc);
+    gn_apply_kernel<<<dim3(chunks, N), T, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), mr, gamma, beta, HW, C, G, ppc, silu);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
 // GroupNorm(+SiLU) forward when the per-(n, channel) sums [N][C][2] (sum, sum of squares; fp32) were already produced by
 // the convolution that wrote x (vqb_conv_gemm with VQB_EPI_STATS): finalise + one apply pass, no statistics pass.
 int vqb_gn_silu_fwd_pre(const void* x, void* y, const float* gamma, const float* beta, float* mr, const float* chsums,

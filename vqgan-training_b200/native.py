@@ -155,6 +155,7 @@ def load():
         "vqb_wgrad3d_gemm": (i32, [C.POINTER(VqbWgrad3dDesc), vp, vp, vp, vp]),
         "vqb_attn_bwd_hd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
         "vqb_gauss_reparam_bwd": (i32, [vp, vp, vp, vp, i32, i32, i64, vp]),
+        "vqb_gn_silu_apply": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)

@@ -817,17 +817,15 @@ class GroupNormSiLUFn(torch.autograd.Function):
     def forward(ctx, x, gamma, beta, groups, eps, silu, with_skip, chsums=None):
         require_cuda(x)
         x = x.contiguous()
-        N, H, W, C = x.shape
-        y = torch.empty_like(x)
-        mr = torch.empty(N, groups, 2, device=x.device, dtype=torch.float32)
-        ga, be = gamma.detach().float(), beta.detach().float()
         if chsums is not None:  # statistics were accumulated by the epilogue of the conv that produced x
+            N, H, W, C = x.shape
+            y = torch.empty_like(x)
+            mr = torch.empty(N, groups, 2, device=x.device, dtype=torch.float32)
+            ga, be = gamma.detach().float(), beta.detach().float()
             check(_L().vqb_gn_silu_fwd_pre(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), ptr(chsums), N, H * W, C, groups,
                                            eps, 1 if silu else 0, stream_ptr()), "gn_silu_fwd_pre")
         else:
-            ws = torch.empty(N * C * 2, device=x.device, dtype=torch.float64)
-            check(_L().vqb_gn_silu_fwd(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), ptr(ws), N, H * W, C, groups, eps,
-                                       1 if silu else 0, stream_ptr()), "gn_silu_fwd")
+            y, mr = gn_silu_fwd(x, gamma, beta, groups, eps, silu)
         ctx.save_for_backward(x, gamma, beta, mr)
         ctx.groups, ctx.silu, ctx.with_skip = groups, silu, with_skip
         ctx.set_materialize_grads(False)  # an unused output arrives as None, not as a zero tensor
@@ -839,21 +837,50 @@ class GroupNormSiLUFn(torch.autograd.Function):
     def backward(ctx, gy, gskip=None):
         x, gamma, beta, mr = ctx.saved_tensors
         inference_only(gamma, beta)
-        N, H, W, C = x.shape
         if gy is None:  # only the skip output was used
             return (gskip, None, None, None, None, None, None, None)
-        gy = gy.contiguous()
-        add = gskip.contiguous() if gskip is not None else None
-        dx = torch.empty_like(x)
-        dg, db = grad_out(gamma), grad_out(beta)
-        ws = torch.empty(N * C * 2 + N * ctx.groups * 2, device=x.device, dtype=torch.float32)
-        ga, be = gamma.detach().float(), beta.detach().float()
-        cs = torch.empty(C, device=x.device, dtype=torch.float32)
-        check(_L().vqb_gn_silu_bwd(ptr(x), ptr(gy), ptr(add), ptr(dx), ptr(ga), ptr(be), ptr(mr), ptr(dg), ptr(db),
-                                   ptr(ws), N, H * W, C, ctx.groups, 1 if ctx.silu else 0, ptr(cs), stream_ptr()),
-              "gn_silu_bwd")
-        _dx_colsum_slot[0] = (dx, dx._version, cs)
+        dx, dg, db = gn_silu_bwd(x, gy, gskip, gamma, beta, mr, ctx.groups, ctx.silu)
         return dx, dg, db, None, None, None, None, None
+
+
+def gn_silu_fwd(x, gamma, beta, groups, eps, silu):
+    """GroupNorm(+swish) of a contiguous bf16 NHWC x through the deterministic statistics pass -> (y, mr), where
+    mr [N, groups, 2] holds the (mean, rstd) the backward and gn_silu_apply take."""
+    N, H, W, C = x.shape
+    y = torch.empty_like(x)
+    mr = torch.empty(N, groups, 2, device=x.device, dtype=torch.float32)
+    ga, be = gamma.detach().float(), beta.detach().float()
+    ws = torch.empty(N * C * 2, device=x.device, dtype=torch.float64)
+    check(_L().vqb_gn_silu_fwd(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), ptr(ws), N, H * W, C, groups, eps,
+                               1 if silu else 0, stream_ptr()), "gn_silu_fwd")
+    return y, mr
+
+
+def gn_silu_apply(x, gamma, beta, mr, silu):
+    """The apply pass of gn_silu_fwd alone, with that call's mr: the same y, bit for bit (vqb_gn_silu_apply)."""
+    N, H, W, C = x.shape
+    y = torch.empty_like(x)
+    ga, be = gamma.detach().float(), beta.detach().float()
+    check(_L().vqb_gn_silu_apply(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), N, H * W, C, mr.shape[1],
+                                 1 if silu else 0, stream_ptr()), "gn_silu_apply")
+    return y
+
+
+def gn_silu_bwd(x, gy, gskip, gamma, beta, mr, groups, silu):
+    """GroupNorm(+swish) backward -> (dx, dgamma, dbeta); gskip (optional) is summed into dx. The per-channel sums of dx
+    are left in the colsum slot for the bias gradient of the conv that produced x."""
+    N, H, W, C = x.shape
+    gy = gy.contiguous()
+    add = gskip.contiguous() if gskip is not None else None
+    dx = torch.empty_like(x)
+    dg, db = grad_out(gamma), grad_out(beta)
+    ws = torch.empty(N * C * 2 + N * groups * 2, device=x.device, dtype=torch.float32)
+    ga, be = gamma.detach().float(), beta.detach().float()
+    cs = torch.empty(C, device=x.device, dtype=torch.float32)
+    check(_L().vqb_gn_silu_bwd(ptr(x), ptr(gy), ptr(add), ptr(dx), ptr(ga), ptr(be), ptr(mr), ptr(dg), ptr(db),
+                               ptr(ws), N, H * W, C, groups, 1 if silu else 0, ptr(cs), stream_ptr()), "gn_silu_bwd")
+    _dx_colsum_slot[0] = (dx, dx._version, cs)
+    return dx, dg, db
 
 
 def group_norm_silu(x, gamma, beta, groups=32, eps=1e-6, silu=True, with_skip=False, chsums=None):
@@ -1139,50 +1166,127 @@ class Conv3dFn(torch.autograd.Function):
     def backward(ctx, gout):
         x, weight = ctx.saved_tensors
         inference_only(weight)
-        cache, kind = ctx.cache, ctx.kind
-        N, T, H, W, Cp = x.shape
-        Cout, Cin = weight.shape[:2]
-        Cop = plans.cpad(Cout)
-        if kind == "p1":
-            g = cache.geom(("p1", N, T, H, W), lambda: plans.geom_s1(N, T * H, W, Cp, 1))
-            To, Ho, Wo = T, H, W
-        else:
-            g = cache.geom((kind, N, T, H, W), lambda: (plans.geom3_s1 if kind == "s1" else plans.geom3_s2)(
-                N, T, H, W, Cp))
-            To, Ho, Wo = g.To, g.Ho, g.Wo
-        dy = _ncthw_grad_to_nthwc(gout, Cout, Cop) if ctx.ncthw_out else gout.contiguous()
-        gx = gw = gb = gres = None
-        if ctx.needs_input_grad[0]:
-            gx = (torch.empty if Cp == Cin else torch.zeros)(N, T, H, W, Cp, device=x.device, dtype=torch.bfloat16)
-            if kind == "p1":
-                gd = cache.geom(("p1d", N, T, H, W), lambda: plans.geom_s1_dgrad(N, T * H, W, Cop, 1))
-                wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
-                run_conv_gemm(gd, dy, wpd, Cin, gx, plans.nhwc_strides(T * H, W, Cp))
-            elif kind == "s1":
-                gd = cache.geom(("s1d", N, T, H, W), lambda: plans.geom3_s1_dgrad(N, T, H, W, Cop))
-                wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
-                run_conv3d(gd, dy, wpd, Cin, gx, plans.nthwc_strides(T, H, W, Cp))
-            else:
-                for pt, ph, pw, gd in cache.geom(("s2d", N, T, H, W),
-                                                 lambda: plans.geom3_s2_dgrad_classes(N, T, H, W, Cop)):
-                    wpd = cache.get(weight, ("dgrad", kind, pt, ph, pw), gd.tapmap, True, Cop)
-                    strides, off = plans.s2_dgrad_out(T, H, W, Cp, pt, ph, pw)
-                    run_conv3d(gd, dy, wpd, Cin, gx, strides, out_off_elems=off)
-        if ctx.needs_input_grad[1]:
-            gw = grad_out(weight)
-            if kind == "p1":
-                run_wgrad(g, x, dy, (Cout, Cin, 1, 1), Cop, out=gw.view(Cout, Cin, 1, 1))
-            else:
-                run_wgrad3d(g, x, dy, weight, Cop, gw)
-        if ctx.has_bias and ctx.needs_input_grad[2]:
-            gb = _bias_grad(dy, N * To * Ho * Wo, Cout, Cop)
-        if ctx.has_res and ctx.needs_input_grad[3]:
-            gres = gout if ctx.ncthw_out else dy
+        gx, gw, gb, gres = conv3d_backward(x, weight, gout, ctx.cache, ctx.kind, ctx.ncthw_out, ctx.has_bias,
+                                           ctx.has_res, ctx.needs_input_grad[:4])
         return gx, gw, gb, gres, None, None, None
+
+
+def conv3d_backward(x, weight, gout, cache, kind, ncthw_out, has_bias, has_res, needs):
+    """Backward of conv3d(x, weight, bias, cache, kind, residual, ncthw_out) from its input x, its weight and the
+    incoming gradient -> (gx, gw, gb, gres); needs: which of (x, weight, bias, residual) want a gradient."""
+    N, T, H, W, Cp = x.shape
+    Cout, Cin = weight.shape[:2]
+    Cop = plans.cpad(Cout)
+    if kind == "p1":
+        g = cache.geom(("p1", N, T, H, W), lambda: plans.geom_s1(N, T * H, W, Cp, 1))
+        To, Ho, Wo = T, H, W
+    else:
+        g = cache.geom((kind, N, T, H, W), lambda: (plans.geom3_s1 if kind == "s1" else plans.geom3_s2)(
+            N, T, H, W, Cp))
+        To, Ho, Wo = g.To, g.Ho, g.Wo
+    dy = _ncthw_grad_to_nthwc(gout, Cout, Cop) if ncthw_out else gout.contiguous()
+    gx = gw = gb = gres = None
+    if needs[0]:
+        gx = (torch.empty if Cp == Cin else torch.zeros)(N, T, H, W, Cp, device=x.device, dtype=torch.bfloat16)
+        if kind == "p1":
+            gd = cache.geom(("p1d", N, T, H, W), lambda: plans.geom_s1_dgrad(N, T * H, W, Cop, 1))
+            wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
+            run_conv_gemm(gd, dy, wpd, Cin, gx, plans.nhwc_strides(T * H, W, Cp))
+        elif kind == "s1":
+            gd = cache.geom(("s1d", N, T, H, W), lambda: plans.geom3_s1_dgrad(N, T, H, W, Cop))
+            wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
+            run_conv3d(gd, dy, wpd, Cin, gx, plans.nthwc_strides(T, H, W, Cp))
+        else:
+            for pt, ph, pw, gd in cache.geom(("s2d", N, T, H, W),
+                                             lambda: plans.geom3_s2_dgrad_classes(N, T, H, W, Cop)):
+                wpd = cache.get(weight, ("dgrad", kind, pt, ph, pw), gd.tapmap, True, Cop)
+                strides, off = plans.s2_dgrad_out(T, H, W, Cp, pt, ph, pw)
+                run_conv3d(gd, dy, wpd, Cin, gx, strides, out_off_elems=off)
+    if needs[1]:
+        gw = grad_out(weight)
+        if kind == "p1":
+            run_wgrad(g, x, dy, (Cout, Cin, 1, 1), Cop, out=gw.view(Cout, Cin, 1, 1))
+        else:
+            run_wgrad3d(g, x, dy, weight, Cop, gw)
+    if has_bias and needs[2]:
+        gb = _bias_grad(dy, N * To * Ho * Wo, Cout, Cop)
+    if has_res and needs[3]:
+        gres = gout if ncthw_out else dy
+    return gx, gw, gb, gres
 
 
 def conv3d_train(x, weight, bias, cache, kind="s1", residual=None, ncthw_out=False):
     return Conv3dFn.apply(x, weight, bias, residual, cache, kind, ncthw_out)
+
+
+class ResnetBlock3dRecomputeFn(torch.autograd.Function):
+    """tae.ResnetBlock as one autograd node that keeps only its input x, the two GroupNorm (mean, rstd) records and its
+    parameters for the backward, instead of x, hn = swish(norm1(x)), h = conv1(hn) and h2 = swish(norm2(h)).
+
+    The forward is the block's inference arithmetic (the kernels the non-recomputing training forward runs). The
+    backward rebuilds hn, h and h2 bit for bit: the GroupNorm apply pass with the saved mr, and conv1, which is
+    deterministic. conv2 is not recomputed; its backward needs only h2, its weight and the incoming gradient. Then it
+    runs the backward of conv2, nin_shortcut, norm2, conv1 and norm1 (with the skip gradient summed in) in the order
+    autograd runs them without recompute, so every gradient, bias column sum and grad_out slot is the same.
+    spec: (groups1, eps1, groups2, eps2, conv1 cache, conv2 cache, nin_shortcut cache or None)."""
+
+    @staticmethod
+    def forward(ctx, x, spec, n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb):
+        g1, e1, g2, e2, k1, k2, ks = spec
+        x = x.contiguous()
+        N, T, H, W, C = x.shape
+        hn, mr1 = gn_silu_fwd(x.view(N, T * H, W, C), n1w, n1b, g1, e1, True)
+        h = conv3d(hn.view(N, T, H, W, C), c1w, c1b, k1, "s1")
+        Co = h.shape[-1]
+        h2, mr2 = gn_silu_fwd(h.view(N, T * H, W, Co), n2w, n2b, g2, e2, True)
+        skip = conv3d(x, sw, sb, ks, "p1") if sw is not None else x
+        out = conv3d(h2.view(N, T, H, W, Co), c2w, c2b, k2, "s1", skip)
+        # the parameters go through save_for_backward so that an in-place change before the backward raises
+        ctx.save_for_backward(x, mr1, mr2, n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb)
+        ctx.spec = spec
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, mr1, mr2, n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb = ctx.saved_tensors
+        inference_only(n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb)
+        g1, _, g2, _, k1, k2, ks = ctx.spec
+        nig = ctx.needs_input_grad
+        N, T, H, W, C = x.shape
+        x4 = x.view(N, T * H, W, C)
+        hn = gn_silu_apply(x4, n1w, n1b, mr1, True).view(N, T, H, W, C)
+        h = conv3d(hn, c1w, c1b, k1, "s1")
+        Co = h.shape[-1]
+        h4 = h.view(N, T * H, W, Co)
+        h2 = gn_silu_apply(h4, n2w, n2b, mr2, True).view(N, T, H, W, Co)
+        # which intermediate gradients the non-recomputing graph would form
+        need_hn = nig[0] or nig[2] or nig[3]  # also the skip output of norm1
+        need_h = need_hn or nig[4] or nig[5]
+        need_h2 = need_h or nig[6] or nig[7]
+        need_res = need_hn or (sw is not None and (nig[10] or nig[11]))
+        gx = gn1w = gn1b = gc1w = gc1b = gn2w = gn2b = gsw = gsb = None
+        gh2, gc2w, gc2b, gskip = conv3d_backward(h2, c2w, gout, k2, "s1", False, c2b is not None, True,
+                                                 (need_h2, nig[8], nig[9], need_res))
+        del h2
+        if sw is not None and need_res:
+            gskip, gsw, gsb, _ = conv3d_backward(x, sw, gskip, ks, "p1", False, sb is not None, False,
+                                                 (need_hn, nig[10], nig[11], False))
+        if need_h2:
+            gh, gn2w, gn2b = gn_silu_bwd(h4, gh2, None, n2w, n2b, mr2, g2, True)
+            del h, h4, gh2
+            if need_h:
+                ghn, gc1w, gc1b, _ = conv3d_backward(hn, c1w, gh.view(N, T, H, W, Co), k1, "s1", False,
+                                                     c1b is not None, False, (need_hn, nig[4], nig[5], False))
+                del hn, gh
+                if need_hn:
+                    gx, gn1w, gn1b = gn_silu_bwd(x4, ghn, gskip, n1w, n1b, mr1, g1, True)
+                    gx = gx.view(N, T, H, W, C)
+        grads = (gn1w, gn1b, gc1w, gc1b, gn2w, gn2b, gc2w, gc2b, gsw, gsb)
+        return (gx, None) + tuple(g if nig[i + 2] else None for i, g in enumerate(grads))
+
+
+def resnet_block3d_recompute(x, spec, *params):
+    return ResnetBlock3dRecomputeFn.apply(x, spec, *params)
 
 
 class UpConv3dFn(torch.autograd.Function):

@@ -22,7 +22,9 @@ autograd functions of ops.py (Conv3dFn, UpConv3dFn, GroupNormSiLUFn, AttentionHd
 the 3-D data- and weight-gradient kernels; parameters may be frozen and the input may require grad (the gradient of the
 video). Without the opt-in, a forward that autograd would have to differentiate (grad enabled and parameters that
 require grad) raises before anything is launched: a grad-enabled forward of a full clip would otherwise keep many GB of
-activations alive. Modules with bf16 parameters stay inference-only. Deviations from the reference (DESIGN.md
+activations alive. `tae.enable_training(vae, recompute=True)` bounds that memory: each ResnetBlock then keeps only its
+input for the backward (ops.ResnetBlock3dRecomputeFn) and rebuilds hn, h and h2 there bit for bit, so the gradients
+are those of the plain path. Modules with bf16 parameters stay inference-only. Deviations from the reference (DESIGN.md
 section 7): training is opt-in; T, H and W divisible by 2^(len(ch_mult)-1) at the encoder; heads of 32 or 64 channels.
 
 Reference citations: tae.py:9-10 swish, :13-54 AttnBlock, :57-90 ResnetBlock, :93-104 Downsample, :107-117 Upsample,
@@ -70,13 +72,19 @@ def _param_dtype(module: nn.Module):
     return p.dtype
 
 
-def enable_training(module: nn.Module, enabled: bool = True) -> nn.Module:
-    """Opts `module` and every submodule into training (enabled=False opts out again); returns `module`.
+def enable_training(module: nn.Module, enabled: bool = True, recompute: bool = False) -> nn.Module:
+    """Opts `module` and every submodule into training (enabled=False opts out again and clears `recompute`); returns
+    `module`.
 
     Once opted in, a grad-enabled forward records for autograd and `loss.backward()` runs the native 3-D gradient
-    kernels; no-grad forwards are unchanged. Parameters must be float32 (bf16 modules are inference-only)."""
+    kernels; no-grad forwards are unchanged. Parameters must be float32 (bf16 modules are inference-only).
+    recompute=True makes every ResnetBlock under `module` keep only its input (plus two [N, 32, 2] GroupNorm records)
+    for the backward and rebuild its three inner activations there, bit for bit: less activation memory for one extra
+    conv1 and two GroupNorm apply passes per block in the backward. Gradients equal the non-recomputing path's."""
     for m in module.modules():
         m._vqb_training = bool(enabled)
+        if isinstance(m, ResnetBlock):
+            m._vqb_recompute = bool(enabled and recompute)
     return module
 
 
@@ -246,9 +254,22 @@ class ResnetBlock(nn.Module):
         if self.in_channels != self.out_channels:
             self.nin_shortcut = Conv3d(in_channels, out_channels, kernel_size=1, stride=1, padding=0)
 
+    def _recompute(self, a: Act3) -> Act3:
+        """Training path of enable_training(..., recompute=True): the block as one autograd node that saves only x."""
+        nin = self.nin_shortcut if self.in_channels != self.out_channels else None
+        spec = (self.norm1.num_groups, self.norm1.eps, self.norm2.num_groups, self.norm2.eps, self.conv1._packed,
+                self.conv2._packed, nin._packed if nin is not None else None)
+        out = ops.resnet_block3d_recompute(
+            a.t, spec, self.norm1.weight, self.norm1.bias, self.conv1.weight, self.conv1.bias, self.norm2.weight,
+            self.norm2.bias, self.conv2.weight, self.conv2.bias, nin.weight if nin is not None else None,
+            nin.bias if nin is not None else None)
+        return Act3(out, self.out_channels)
+
     def forward(self, x):
         a, ext = _enter(x, self)
         with _mode(self):
+            if torch.is_grad_enabled() and getattr(self, "_vqb_recompute", False):
+                return _exit(self._recompute(a), ext, self)
             if torch.is_grad_enabled():  # training path
                 hn, skip = _norm_skip(self.norm1, a, silu=True)
                 h = self.conv1.forward_act(hn)
