@@ -12,6 +12,8 @@ Internally activations are bf16 NHWC (`Act`); modules accept either an `Act` (in
 (reference calling convention: converted at the boundary, result returned as NCHW in the dtype of the module's
 parameters). Modules converted with `.bfloat16()` run the same kernels from bf16 master weights and return bf16, like
 the reference's model-card inference recipe; they are inference-only (a backward through them raises).
+`enable_recompute(vae)` bounds training memory: each ResnetBlock then keeps only its input for the backward
+(ops.ResnetBlockRecomputeFn) and rebuilds hn, h and h2 there bit for bit.
 
 Reference citations: ae.py:13-14 swish, :41-53 FP32GroupNorm, :56-93 AttnBlock, :96-140 ResnetBlock, :143-154 Downsample,
 :157-167 Upsample, :170-257 Encoder, :260-333 Decoder, :336-348 DiagonalGaussian, :351-392 VAE.
@@ -200,14 +202,41 @@ class ResnetBlock(nn.Module):
         nn.init.zeros_(self.conv2.bias)
         self.counter = 0
 
+    def _recompute(self, a: Act) -> Act:
+        """Grad-enabled path of enable_recompute: the block as one autograd node that saves only x."""
+        nin = self.nin_shortcut if self.in_channels != self.out_channels else None
+        spec = (self.norm1.num_groups, self.norm1.eps, self.norm2.num_groups, self.norm2.eps, self.conv1._packed,
+                self.conv2._packed, nin._packed if nin is not None else None)
+        out, stats = ops.resnet_block_recompute(
+            a.t, a.stats, spec, self.norm1.weight, self.norm1.bias, self.conv1.weight, self.conv1.bias,
+            self.norm2.weight, self.norm2.bias, self.conv2.weight, self.conv2.bias,
+            nin.weight if nin is not None else None, nin.bias if nin is not None else None)
+        return Act(out, self.out_channels, stats)
+
     def forward(self, x):
         a, ext = _enter(x, self)
+        if torch.is_grad_enabled() and getattr(self, "_vqb_recompute", False):
+            return _exit(self._recompute(a), ext, self)
         h, a_skip = self.norm1.forward_with_skip(a, silu=True)
         h = self.conv1.forward_act(h, want_stats=_stats_fusion())  # norm2's statistics from conv1's epilogue
         h = self.norm2(h, silu=True)
         skip = self.nin_shortcut.forward_act(a_skip) if self.in_channels != self.out_channels else a_skip
         out = self.conv2.forward_act(h, residual=skip, want_stats=_stats_fusion())  # x + h fused in the epilogue
         return _exit(out, ext, self)
+
+
+def enable_recompute(module: nn.Module, enabled: bool = True) -> nn.Module:
+    """Makes every ResnetBlock under `module` (encoder, decoder, the HR decoder's extra level) recompute its inner
+    activations in the backward (enabled=False restores the default); returns `module`.
+
+    With the flag set, a grad-enabled forward of a block keeps only its input (plus two [N, 32, 2] GroupNorm records)
+    for the backward instead of also hn = swish(norm1(x)), h = conv1(hn) and h2 = swish(norm2(h)), and rebuilds those
+    three there bit for bit: less activation memory for one extra conv1 and two GroupNorm apply passes per block in the
+    backward. The forward, and the gradients, are those of the default path. No-grad forwards are unchanged."""
+    for m in module.modules():
+        if isinstance(m, ResnetBlock):
+            m._vqb_recompute = bool(enabled)
+    return module
 
 
 class Downsample(nn.Module):

@@ -577,24 +577,14 @@ class ConvFn(torch.autograd.Function):
         Cout, Cin, KH, KW = weight.shape
         assert Cp == plans.cpad(Cin), f"conv input has {Cp} channels, weight expects {Cin}"
         x = x.contiguous()
-        if kind == "fat3":  # x is the zero-framed [N, H+2, W+2, 8] image
+        if kind == "fat3":
             assert Cp == 8 and KH == 3
-            H, W = H - 2, W - 2
-            g = cache.geom(("fat", N, H, W), lambda: plans.geom_fat3(N, H, W))
-        elif kind == "s1":
-            g = cache.geom(("f", N, H, W), lambda: plans.geom_s1(N, H, W, Cp, KH))
-        elif kind == "s2":
-            g = cache.geom(("f", N, H, W), lambda: plans.geom_s2(N, H, W, Cp))
-        elif kind == "patch":
-            g = cache.geom(("f", N, H, W), lambda: plans.geom_patch(N, H, W, Cp, KH))
-        else:
-            raise ValueError(kind)
+        g, H, W = _conv_geom(cache, kind, N, H, W, Cp, KH)
         if kind == "fat3":
             wp = _fat_weights(cache, weight, ("fwd", kind), g.tapmap, False, Cp)
         else:
             wp = cache.get(weight, ("fwd", kind), g.tapmap, False, Cp)
         Cop = plans.cpad(Cout)
-        ctx.HW = (H, W)
         b = None
         if bias is not None:
             b = bias.detach()
@@ -614,7 +604,7 @@ class ConvFn(torch.autograd.Function):
                 stats = torch.zeros(N, Cout, 2, device=x.device, dtype=torch.float32)
             run_conv_gemm(g, x, wp, Cout, out, ostr, bias=b, res=res, relu=relu, stats=stats)
         ctx.save_for_backward(x, weight)
-        ctx.cache, ctx.kind, ctx.g = cache, kind, g
+        ctx.cache, ctx.kind = cache, kind
         ctx.has_bias, ctx.has_res = bias is not None, residual is not None
         ctx.input_is_relu, ctx.nchw_out = input_is_relu, nchw_out
         if want_stats and not nchw_out:
@@ -628,83 +618,106 @@ class ConvFn(torch.autograd.Function):
     def backward(ctx, gout, _gstats=None):
         x, weight = ctx.saved_tensors
         inference_only(weight)
-        g, kind, cache = ctx.g, ctx.kind, ctx.cache
-        N, _, _, Cp = x.shape
-        H, W = ctx.HW
-        Cout, Cin, KH, KW = weight.shape
-        Cop = plans.cpad(Cout)
-        dy_framed = False
-        if ctx.nchw_out:
-            gn = gout.float().contiguous()
-            if Cop == 8 and KH == 3 and kind == "s1" and fat_conv_enabled():
-                # tiny-Cout conv (decoder conv_out): keep dy in a zero-framed buffer so that the data gradient runs as a
-                # 3-tap fat-pixel conv (24-wide K runs) instead of 9 taps of 8 channels
-                dy_framed = True
-                dy = alloc_framed(N, g.Ho, g.Wo, Cop, x.device)
-                check(_L().vqb_nchw_to_nhwc_pad(ptr(gn), ptr(dy), N, Cout, g.Ho, g.Wo, Cop, 1, 0, 0, stream_ptr()),
-                      "nchw_to_nhwc_pad")
-            else:
-                dy = torch.empty(N, g.Ho, g.Wo, Cop, device=x.device, dtype=torch.bfloat16)
-                check(_L().vqb_nchw_to_nhwc(ptr(gn), ptr(dy), N, Cout, g.Ho, g.Wo, Cop, 0, 0, stream_ptr()),
-                      "nchw_to_nhwc")
-        else:
-            dy = gout.contiguous()
-        gx = gw = gb = gres = None
-        if ctx.needs_input_grad[0]:
-            mask = x if ctx.input_is_relu else None
-            gx_alloc = torch.empty if Cp == Cin else torch.zeros
-            if kind == "fat3":  # gradient w.r.t. the framed image: write the interior of a zero-framed buffer
-                gx = torch.zeros(N, H + 2, W + 2, Cp, device=x.device, dtype=torch.bfloat16)
-                gd = cache.geom(("d", N, H, W), lambda: plans.geom_s1_dgrad(N, H, W, Cop, KH))
-                wpd = cache.get(weight, ("dgrad", "s1"), gd.tapmap, True, Cop)
-                run_conv_gemm(gd, dy, wpd, Cin, gx, ((H + 2) * (W + 2) * Cp, (W + 2) * Cp, Cp, 1),
-                              out_ptr_offset_bytes=((W + 2) + 1) * Cp * 2)
-            elif dy_framed:
-                gx = gx_alloc(N, H, W, Cp, device=x.device, dtype=torch.bfloat16)
-                gdf = cache.geom(("dfat", N, H, W), lambda: plans.geom_fat3(N, H, W, dgrad=True))
-                wpd = _fat_weights(cache, weight, ("dgrad", "fat3"), gdf.tapmap, True, Cop)
-                run_conv_gemm(gdf, dy, wpd, Cin, gx, plans.nhwc_strides(H, W, Cp), mask=mask)
-            else:
-                gx = gx_alloc(N, H, W, Cp, device=x.device, dtype=torch.bfloat16)
-            if kind == "fat3" or dy_framed:
-                pass
-            elif kind == "s1":
-                gd = cache.geom(("d", N, H, W), lambda: plans.geom_s1_dgrad(N, H, W, Cop, KH))
-                wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
-                run_conv_gemm(gd, dy, wpd, Cin, gx, plans.nhwc_strides(H, W, Cp), mask=mask)
-            elif kind == "s2":
-                for ph, pw, gd in cache.geom(("d", N, H, W), lambda: plans.geom_s2_dgrad_classes(N, H, W, Cop)):
-                    wpd = cache.get(weight, ("dgrad", kind, ph, pw), gd.tapmap, True, Cop)
-                    run_conv_gemm(gd, dy, wpd, Cin, gx, (H * W * Cp, 2 * W * Cp, 2 * Cp, 1),
-                                  out_ptr_offset_bytes=(ph * W + pw) * Cp * 2, mask=mask)
-            elif kind == "patch":
-                # non-overlapping windows: each input pixel belongs to exactly one (output pixel, tap): one 1-tap
-                # "conv" per tap writing the strided sub-grid of dx
-                k = KH
-                for kh in range(k):
-                    for kw in range(k):
-                        gd = cache.geom(("d", N, H, W, kh, kw), lambda: plans.ConvGeom(
-                            N, g.Ho, g.Wo, Cop, [native.dense_view(N, g.Ho, g.Wo, Cop)], [(0, 0, 0)], [kh * k + kw]))
-                        wpd = cache.get(weight, ("dgrad", kind, kh, kw), gd.tapmap, True, Cop)
-                        run_conv_gemm(gd, dy, wpd, Cin, gx, (H * W * Cp, k * W * Cp, k * Cp, 1),
-                                      out_ptr_offset_bytes=(kh * W + kw) * Cp * 2, mask=mask)
-        if ctx.needs_input_grad[1]:
-            if kind == "fat3":  # [Cout][kw*8 + c][kh] -> OIHW
-                g3 = run_wgrad(g, x, dy, (Cout, plans.FAT_K, 3, 1), Cop)  # [Cout][kw*8 + c (24 real of 64)][kh]
-                gw = g3[:, :24, :, 0].reshape(Cout, 3, 8, 3)[:, :, :Cin, :].permute(0, 2, 3, 1).contiguous()
-            elif dy_framed:
-                gw = run_wgrad(g, x, dy, weight.shape, Cop,
-                               dy_view=plans.framed_interior_view(N, g.Ho, g.Wo, Cop), out=grad_out(weight))
-            else:
-                gw = run_wgrad(g, x, dy, weight.shape, Cop, out=grad_out(weight))
-        if ctx.has_bias and ctx.needs_input_grad[2]:
-            rows = N * (g.Ho + 2) * (g.Wo + 2) if dy_framed else N * g.Ho * g.Wo  # the zero frame adds nothing
-            gb = None if dy_framed else _take_dx_colsum(dy, Cop)
-            if gb is None:
-                gb = colsum(rows, dy, Cop)[:Cout]
-        if ctx.has_res and ctx.needs_input_grad[3]:
-            gres = dy
+        gx, gw, gb, gres = conv_backward(x, weight, gout, ctx.cache, ctx.kind, ctx.has_bias, ctx.has_res,
+                                         ctx.input_is_relu, ctx.nchw_out, ctx.needs_input_grad[:4])
         return gx, gw, gb, gres, None, None, None, None, None, None
+
+
+def _conv_geom(cache, kind, N, H, W, Cp, KH):
+    """-> (forward geometry, H, W) of conv kind `kind` over an [N, H, W, Cp] input; for "fat3" the input is the
+    zero-framed [N, H+2, W+2, 8] image and H, W are those of the image inside the frame."""
+    if kind == "fat3":
+        H, W = H - 2, W - 2
+        return cache.geom(("fat", N, H, W), lambda: plans.geom_fat3(N, H, W)), H, W
+    if kind == "s1":
+        return cache.geom(("f", N, H, W), lambda: plans.geom_s1(N, H, W, Cp, KH)), H, W
+    if kind == "s2":
+        return cache.geom(("f", N, H, W), lambda: plans.geom_s2(N, H, W, Cp)), H, W
+    if kind == "patch":
+        return cache.geom(("f", N, H, W), lambda: plans.geom_patch(N, H, W, Cp, KH)), H, W
+    raise ValueError(kind)
+
+
+def conv_backward(x, weight, gout, cache, kind, has_bias, has_res, input_is_relu, nchw_out, needs):
+    """Backward of conv(x, weight, bias, cache, kind, residual, relu, input_is_relu, nchw_out) from its input x, its
+    weight and the incoming gradient -> (gx, gw, gb, gres); needs: which of (x, weight, bias, residual) want a
+    gradient."""
+    N, H, W, Cp = x.shape
+    Cout, Cin, KH, KW = weight.shape
+    g, H, W = _conv_geom(cache, kind, N, H, W, Cp, KH)
+    Cop = plans.cpad(Cout)
+    dy_framed = False
+    if nchw_out:
+        gn = gout.float().contiguous()
+        if Cop == 8 and KH == 3 and kind == "s1" and fat_conv_enabled():
+            # tiny-Cout conv (decoder conv_out): keep dy in a zero-framed buffer so that the data gradient runs as a
+            # 3-tap fat-pixel conv (24-wide K runs) instead of 9 taps of 8 channels
+            dy_framed = True
+            dy = alloc_framed(N, g.Ho, g.Wo, Cop, x.device)
+            check(_L().vqb_nchw_to_nhwc_pad(ptr(gn), ptr(dy), N, Cout, g.Ho, g.Wo, Cop, 1, 0, 0, stream_ptr()),
+                  "nchw_to_nhwc_pad")
+        else:
+            dy = torch.empty(N, g.Ho, g.Wo, Cop, device=x.device, dtype=torch.bfloat16)
+            check(_L().vqb_nchw_to_nhwc(ptr(gn), ptr(dy), N, Cout, g.Ho, g.Wo, Cop, 0, 0, stream_ptr()),
+                  "nchw_to_nhwc")
+    else:
+        dy = gout.contiguous()
+    gx = gw = gb = gres = None
+    if needs[0]:
+        mask = x if input_is_relu else None
+        gx_alloc = torch.empty if Cp == Cin else torch.zeros
+        if kind == "fat3":  # gradient w.r.t. the framed image: write the interior of a zero-framed buffer
+            gx = torch.zeros(N, H + 2, W + 2, Cp, device=x.device, dtype=torch.bfloat16)
+            gd = cache.geom(("d", N, H, W), lambda: plans.geom_s1_dgrad(N, H, W, Cop, KH))
+            wpd = cache.get(weight, ("dgrad", "s1"), gd.tapmap, True, Cop)
+            run_conv_gemm(gd, dy, wpd, Cin, gx, ((H + 2) * (W + 2) * Cp, (W + 2) * Cp, Cp, 1),
+                          out_ptr_offset_bytes=((W + 2) + 1) * Cp * 2)
+        elif dy_framed:
+            gx = gx_alloc(N, H, W, Cp, device=x.device, dtype=torch.bfloat16)
+            gdf = cache.geom(("dfat", N, H, W), lambda: plans.geom_fat3(N, H, W, dgrad=True))
+            wpd = _fat_weights(cache, weight, ("dgrad", "fat3"), gdf.tapmap, True, Cop)
+            run_conv_gemm(gdf, dy, wpd, Cin, gx, plans.nhwc_strides(H, W, Cp), mask=mask)
+        else:
+            gx = gx_alloc(N, H, W, Cp, device=x.device, dtype=torch.bfloat16)
+        if kind == "fat3" or dy_framed:
+            pass
+        elif kind == "s1":
+            gd = cache.geom(("d", N, H, W), lambda: plans.geom_s1_dgrad(N, H, W, Cop, KH))
+            wpd = cache.get(weight, ("dgrad", kind), gd.tapmap, True, Cop)
+            run_conv_gemm(gd, dy, wpd, Cin, gx, plans.nhwc_strides(H, W, Cp), mask=mask)
+        elif kind == "s2":
+            for ph, pw, gd in cache.geom(("d", N, H, W), lambda: plans.geom_s2_dgrad_classes(N, H, W, Cop)):
+                wpd = cache.get(weight, ("dgrad", kind, ph, pw), gd.tapmap, True, Cop)
+                run_conv_gemm(gd, dy, wpd, Cin, gx, (H * W * Cp, 2 * W * Cp, 2 * Cp, 1),
+                              out_ptr_offset_bytes=(ph * W + pw) * Cp * 2, mask=mask)
+        elif kind == "patch":
+            # non-overlapping windows: each input pixel belongs to exactly one (output pixel, tap): one 1-tap
+            # "conv" per tap writing the strided sub-grid of dx
+            k = KH
+            for kh in range(k):
+                for kw in range(k):
+                    gd = cache.geom(("d", N, H, W, kh, kw), lambda: plans.ConvGeom(
+                        N, g.Ho, g.Wo, Cop, [native.dense_view(N, g.Ho, g.Wo, Cop)], [(0, 0, 0)], [kh * k + kw]))
+                    wpd = cache.get(weight, ("dgrad", kind, kh, kw), gd.tapmap, True, Cop)
+                    run_conv_gemm(gd, dy, wpd, Cin, gx, (H * W * Cp, k * W * Cp, k * Cp, 1),
+                                  out_ptr_offset_bytes=(kh * W + kw) * Cp * 2, mask=mask)
+    if needs[1]:
+        if kind == "fat3":  # [Cout][kw*8 + c][kh] -> OIHW
+            g3 = run_wgrad(g, x, dy, (Cout, plans.FAT_K, 3, 1), Cop)  # [Cout][kw*8 + c (24 real of 64)][kh]
+            gw = g3[:, :24, :, 0].reshape(Cout, 3, 8, 3)[:, :, :Cin, :].permute(0, 2, 3, 1).contiguous()
+        elif dy_framed:
+            gw = run_wgrad(g, x, dy, weight.shape, Cop,
+                           dy_view=plans.framed_interior_view(N, g.Ho, g.Wo, Cop), out=grad_out(weight))
+        else:
+            gw = run_wgrad(g, x, dy, weight.shape, Cop, out=grad_out(weight))
+    if has_bias and needs[2]:
+        rows = N * (g.Ho + 2) * (g.Wo + 2) if dy_framed else N * g.Ho * g.Wo  # the zero frame adds nothing
+        gb = None if dy_framed else _take_dx_colsum(dy, Cop)
+        if gb is None:
+            gb = colsum(rows, dy, Cop)[:Cout]
+    if has_res and needs[3]:
+        gres = dy
+    return gx, gw, gb, gres
 
 
 def conv(x, weight, bias, cache, kind="s1", residual=None, relu=False, input_is_relu=False, nchw_out=False,
@@ -818,12 +831,7 @@ class GroupNormSiLUFn(torch.autograd.Function):
         require_cuda(x)
         x = x.contiguous()
         if chsums is not None:  # statistics were accumulated by the epilogue of the conv that produced x
-            N, H, W, C = x.shape
-            y = torch.empty_like(x)
-            mr = torch.empty(N, groups, 2, device=x.device, dtype=torch.float32)
-            ga, be = gamma.detach().float(), beta.detach().float()
-            check(_L().vqb_gn_silu_fwd_pre(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), ptr(chsums), N, H * W, C, groups,
-                                           eps, 1 if silu else 0, stream_ptr()), "gn_silu_fwd_pre")
+            y, mr = gn_silu_fwd_pre(x, gamma, beta, chsums, groups, eps, silu)
         else:
             y, mr = gn_silu_fwd(x, gamma, beta, groups, eps, silu)
         ctx.save_for_backward(x, gamma, beta, mr)
@@ -856,8 +864,21 @@ def gn_silu_fwd(x, gamma, beta, groups, eps, silu):
     return y, mr
 
 
+def gn_silu_fwd_pre(x, gamma, beta, chsums, groups, eps, silu):
+    """GroupNorm(+swish) of a contiguous bf16 NHWC x from the per-(n, channel) sums [N, C, 2] that the epilogue of the
+    conv producing x accumulated (VQB_EPI_STATS) -> (y, mr), as gn_silu_fwd."""
+    N, H, W, C = x.shape
+    y = torch.empty_like(x)
+    mr = torch.empty(N, groups, 2, device=x.device, dtype=torch.float32)
+    ga, be = gamma.detach().float(), beta.detach().float()
+    check(_L().vqb_gn_silu_fwd_pre(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), ptr(chsums), N, H * W, C, groups, eps,
+                                   1 if silu else 0, stream_ptr()), "gn_silu_fwd_pre")
+    return y, mr
+
+
 def gn_silu_apply(x, gamma, beta, mr, silu):
-    """The apply pass of gn_silu_fwd alone, with that call's mr: the same y, bit for bit (vqb_gn_silu_apply)."""
+    """The apply pass of gn_silu_fwd or gn_silu_fwd_pre alone, with that call's mr: the same y, bit for bit
+    (vqb_gn_silu_apply)."""
     N, H, W, C = x.shape
     y = torch.empty_like(x)
     ga, be = gamma.detach().float(), beta.detach().float()
@@ -885,6 +906,87 @@ def gn_silu_bwd(x, gy, gskip, gamma, beta, mr, groups, silu):
 
 def group_norm_silu(x, gamma, beta, groups=32, eps=1e-6, silu=True, with_skip=False, chsums=None):
     return GroupNormSiLUFn.apply(x, gamma, beta, groups, eps, silu, with_skip, chsums)
+
+
+class ResnetBlockRecomputeFn(torch.autograd.Function):
+    """ae.ResnetBlock as one autograd node that keeps only its input x, the two GroupNorm (mean, rstd) records and its
+    parameters for the backward, instead of x, hn = swish(norm1(x)), h = conv1(hn) and h2 = swish(norm2(h)).
+
+    The forward runs the kernels of the block's non-recomputing training forward: norm1 from the column sums chsums of
+    the conv that produced x when it accumulated them (else the statistics pass), conv1 with the statistics epilogue
+    where the shape allows it and norm2 from its sums, nin_shortcut, conv2 with the residual and the statistics of its
+    output, which it returns as a second, non-differentiable output (an empty tensor when the epilogue cannot produce
+    them). The backward rebuilds hn, h and h2 bit for bit: the GroupNorm apply pass with the saved mr, and conv1, whose
+    stored values do not depend on the statistics epilogue. conv2 is not recomputed; its backward needs only h2, its
+    weight and the incoming gradient. Then it runs the backward of conv2, nin_shortcut, norm2, conv1 and norm1 (with
+    the skip gradient summed in) in the order autograd runs them without recompute, so every gradient, bias column sum
+    and grad_out slot is the same.
+    spec: (groups1, eps1, groups2, eps2, conv1 cache, conv2 cache, nin_shortcut cache or None)."""
+
+    @staticmethod
+    def forward(ctx, x, chsums, spec, n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb):
+        require_cuda(x)
+        g1, e1, g2, e2, k1, k2, ks = spec
+        x = x.contiguous()
+        if chsums is not None:
+            hn, mr1 = gn_silu_fwd_pre(x, n1w, n1b, chsums, g1, e1, True)
+        else:
+            hn, mr1 = gn_silu_fwd(x, n1w, n1b, g1, e1, True)
+        h, st = conv(hn, c1w, c1b, k1, "s1", want_stats=True)
+        del hn
+        if st is not None:
+            h2, mr2 = gn_silu_fwd_pre(h, n2w, n2b, st, g2, e2, True)
+        else:
+            h2, mr2 = gn_silu_fwd(h, n2w, n2b, g2, e2, True)
+        del h
+        skip = conv(x, sw, sb, ks, "s1") if sw is not None else x
+        out, stats = conv(h2, c2w, c2b, k2, "s1", residual=skip, want_stats=True)
+        # the parameters go through save_for_backward so that an in-place change before the backward raises
+        ctx.save_for_backward(x, mr1, mr2, n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb)
+        ctx.spec = spec
+        if stats is None:
+            stats = torch.empty(0, device=x.device)  # "not available" marker, as ConvFn's
+        ctx.mark_non_differentiable(stats)
+        return out, stats
+
+    @staticmethod
+    def backward(ctx, gout, _gstats=None):
+        x, mr1, mr2, n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb = ctx.saved_tensors
+        inference_only(n1w, n1b, c1w, c1b, n2w, n2b, c2w, c2b, sw, sb)
+        g1, _, g2, _, k1, k2, ks = ctx.spec
+        nig = ctx.needs_input_grad
+        hn = gn_silu_apply(x, n1w, n1b, mr1, True)
+        h = conv(hn, c1w, c1b, k1, "s1")
+        h2 = gn_silu_apply(h, n2w, n2b, mr2, True)
+        # which intermediate gradients the non-recomputing graph would form
+        need_hn = nig[0] or nig[3] or nig[4]  # also the skip output of norm1
+        need_h = need_hn or nig[5] or nig[6]
+        need_h2 = need_h or nig[7] or nig[8]
+        need_res = need_hn or (sw is not None and (nig[11] or nig[12]))
+        gx = gn1w = gn1b = gc1w = gc1b = gn2w = gn2b = gsw = gsb = None
+        gh2, gc2w, gc2b, gskip = conv_backward(h2, c2w, gout, k2, "s1", c2b is not None, True, False, False,
+                                               (need_h2, nig[9], nig[10], need_res))
+        del h2
+        if sw is not None and need_res:
+            gskip, gsw, gsb, _ = conv_backward(x, sw, gskip, ks, "s1", sb is not None, False, False, False,
+                                               (need_hn, nig[11], nig[12], False))
+        if need_h2:
+            gh, gn2w, gn2b = gn_silu_bwd(h, gh2, None, n2w, n2b, mr2, g2, True)
+            del h, gh2
+            if need_h:
+                ghn, gc1w, gc1b, _ = conv_backward(hn, c1w, gh, k1, "s1", c1b is not None, False, False, False,
+                                                   (need_hn, nig[5], nig[6], False))
+                del hn, gh
+                if need_hn:
+                    gx, gn1w, gn1b = gn_silu_bwd(x, ghn, gskip, n1w, n1b, mr1, g1, True)
+        grads = (gn1w, gn1b, gc1w, gc1b, gn2w, gn2b, gc2w, gc2b, gsw, gsb)
+        return (gx, None, None) + tuple(g if nig[i + 3] else None for i, g in enumerate(grads))
+
+
+def resnet_block_recompute(x, chsums, spec, *params):
+    """-> (out, stats of out or None); see ResnetBlockRecomputeFn."""
+    out, st = ResnetBlockRecomputeFn.apply(x, chsums, spec, *params)
+    return out, (st if st.numel() > 0 else None)
 
 
 class MaxPool2Fn(torch.autograd.Function):

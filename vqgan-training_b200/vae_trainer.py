@@ -34,7 +34,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 import torch.optim as optim
 
-from ae import VAE
+from ae import VAE, enable_recompute
 from utils import LPIPS, PatchDiscriminator, prepare_filter
 
 try:  # optional: only needed for real datasets
@@ -388,7 +388,10 @@ class Trainer:
                  use_wavelet=False, do_ganloss=False, learning_rate_vae=1e-5, learning_rate_disc=2e-4, max_steps=1000,
                  do_clamp=False, clamp_th=8.0, crop_invariance=False, flip_invariance=False,
                  augment_before_perceptual_loss=False, downscale_factor=16, use_lecam=False, disc_type="bce",
-                 lpips_eval=True, seed=42, use_vq=False, vq_codebook_size=8192, vq_beta=0.25, cuda_graph=None):
+                 lpips_eval=True, seed=42, use_vq=False, vq_codebook_size=8192, vq_beta=0.25, cuda_graph=None,
+                 recompute=False):
+        """recompute=True: ae.enable_recompute on the VAE, so that every ResnetBlock keeps only its input for the
+        backward (larger batches or resolutions per GPU for one extra conv1 and two GroupNorm apply passes per block)."""
         self.device = device
         # CUDA-graph the whole step (forward, backward, NCCL collectives, optimizers, weight re-pack): ~600-1100 launches
         # per step otherwise keep the host within ~10 % of being the limiter. Auto-enabled (None) when no host-side
@@ -419,6 +422,8 @@ class Trainer:
                   ch_mult=[int(x) for x in str(vae_ch_mult).split(",")], num_res_blocks=vae_num_res_blocks,
                   z_channels=vae_z_channels, use_attn=do_attn, decoder_also_perform_hr=decoder_also_perform_hr,
                   use_wavelet=use_wavelet).to(device)
+        if recompute:
+            enable_recompute(vae)
         self.use_vq = use_vq
         if use_vq:  # BASELINE.json config 4: the codebook replaces vae.module.reg (vae_trainer.py:563)
             from ae import VectorQuantizer
