@@ -306,12 +306,13 @@ int vqb_wgrad3d_gemm(const VqbWgrad3dDesc* d, const void* dy, const void* x, flo
 /*
  * Attention core of tae.AttnBlock (tae.py:26-51: 8 heads of C/8 channels, F.scaled_dot_product_attention with its
  * default scale 1/sqrt(head_dim)): qkv [N][T][3C] bf16 (q | k | v channel blocks, head h owns channels
- * h*head_dim .. of each block) -> out [N][T][C] bf16; lse [N][C/head_dim][T] fp32. head_dim is 32 or 64; any other
- * value is refused with a message naming it. vqb_attn_fwd is this with head_dim = 64.
+ * h*head_dim .. of each block) -> out [N][T][C] bf16; lse [N][C/head_dim][T] fp32. head_dim is a multiple of 8 from 8
+ * to 112; any other value is refused with a message naming it. vqb_attn_fwd is this with head_dim = 64.
  */
 int vqb_attn_fwd_hd(const void* qkv, void* out, float* lse, int N, int T, int C, int head_dim, void* stream);
 /* Its backward (autograd of F.scaled_dot_product_attention at tae.py:31-50): dqkv [N][T][3C] bf16 from qkv, out, dout
- * and lse of the forward; dvec is a workspace of lse's shape. head_dim 32 or 64; vqb_attn_bwd is this with 64. */
+ * and lse of the forward; dvec is a workspace of lse's shape. head_dim as in the forward; vqb_attn_bwd is this with
+ * 64. */
 int vqb_attn_bwd_hd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec, void* dqkv,
                     int N, int T, int C, int head_dim, void* stream);
 

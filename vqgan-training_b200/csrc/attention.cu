@@ -1,4 +1,4 @@
-// Multi-head self-attention core of AttnBlock (ae.py:74-93): softmax(q k^T / sqrt(64)) v per head of 64 channels,
+// Multi-head self-attention core of AttnBlock (ae.py:74-93, heads of 64) and tae.AttnBlock (heads of 8 to 112 channels),
 // flash-attention style (online softmax, no T x T matrix in HBM), warp-level tensor-core MMA
 // (mma.sync.m16n8k16 bf16 -> fp32). The 1x1 qkv / proj_out convolutions and the GroupNorm around it run on the
 // wgmma conv / GN kernels; this file is only the [T x T] part: T = (H/8)(W/8) = 1024 tokens at 256^2, 8 heads at
@@ -9,6 +9,8 @@
 //
 // Backward: D = rowsum(dO * O); one kernel owns key tiles and produces dK, dV; one owns query tiles and produces dQ.
 // Both recompute P from q, k and the saved log-sum-exp.
+#include <cmath>
+
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -17,6 +19,20 @@ namespace vqb {
 constexpr int kTQ = 64;   // rows per block (4 warps x 16)
 constexpr int kLD = 72;   // smem row pitch in bf16 (144 B: conflict-free 32-bit fragment loads)
 
+// A head of HD channels (a multiple of 8, at most 112) is padded to kHP = the next multiple of 16 for the k-steps of
+// Q.K^T; the padding columns of the [64][kHP] tiles are zero-filled in shared memory, never read from global memory.
+// Tiles up to 64 channels keep the 72-element pitch; wider ones take kHP + 8 (conflict-free 32-bit fragment loads for
+// every multiple of 16). Transposed tiles ([d][64 tokens], pitch kLD) get HD rows, at least 64.
+template <int HD>
+struct HeadShape {
+    static_assert(HD % 8 == 0 && HD >= 8 && HD <= 112, "heads of 8 to 112 channels in steps of 8");
+    static constexpr int kHP = (HD + 15) / 16 * 16;
+    static constexpr int kL = kHP <= 64 ? kLD : kHP + 8;
+    static constexpr int kRT = HD > 64 ? HD : 64;
+    static constexpr int kKS = kHP / 16, kNO = HD / 8;
+    static constexpr bool kSplitKV = kHP > 64;  // dK and dV in separate CTAs (attn_bwd_dkdv_kernel)
+};
+
 __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile(
         "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -24,16 +40,21 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], 
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// 64 x COLS bf16 tile: rows row0.. of a [T][ld] matrix (column offset already applied to src) -> dst[64][kLD]; rows >= T
-// zero.
-template <int COLS = 64>
+// 64 x COLS bf16 tile: rows row0.. of a [T][ld] matrix (column offset already applied to src) -> dst[64][LD]; rows >= T
+// zero. PCOLS > COLS: columns COLS..PCOLS-1 (one 16-byte vector) are zero-filled.
+template <int COLS = 64, int LD = kLD, int PCOLS = COLS>
 __device__ __forceinline__ void load_tile(__nv_bfloat16* dst, const __nv_bfloat16* src, int64_t ld, int row0, int T) {
     constexpr int kV = COLS / 8;  // 16-byte vectors per row
     for (int i = threadIdx.x; i < 64 * kV; i += blockDim.x) {
         const int r = i / kV, v = i % kV;
         uint4 u = make_uint4(0, 0, 0, 0);
         if (row0 + r < T) u = __ldg(reinterpret_cast<const uint4*>(src + static_cast<int64_t>(row0 + r) * ld + v * 8));
-        *reinterpret_cast<uint4*>(dst + r * kLD + v * 8) = u;
+        *reinterpret_cast<uint4*>(dst + r * LD + v * 8) = u;
+    }
+    if constexpr (PCOLS > COLS) {
+        static_assert(PCOLS == COLS + 8, "one padding vector per row");
+        for (int r = threadIdx.x; r < 64; r += blockDim.x)
+            *reinterpret_cast<uint4*>(dst + r * LD + COLS) = make_uint4(0, 0, 0, 0);
     }
 }
 // same tile stored transposed: dst[col][row]
@@ -49,20 +70,20 @@ __device__ __forceinline__ void load_tile_t(__nv_bfloat16* dst, const __nv_bfloa
         for (int j = 0; j < 8; ++j) dst[(v * 8 + j) * kLD + r] = e[j];
     }
 }
-// A fragments (16 rows of this warp x 16*KS cols) of a [64][kLD] smem tile
-template <int KS = 4>
+// A fragments (16 rows of this warp x 16*KS cols) of a [64][LD] smem tile
+template <int KS = 4, int LD = kLD>
 __device__ __forceinline__ void load_a_frags(const __nv_bfloat16* s, int warp, int lane, uint32_t (&a)[KS][4]) {
     const int r = warp * 16 + (lane >> 2), c = (lane & 3) * 2;
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
-        a[ks][0] = *reinterpret_cast<const uint32_t*>(s + r * kLD + ks * 16 + c);
-        a[ks][1] = *reinterpret_cast<const uint32_t*>(s + (r + 8) * kLD + ks * 16 + c);
-        a[ks][2] = *reinterpret_cast<const uint32_t*>(s + r * kLD + ks * 16 + c + 8);
-        a[ks][3] = *reinterpret_cast<const uint32_t*>(s + (r + 8) * kLD + ks * 16 + c + 8);
+        a[ks][0] = *reinterpret_cast<const uint32_t*>(s + r * LD + ks * 16 + c);
+        a[ks][1] = *reinterpret_cast<const uint32_t*>(s + (r + 8) * LD + ks * 16 + c);
+        a[ks][2] = *reinterpret_cast<const uint32_t*>(s + r * LD + ks * 16 + c + 8);
+        a[ks][3] = *reinterpret_cast<const uint32_t*>(s + (r + 8) * LD + ks * 16 + c + 8);
     }
 }
-// acc[nt] += A(16 x 16*KS) * B where B[k][n] = s[n][k] (s is a [8*NT n][kLD] smem tile, k contiguous)
-template <int KS = 4, int NT = 8>
+// acc[nt] += A(16 x 16*KS) * B where B[k][n] = s[n][k] (s is a [8*NT n][LD] smem tile, k contiguous)
+template <int KS = 4, int NT = 8, int LD = kLD>
 __device__ __forceinline__ void mma_a_bT(float (&acc)[NT][4], const uint32_t (&a)[KS][4], const __nv_bfloat16* s,
                                          int lane) {
     const int n = lane >> 2, c = (lane & 3) * 2;
@@ -70,8 +91,8 @@ __device__ __forceinline__ void mma_a_bT(float (&acc)[NT][4], const uint32_t (&a
     for (int ks = 0; ks < KS; ++ks)
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt) {
-            const uint32_t b0 = *reinterpret_cast<const uint32_t*>(s + (nt * 8 + n) * kLD + ks * 16 + c);
-            const uint32_t b1 = *reinterpret_cast<const uint32_t*>(s + (nt * 8 + n) * kLD + ks * 16 + c + 8);
+            const uint32_t b0 = *reinterpret_cast<const uint32_t*>(s + (nt * 8 + n) * LD + ks * 16 + c);
+            const uint32_t b1 = *reinterpret_cast<const uint32_t*>(s + (nt * 8 + n) * LD + ks * 16 + c + 8);
             mma16816(acc[nt], a[ks], b0, b1);
         }
 }
@@ -87,24 +108,26 @@ __device__ __forceinline__ void acc_to_a(const float (&p)[8][4], uint32_t (&a)[4
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-// HD: head dim (64: ae.AttnBlock and tae heads of 64; 32: tae.AttnBlock at ch = 64). Q.K^T runs HD/16 k-steps over
-// 8 key n-tiles; P.V runs 4 key k-steps over HD/8 output n-tiles.
+// HD: head dim (64: ae.AttnBlock; tae.AttnBlock heads of C/8, any multiple of 8 up to 112). Q.K^T runs kHP/16 k-steps
+// over 8 key n-tiles; P.V runs 4 key k-steps over HD/8 output n-tiles. Shared memory is static: 46,848 B at HD = 112.
+// min-blocks 1 for heads of 72: without it ptxas caps the registers at 128 and spills
 template <int HD>
-__global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __restrict__ qkv,
+__global__ void __launch_bounds__(128, HD == 72 ? 1 : 0) attn_fwd_kernel(const __nv_bfloat16* __restrict__ qkv,
                                                        __nv_bfloat16* __restrict__ out, float* __restrict__ lse, int T,
                                                        int C, float scale) {
-    constexpr int kKS = HD / 16, kNO = HD / 8;
-    __shared__ __align__(16) __nv_bfloat16 sQ[64 * kLD];
-    __shared__ __align__(16) __nv_bfloat16 sK[64 * kLD];
-    __shared__ __align__(16) __nv_bfloat16 sVt[64 * kLD];
+    using S = HeadShape<HD>;
+    constexpr int kHP = S::kHP, kL = S::kL, kKS = S::kKS, kNO = S::kNO;
+    __shared__ __align__(16) __nv_bfloat16 sQ[64 * kL];
+    __shared__ __align__(16) __nv_bfloat16 sK[64 * kL];
+    __shared__ __align__(16) __nv_bfloat16 sVt[S::kRT * kLD];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * kTQ, h = blockIdx.y, n = blockIdx.z, heads = gridDim.y;
     const int64_t ld = 3 * static_cast<int64_t>(C);
     const __nv_bfloat16* base = qkv + static_cast<int64_t>(n) * T * ld;
-    load_tile<HD>(sQ, base + h * HD, ld, q0, T);
+    load_tile<HD, kL, kHP>(sQ, base + h * HD, ld, q0, T);
     __syncthreads();
     uint32_t qa[kKS][4];
-    load_a_frags<kKS>(sQ, warp, lane, qa);
+    load_a_frags<kKS, kL>(sQ, warp, lane, qa);
     float m_i[2] = {-INFINITY, -INFINITY}, l_i[2] = {0.f, 0.f};
     float o[kNO][4];
 #pragma unroll
@@ -114,7 +137,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __re
     const int nkt = (T + 63) / 64;
     for (int kt = 0; kt < nkt; ++kt) {
         __syncthreads();
-        load_tile<HD>(sK, base + C + h * HD, ld, kt * 64, T);
+        load_tile<HD, kL, kHP>(sK, base + C + h * HD, ld, kt * 64, T);
         load_tile_t<HD>(sVt, base + 2 * C + h * HD, ld, kt * 64, T);
         __syncthreads();
         float s[8][4];
@@ -122,7 +145,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __re
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-        mma_a_bT<kKS, 8>(s, qa, sK, lane);
+        mma_a_bT<kKS, 8, kL>(s, qa, sK, lane);
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt)
@@ -181,7 +204,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const __nv_bfloat16* __re
     }
 }
 
-// D[n][h][q] = sum_d dO * O   (HD: head dim, 64 or 32; lane l holds channels 2l, 2l + 1 of the head)
+// D[n][h][q] = sum_d dO * O   (HD: head dim; lane l holds channels 2l, 2l + 1 of the head, and 64 + 2l, 65 + 2l above
+// 64)
 template <int HD>
 __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ dout,
                                      float* __restrict__ dvec, int T, int C, int heads, int64_t total) {
@@ -192,10 +216,17 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const 
     const int64_t nq = i / heads;
     const int64_t off = nq * C + h * HD + lane * 2;
     float s = 0.f;
-    if (HD == 64 || lane * 2 < HD) {
+    if (HD >= 64 || lane * 2 < HD) {
         const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(o + off));
         const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + off));
         s = a.x * b.x + a.y * b.y;
+    }
+    if constexpr (HD > 64) {
+        if (64 + lane * 2 < HD) {
+            const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(o + off + 64));
+            const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + off + 64));
+            s += a.x * b.x + a.y * b.y;
+        }
     }
 #pragma unroll
     for (int k = 16; k > 0; k >>= 1) s += __shfl_xor_sync(0xffffffffu, s, k);
@@ -206,34 +237,34 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const 
 }
 
 // ------------------------------------------------------------------------------------------------ backward: dK, dV
-// HD as in the forward: K.Q^T and V.dO^T run HD/16 k-steps over 8 query n-tiles; dV and dK run 4 query k-steps over HD/8
-// n-tiles.
-template <int HD>
-__global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ qkv,
-                                                            const __nv_bfloat16* __restrict__ dout,
-                                                            const float* __restrict__ lse,
-                                                            const float* __restrict__ dvec,
-                                                            __nv_bfloat16* __restrict__ dqkv, int T, int C, float scale) {
+// HD as in the forward: K.Q^T and V.dO^T run kHP/16 k-steps over 8 query n-tiles; dV and dK run 4 query k-steps over
+// HD/8 n-tiles. kDK / kDV: which of dK, dV this CTA produces (both for heads up to 64 channels).
+template <int HD, bool kDK, bool kDV>
+__device__ __forceinline__ void attn_bwd_kv_tile(const __nv_bfloat16* __restrict__ qkv,
+                                                 const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
+                                                 const float* __restrict__ dvec, __nv_bfloat16* __restrict__ dqkv,
+                                                 int T, int C, float scale, int h, int heads) {
+    using S = HeadShape<HD>;
+    constexpr int kHP = S::kHP, kL = S::kL, kKS = S::kKS, kNO = S::kNO;
     extern __shared__ __align__(16) uint8_t smem_dyn[];
     __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_dyn);
-    __nv_bfloat16* sQt = sQ + 64 * kLD;
-    __nv_bfloat16* sdO = sQt + 64 * kLD;
-    __nv_bfloat16* sdOt = sdO + 64 * kLD;
-    float* sLse = reinterpret_cast<float*>(sdOt + 64 * kLD);
+    __nv_bfloat16* sQt = sQ + 64 * kL;
+    __nv_bfloat16* sdO = sQt + S::kRT * kLD;
+    __nv_bfloat16* sdOt = sdO + 64 * kL;
+    float* sLse = reinterpret_cast<float*>(sdOt + S::kRT * kLD);
     float* sD = sLse + 64;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int k0 = blockIdx.x * 64, h = blockIdx.y, n = blockIdx.z, heads = gridDim.y;
+    const int k0 = blockIdx.x * 64, n = blockIdx.z;
     const int64_t ld = 3 * static_cast<int64_t>(C);
     const __nv_bfloat16* base = qkv + static_cast<int64_t>(n) * T * ld;
-    constexpr int kKS = HD / 16, kNO = HD / 8;
     const __nv_bfloat16* dob = dout + static_cast<int64_t>(n) * T * C + h * HD;
     // K and V rows of this warp as A fragments (staged through sQ / sdO once)
-    load_tile<HD>(sQ, base + C + h * HD, ld, k0, T);
-    load_tile<HD>(sdO, base + 2 * C + h * HD, ld, k0, T);
+    load_tile<HD, kL, kHP>(sQ, base + C + h * HD, ld, k0, T);
+    if constexpr (kDK) load_tile<HD, kL, kHP>(sdO, base + 2 * C + h * HD, ld, k0, T);
     __syncthreads();
     uint32_t ka[kKS][4], va[kKS][4];
-    load_a_frags<kKS>(sQ, warp, lane, ka);
-    load_a_frags<kKS>(sdO, warp, lane, va);
+    load_a_frags<kKS, kL>(sQ, warp, lane, ka);
+    if constexpr (kDK) load_a_frags<kKS, kL>(sdO, warp, lane, va);
     float dk[kNO][4], dv[kNO][4];
 #pragma unroll
     for (int i = 0; i < kNO; ++i)
@@ -243,14 +274,14 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
     const int nqt = (T + 63) / 64;
     for (int qt = 0; qt < nqt; ++qt) {
         __syncthreads();
-        load_tile<HD>(sQ, base + h * HD, ld, qt * 64, T);
-        load_tile_t<HD>(sQt, base + h * HD, ld, qt * 64, T);
-        load_tile<HD>(sdO, dob, C, qt * 64, T);
-        load_tile_t<HD>(sdOt, dob, C, qt * 64, T);
+        load_tile<HD, kL, kHP>(sQ, base + h * HD, ld, qt * 64, T);
+        if constexpr (kDK) load_tile_t<HD>(sQt, base + h * HD, ld, qt * 64, T);
+        if constexpr (kDK) load_tile<HD, kL, kHP>(sdO, dob, C, qt * 64, T);
+        if constexpr (kDV) load_tile_t<HD>(sdOt, dob, C, qt * 64, T);
         if (threadIdx.x < 64) {
             const int q = qt * 64 + threadIdx.x;
             sLse[threadIdx.x] = q < T ? lse[(static_cast<int64_t>(n) * heads + h) * T + q] : 0.f;
-            sD[threadIdx.x] = q < T ? dvec[(static_cast<int64_t>(n) * heads + h) * T + q] : 0.f;
+            if constexpr (kDK) sD[threadIdx.x] = q < T ? dvec[(static_cast<int64_t>(n) * heads + h) * T + q] : 0.f;
         }
         __syncthreads();
         float st[8][4], dp[8][4];
@@ -258,8 +289,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) st[i][j] = dp[i][j] = 0.f;
-        mma_a_bT<kKS, 8>(st, ka, sQ, lane);   // S^T[key][q] = sum_d K[key][d] Q[q][d]
-        mma_a_bT<kKS, 8>(dp, va, sdO, lane);  // dP^T[key][q] = sum_d V[key][d] dO[q][d]
+        mma_a_bT<kKS, 8, kL>(st, ka, sQ, lane);                     // S^T[key][q] = sum_d K[key][d] Q[q][d]
+        if constexpr (kDK) mma_a_bT<kKS, 8, kL>(dp, va, sdO, lane);  // dP^T[key][q] = sum_d V[key][d] dO[q][d]
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -269,13 +300,13 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
                 const bool ok = (qt * 64 + ql < T) && (key < T);
                 const float pt = ok ? __expf(st[nt][j] * scale - sLse[ql]) : 0.f;
                 st[nt][j] = pt;
-                dp[nt][j] = pt * (dp[nt][j] - sD[ql]) * scale;
+                if constexpr (kDK) dp[nt][j] = pt * (dp[nt][j] - sD[ql]) * scale;
             }
         uint32_t pa[4][4], dsa[4][4];
-        acc_to_a(st, pa);
-        acc_to_a(dp, dsa);
-        mma_a_bT<4, kNO>(dv, pa, sdOt, lane);  // dV[key][d] += sum_q P^T[key][q] dO[q][d]
-        mma_a_bT<4, kNO>(dk, dsa, sQt, lane);  // dK[key][d] += sum_q dS^T[key][q] Q[q][d]
+        if constexpr (kDV) acc_to_a(st, pa);
+        if constexpr (kDK) acc_to_a(dp, dsa);
+        if constexpr (kDV) mma_a_bT<4, kNO>(dv, pa, sdOt, lane);  // dV[key][d] += sum_q P^T[key][q] dO[q][d]
+        if constexpr (kDK) mma_a_bT<4, kNO>(dk, dsa, sQt, lane);  // dK[key][d] += sum_q dS^T[key][q] Q[q][d]
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -285,10 +316,33 @@ __global__ void __launch_bounds__(128) attn_bwd_dkdv_kernel(const __nv_bfloat16*
             __nv_bfloat16* vp = kp + C;
 #pragma unroll
             for (int nt = 0; nt < kNO; ++nt) {
-                *reinterpret_cast<uint32_t*>(kp + nt * 8) = pack_bf16x2(dk[nt][2 * r], dk[nt][2 * r + 1]);
-                *reinterpret_cast<uint32_t*>(vp + nt * 8) = pack_bf16x2(dv[nt][2 * r], dv[nt][2 * r + 1]);
+                if constexpr (kDK)
+                    *reinterpret_cast<uint32_t*>(kp + nt * 8) = pack_bf16x2(dk[nt][2 * r], dk[nt][2 * r + 1]);
+                if constexpr (kDV)
+                    *reinterpret_cast<uint32_t*>(vp + nt * 8) = pack_bf16x2(dv[nt][2 * r], dv[nt][2 * r + 1]);
             }
         }
+    }
+}
+
+// Heads up to 64 channels: one CTA per (key tile, head) produces dK and dV. Wider heads would hold K and V A fragments
+// plus both accumulators (~260 registers at 112) and spill, so the work is split: blockIdx.y = 2 h + 1 produces dK,
+// 2 h produces dV and recomputes S on its own (one more K.Q^T per tile, no dP, half the live accumulators).
+// min-blocks 1 for heads of 56, which otherwise spill at a 168-register cap.
+template <int HD>
+__global__ void __launch_bounds__(128, HD == 56 ? 1 : 0) attn_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ qkv,
+                                                            const __nv_bfloat16* __restrict__ dout,
+                                                            const float* __restrict__ lse,
+                                                            const float* __restrict__ dvec,
+                                                            __nv_bfloat16* __restrict__ dqkv, int T, int C, float scale) {
+    if constexpr (!HeadShape<HD>::kSplitKV) {
+        attn_bwd_kv_tile<HD, true, true>(qkv, dout, lse, dvec, dqkv, T, C, scale, blockIdx.y, gridDim.y);
+    } else {
+        const int h = blockIdx.y >> 1, heads = gridDim.y >> 1;
+        if (blockIdx.y & 1)
+            attn_bwd_kv_tile<HD, true, false>(qkv, dout, lse, dvec, dqkv, T, C, scale, h, heads);
+        else
+            attn_bwd_kv_tile<HD, false, true>(qkv, dout, lse, dvec, dqkv, T, C, scale, h, heads);
     }
 }
 
@@ -299,21 +353,22 @@ __global__ void __launch_bounds__(128, HD == 32 ? 1 : 0) attn_bwd_dq_kernel(cons
                                                           const __nv_bfloat16* __restrict__ dout,
                                                           const float* __restrict__ lse, const float* __restrict__ dvec,
                                                           __nv_bfloat16* __restrict__ dqkv, int T, int C, float scale) {
-    __shared__ __align__(16) __nv_bfloat16 sK[64 * kLD];
-    __shared__ __align__(16) __nv_bfloat16 sKt[64 * kLD];
-    __shared__ __align__(16) __nv_bfloat16 sV[64 * kLD];
+    using S = HeadShape<HD>;
+    constexpr int kHP = S::kHP, kL = S::kL, kKS = S::kKS, kNO = S::kNO;
+    __shared__ __align__(16) __nv_bfloat16 sK[64 * kL];
+    __shared__ __align__(16) __nv_bfloat16 sKt[S::kRT * kLD];
+    __shared__ __align__(16) __nv_bfloat16 sV[64 * kL];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * 64, h = blockIdx.y, n = blockIdx.z, heads = gridDim.y;
     const int64_t ld = 3 * static_cast<int64_t>(C);
     const __nv_bfloat16* base = qkv + static_cast<int64_t>(n) * T * ld;
-    constexpr int kKS = HD / 16, kNO = HD / 8;
     const __nv_bfloat16* dob = dout + static_cast<int64_t>(n) * T * C + h * HD;
-    load_tile<HD>(sK, base + h * HD, ld, q0, T);
-    load_tile<HD>(sV, dob, C, q0, T);
+    load_tile<HD, kL, kHP>(sK, base + h * HD, ld, q0, T);
+    load_tile<HD, kL, kHP>(sV, dob, C, q0, T);
     __syncthreads();
     uint32_t qa[kKS][4], doa[kKS][4];
-    load_a_frags<kKS>(sK, warp, lane, qa);
-    load_a_frags<kKS>(sV, warp, lane, doa);
+    load_a_frags<kKS, kL>(sK, warp, lane, qa);
+    load_a_frags<kKS, kL>(sV, warp, lane, doa);
     const int qr0 = q0 + warp * 16 + (lane >> 2);
     float lse_r[2], d_r[2];
 #pragma unroll
@@ -330,17 +385,17 @@ __global__ void __launch_bounds__(128, HD == 32 ? 1 : 0) attn_bwd_dq_kernel(cons
     const int nkt = (T + 63) / 64;
     for (int kt = 0; kt < nkt; ++kt) {
         __syncthreads();
-        load_tile<HD>(sK, base + C + h * HD, ld, kt * 64, T);
+        load_tile<HD, kL, kHP>(sK, base + C + h * HD, ld, kt * 64, T);
         load_tile_t<HD>(sKt, base + C + h * HD, ld, kt * 64, T);
-        load_tile<HD>(sV, base + 2 * C + h * HD, ld, kt * 64, T);
+        load_tile<HD, kL, kHP>(sV, base + 2 * C + h * HD, ld, kt * 64, T);
         __syncthreads();
         float s[8][4], dp[8][4];
 #pragma unroll
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-        mma_a_bT<kKS, 8>(s, qa, sK, lane);    // S[q][key]
-        mma_a_bT<kKS, 8>(dp, doa, sV, lane);  // dP[q][key] = sum_d dO[q][d] V[key][d]
+        mma_a_bT<kKS, 8, kL>(s, qa, sK, lane);    // S[q][key]
+        mma_a_bT<kKS, 8, kL>(dp, doa, sV, lane);  // dP[q][key] = sum_d dO[q][d] V[key][d]
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -368,23 +423,33 @@ __global__ void __launch_bounds__(128, HD == 32 ? 1 : 0) attn_bwd_dq_kernel(cons
 }
 
 template <int HD>
+static void launch_attn_fwd(const void* qkv, void* out, float* lse, int N, int T, int C, float scale, cudaStream_t st) {
+    dim3 grid((T + 63) / 64, C / HD, N);
+    attn_fwd_kernel<HD><<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv), static_cast<__nv_bfloat16*>(out),
+                                              lse, T, C, scale);
+}
+
+template <int HD>
 static int launch_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec,
                            void* dqkv, int N, int T, int C, float scale, cudaStream_t st) {
+    using S = HeadShape<HD>;
     const int heads = C / HD;
     const int64_t total = static_cast<int64_t>(N) * T * heads;
     attn_bwd_prep_kernel<HD><<<static_cast<int>((total + 7) / 8), 256, 0, st>>>(
         static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), dvec, T, C, heads, total);
     dim3 grid((T + 63) / 64, heads, N);
-    const size_t smem = 4 * 64 * kLD * sizeof(__nv_bfloat16) + 2 * 64 * sizeof(float);
+    dim3 grid_kv((T + 63) / 64, S::kSplitKV ? 2 * heads : heads, N);
+    // sQ, sdO [64][kL]; sQt, sdOt [kRT][kLD]; lse, D: 63,488 B at HD = 112
+    const size_t smem = (2 * 64 * S::kL + 2 * S::kRT * kLD) * sizeof(__nv_bfloat16) + 2 * 64 * sizeof(float);
     static bool attr = false;
     if (!attr) {
         VQB_CUDA(cudaFuncSetAttribute(attn_bwd_dkdv_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      64 * 1024));
+                                      static_cast<int>(smem)));
         attr = true;
     }
-    attn_bwd_dkdv_kernel<HD><<<grid, 128, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv),
-                                                       static_cast<const __nv_bfloat16*>(dout), lse, dvec,
-                                                       static_cast<__nv_bfloat16*>(dqkv), T, C, scale);
+    attn_bwd_dkdv_kernel<HD><<<grid_kv, 128, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv),
+                                                          static_cast<const __nv_bfloat16*>(dout), lse, dvec,
+                                                          static_cast<__nv_bfloat16*>(dqkv), T, C, scale);
     attn_bwd_dq_kernel<HD><<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv),
                                                  static_cast<const __nv_bfloat16*>(dout), lse, dvec,
                                                  static_cast<__nv_bfloat16*>(dqkv), T, C, scale);
@@ -392,6 +457,15 @@ static int launch_attn_bwd(const void* qkv, const void* out, const void* dout, c
     count_launch(3);
     return VQB_OK;
 }
+
+// The head dimensions of vqb_attn_fwd_hd / vqb_attn_bwd_hd: multiples of 8 from 8 to 112 (tae.AttnBlock's C/8 for C a
+// multiple of 64 up to 896).
+#define VQB_ATTN_HEAD_DIMS(X) X(8) X(16) X(24) X(32) X(40) X(48) X(56) X(64) X(72) X(80) X(88) X(96) X(104) X(112)
+
+static bool attn_head_dim_ok(int hd) { return hd >= 8 && hd <= 112 && hd % 8 == 0; }
+
+// SDPA's default scale 1/sqrt(head_dim), rounded once to fp32 (0.125f at 64, 0.17677669529663687f at 32)
+static float attn_scale(int hd) { return static_cast<float>(1.0 / std::sqrt(static_cast<double>(hd))); }
 
 }  // namespace vqb
 
@@ -412,27 +486,26 @@ int vqb_attn_fwd(const void* qkv, void* out, float* lse, int N, int T, int C, vo
     return VQB_OK;
 }
 
-// tae.AttnBlock (tae.py:26-51): heads of head_dim = C/8 channels, SDPA's default scale 1/sqrt(head_dim). Replaces
-// F.scaled_dot_product_attention + the einops rearranges at tae.py:31-50.
+// tae.AttnBlock (tae.py:26-51): heads of head_dim = C/8 channels (a multiple of 8 from 8 to 112), SDPA's default scale
+// 1/sqrt(head_dim). Replaces F.scaled_dot_product_attention + the einops rearranges at tae.py:31-50.
 int vqb_attn_fwd_hd(const void* qkv, void* out, float* lse, int N, int T, int C, int head_dim, void* stream) {
     VQB_CHECK(qkv && out && lse, "vqb_attn_fwd_hd: null pointer");
-    VQB_CHECK(head_dim == 32 || head_dim == 64,
-              "vqb_attn_fwd_hd: head_dim=%d is not supported (heads of 32 or 64 channels only)", head_dim);
+    VQB_CHECK(attn_head_dim_ok(head_dim),
+              "vqb_attn_fwd_hd: head_dim=%d is not supported (heads of 8 to 112 channels in steps of 8 only)",
+              head_dim);
     VQB_CHECK(C > 0 && C % head_dim == 0 && T > 0 && N > 0,
               "vqb_attn_fwd_hd: C=%d must be a positive multiple of head_dim %d (T=%d N=%d)", C, head_dim, T, N);
     VQB_CHECK(((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out)) & 15u) == 0 &&
                   (reinterpret_cast<uintptr_t>(lse) & 3u) == 0,
               "vqb_attn_fwd_hd: qkv / out must be 16-byte aligned");
     if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_attn_fwd_hd: current device is not sm_90");
-    dim3 grid((T + 63) / 64, C / head_dim, N);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (head_dim == 64)
-        attn_fwd_kernel<64><<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv),
-                                                   static_cast<__nv_bfloat16*>(out), lse, T, C, 0.125f);
-    else
-        attn_fwd_kernel<32><<<grid, 128, 0, st>>>(static_cast<const __nv_bfloat16*>(qkv),
-                                                   static_cast<__nv_bfloat16*>(out), lse, T, C,
-                                                   0.17677669529663687f);  // 1/sqrt(32)
+    switch (head_dim) {
+#define VQB_ATTN_FWD_CASE(D) \
+    case D: launch_attn_fwd<D>(qkv, out, lse, N, T, C, attn_scale(D), st); break;
+        VQB_ATTN_HEAD_DIMS(VQB_ATTN_FWD_CASE)
+#undef VQB_ATTN_FWD_CASE
+    }
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
@@ -451,8 +524,9 @@ int vqb_attn_bwd(const void* qkv, const void* out, const void* dout, const float
 int vqb_attn_bwd_hd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec, void* dqkv,
                     int N, int T, int C, int head_dim, void* stream) {
     VQB_CHECK(qkv && out && dout && lse && dvec && dqkv, "vqb_attn_bwd_hd: null pointer");
-    VQB_CHECK(head_dim == 32 || head_dim == 64,
-              "vqb_attn_bwd_hd: head_dim=%d is not supported (heads of 32 or 64 channels only)", head_dim);
+    VQB_CHECK(attn_head_dim_ok(head_dim),
+              "vqb_attn_bwd_hd: head_dim=%d is not supported (heads of 8 to 112 channels in steps of 8 only)",
+              head_dim);
     VQB_CHECK(C > 0 && C % head_dim == 0 && T > 0 && N > 0,
               "vqb_attn_bwd_hd: C=%d must be a positive multiple of head_dim %d (T=%d N=%d)", C, head_dim, T, N);
     VQB_CHECK(((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out) |
@@ -461,8 +535,13 @@ int vqb_attn_bwd_hd(const void* qkv, const void* out, const void* dout, const fl
               "vqb_attn_bwd_hd: qkv / out / dout / dqkv must be 16-byte aligned");
     if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_attn_bwd_hd: current device is not sm_90");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (head_dim == 64) return launch_attn_bwd<64>(qkv, out, dout, lse, dvec, dqkv, N, T, C, 0.125f, st);
-    return launch_attn_bwd<32>(qkv, out, dout, lse, dvec, dqkv, N, T, C, 0.17677669529663687f, st);  // 1/sqrt(32)
+    switch (head_dim) {
+#define VQB_ATTN_BWD_CASE(D) \
+    case D: return launch_attn_bwd<D>(qkv, out, dout, lse, dvec, dqkv, N, T, C, attn_scale(D), st);
+        VQB_ATTN_HEAD_DIMS(VQB_ATTN_BWD_CASE)
+#undef VQB_ATTN_BWD_CASE
+    }
+    return VQB_OK;  // unreachable: head_dim was checked above
 }
 
 }  // extern "C"

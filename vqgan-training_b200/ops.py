@@ -1171,17 +1171,21 @@ def group_norm_silu3d(x, gamma, beta, groups=32, eps=1e-6, silu=True):
     return y.view(N, T, H, W, C)
 
 
+# head dimensions of the native attention forward and backward (vqb_attn_fwd_hd / vqb_attn_bwd_hd)
+ATTN_HEAD_DIMS = tuple(range(8, 113, 8))
+
+
 def attention_hd(qkv, heads, head_dim):
     """qkv [N, T, H, W, 3C] bf16 (q | k | v channel blocks) -> softmax(q k^T / sqrt(head_dim)) v as [N, T, H, W, C]
-    (tae.py:26-51). head_dim 32 or 64."""
+    (tae.py:26-51). head_dim a multiple of 8 from 8 to 112 (ATTN_HEAD_DIMS)."""
     return _attention_hd_fwd(qkv, heads, head_dim)[0]
 
 
 def _attention_hd_fwd(qkv, heads, head_dim):
     """-> (out, lse) of attention_hd; lse [N, heads, T*H*W] is what the backward needs."""
-    if head_dim not in (32, 64):
+    if head_dim not in ATTN_HEAD_DIMS:
         raise NotImplementedError(f"vqgan-training_b200: attention heads of {head_dim} channels are not supported "
-                                  "(heads of 32 or 64 channels only)")
+                                  "(heads of 8 to 112 channels in steps of 8 only)")
     qkv = qkv.contiguous()
     N, T, H, W, C3 = qkv.shape
     C = C3 // 3
@@ -1455,7 +1459,7 @@ def upsample_conv3d_train(x, weight, bias, cache):
 
 
 class AttentionHdFn(torch.autograd.Function):
-    """Autograd form of attention_hd; the backward is vqb_attn_bwd_hd (heads of 32 or 64)."""
+    """Autograd form of attention_hd; the backward is vqb_attn_bwd_hd (the same head dimensions)."""
 
     @staticmethod
     def forward(ctx, qkv, heads, head_dim):

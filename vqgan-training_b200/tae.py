@@ -11,7 +11,8 @@ einops. Every forward runs hand-written sm_90a kernels (libvqb200.so):
                                                                               low-resolution input (8/27 of the MACs)
   1x1x1 convs (nin_shortcut, qkv, proj_out)                               -> vqb_conv_gemm on the [N][T*H][W][C] view
   GroupNorm(+swish)                                                        -> the GroupNorm kernels over T*H*W voxels
-  AttnBlock core (8 heads of C/8 channels)                                 -> flash-style kernel, heads of 32 or 64
+  AttnBlock core (8 heads of C/8 channels)                                 -> flash-style kernel, heads of 8 to 112
+                                                                              channels in steps of 8
   DiagonalGaussian                                                         -> torch.randn_like(mean) + one fused kernel
 
 Internally activations are bf16 NTHWC (`Act3`); modules accept an `Act3` or an NCTHW tensor and return NCTHW in the
@@ -25,7 +26,8 @@ require grad) raises before anything is launched: a grad-enabled forward of a fu
 activations alive. `tae.enable_training(vae, recompute=True)` bounds that memory: each ResnetBlock then keeps only its
 input for the backward (ops.ResnetBlock3dRecomputeFn) and rebuilds hn, h and h2 there bit for bit, so the gradients
 are those of the plain path. Modules with bf16 parameters stay inference-only. Deviations from the reference (DESIGN.md
-section 7): training is opt-in; T, H and W divisible by 2^(len(ch_mult)-1) at the encoder; heads of 32 or 64 channels.
+section 7): training is opt-in; T, H and W divisible by 2^(len(ch_mult)-1) at the encoder; heads of 8 to 112
+channels in steps of 8 (C a multiple of 64 up to 896).
 
 Reference citations: tae.py:9-10 swish, :13-54 AttnBlock, :57-90 ResnetBlock, :93-104 Downsample, :107-117 Upsample,
 :120-184 Encoder, :187-250 Decoder, :253-266 DiagonalGaussian, :269-297 TVAE.
@@ -213,10 +215,10 @@ class AttnBlock(nn.Module):
         nn.init.normal_(self.proj_out.weight, std=0.2 / math.sqrt(in_channels))
 
     def _check_heads(self):
-        if self.head_dim not in (32, 64) or self.head_dim * self.num_heads != self.in_channels:
+        if self.head_dim not in ops.ATTN_HEAD_DIMS or self.head_dim * self.num_heads != self.in_channels:
             raise NotImplementedError(
                 f"tae.AttnBlock({self.in_channels}): heads of {self.in_channels / self.num_heads:g} channels are not "
-                "supported (heads of 32 or 64 channels only: in_channels 256 or 512)")
+                "supported (heads of 8 to 112 channels in steps of 8 only: in_channels a multiple of 64 up to 896)")
 
     def attention(self, h_) -> Act3:
         self._check_heads()
