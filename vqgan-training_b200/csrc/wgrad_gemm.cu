@@ -3,7 +3,12 @@
 //   dWp[co][t*C64 + c] = sum_{n,h,w} dy[n,h,w,co] * X_view(t)[n, h+dh_t, w+dw_t, c]
 //
 // GEMM view: M = Cout (tiles of 128, two consumer warpgroups of 64 rows), N = ntaps*C64 flattened (tap, channel)
-// columns in tiles of BLOCK_N (a whole number of 64-channel atoms), K = output pixels walked in boxes of 64 pixels.
+// columns in wgmma blocks of BLOCK_N = 128 or 64 (a whole number of 64-channel atoms), K = output pixels walked in
+// boxes of 64 pixels. A CTA tile is NB column blocks wide: two 128-column blocks when the columns divide by 256 (the
+// tile may then span two taps), else one. Both operands stream from L2, so the tile width sets the bytes moved per
+// FLOP: 16 KB dy + 16 KB x per K block at 128 columns, 16 KB + 32 KB for twice the work at 256 (a quarter less). Two
+// blocks are 128 accumulator registers per consumer thread: the warpgroups re-split the register file at the role
+// split (setmaxnreg: producer 40, consumers 232).
 // Both operands are "MN-major": dy[pixel][co] and x[pixel][c] have the GEMM M/N index contiguous and K (the pixel)
 // strided, which wgmma consumes directly (transposed operands) from 128B-swizzled [64 px][64 ch] atoms (no transposes,
 // no im2col buffer). The tap shift is a coordinate offset of the TMA box and conv padding is TMA zero fill. K is split
@@ -24,6 +29,12 @@ constexpr int kWThreads = 384;  // warpgroup 0: TMA producer; warpgroups 1, 2: 6
 constexpr int kWMaxStages = 8;
 constexpr int kWPix = 64;                     // pixels per K block
 constexpr uint32_t kAtomBytes = kWPix * 128;  // [64 px][64 ch] bf16
+constexpr int kWProducerRegs = 40, kWConsumerRegs = 232;
+
+// wgmma column block and blocks per CTA tile for `cols` (tap, channel) columns; ops._wgrad_block_n and
+// ops._wgrad_tile_blocks mirror them to size split-K.
+static int wgrad_block_n(int cols) { return cols % 128 == 0 ? 128 : 64; }
+static int wgrad_tile_blocks(int cols) { return cols % 256 == 0 ? 2 : 1; }
 
 struct alignas(64) WgradParams {
     static constexpr int kRank = 4;  // NHWC, 4-D TMA boxes [64 ch][bw][bh][bn]
@@ -59,10 +70,10 @@ struct alignas(64) Wgrad3dParams {
     float* partial;
 };
 
-template <int BN, class P>
+template <int BN, int NB, class P>
 __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_constant__ P p) {
     extern __shared__ uint8_t smem_raw[];
-    constexpr int kAtoms = BN / 64;
+    constexpr int kAtoms = NB * BN / 64;
     constexpr uint32_t kABytes = 2 * kAtomBytes;
     constexpr uint32_t kStageBytes = kABytes + kAtoms * kAtomBytes;
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -96,13 +107,14 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
 
     if (wg == 0) {
         // ===================== TMA producer (one elected thread) =====================
+        setmaxnreg_dec<kWProducerRegs>();
         if (warp == 0 && elect_one()) {
             uint32_t stage = 0, phase = 0;
             for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x) {
                 int m_tile, n_tile, s, kb0, kb1;
                 unit_range(unit, m_tile, n_tile, s, kb0, kb1);
                 const int co0 = m_tile * kWM;
-                const int colbase = n_tile * BN;
+                const int colbase = n_tile * (NB * BN);
                 // CTAs working on the same pixel split stream the same x / dy boxes in lock-step, so each box is
                 // fetched from HBM once and hit in L2 by the other tiles
                 for (int kb = kb0; kb < kb1; ++kb) {
@@ -155,11 +167,14 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
     }
 
     // ===================== consumers: warpgroup cw owns Cout rows 64*cw .. 64*cw + 63 of every tile =====================
+    setmaxnreg_inc<kWConsumerRegs>();
     const uint32_t cw = wg - 1;
     const uint32_t ring = smem_u32(base);
-    float acc[BN / 2];
+    float acc[NB][BN / 2];  // acc[nb]: columns BN*nb .. BN*nb + BN - 1 of the tile
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[nb][i] = 0.f;
     uint32_t stage = 0, phase = 0;
     for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x) {
         int m_tile, n_tile, s, kb0, kb1;
@@ -171,13 +186,18 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
             // MN-major, 128B swizzle: SBO = 8 K-rows (1024 B), LBO = next 64-wide MN atom
             const uint64_t da = make_smem_desc(a + cw * kAtomBytes, kAtomBytes, 1024);
             const uint64_t db = make_smem_desc(a + kABytes, kAtomBytes, 1024);
-            fence_operands(acc);
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) fence_operands(acc[nb]);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kWPix / 16; ++k)  // 16 pixel rows of 128 B per K = 16 step
-                wgmma_bf16<BN, 1, 1>(acc, da + 128 * k, db + 128 * k, (kb > kb0 || k > 0) ? 1u : 0u);
+            for (int nb = 0; nb < NB; ++nb)  // the block's first atom (descriptor addresses count 16 B)
+#pragma unroll
+                for (int k = 0; k < kWPix / 16; ++k)  // 16 pixel rows of 128 B per K = 16 step
+                    wgmma_bf16<BN, 1, 1>(acc[nb], da + 128 * k, db + nb * (BN / 64) * (kAtomBytes >> 4) + 128 * k,
+                                         (kb > kb0 || k > 0) ? 1u : 0u);
             wgmma_commit();
-            fence_operands(acc);
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) fence_operands(acc[nb]);
             // keep this K-block's group in flight while the next stage is awaited; the previous one has retired
             wgmma_wait<1>();
             if (kb > kb0 && lane == 0) mbar_arrive(&empty[prev]);
@@ -188,7 +208,8 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
             }
         }
         wgmma_wait<0>();
-        fence_operands(acc);  // the epilogue's reads of acc stay below the wait
+#pragma unroll
+        for (int nb = 0; nb < NB; ++nb) fence_operands(acc[nb]);  // the epilogue's reads of acc stay below the wait
         if (kb1 > kb0 && lane == 0) mbar_arrive(&empty[prev]);
         // ---------------- epilogue: fp32 partial tile -> global
         const bool empty_range = (kb1 <= kb0);  // more splits than pixel boxes: contributes zeros
@@ -196,29 +217,39 @@ __global__ void __launch_bounds__(kWThreads, 1) wgrad_gemm_kernel(const __grid_c
         for (int i = 0; i < 2; ++i) {
             const int co = m_tile * kWM + static_cast<int>(cw * 64 + warp * 16 + (lane >> 2)) + 8 * i;
             if (co >= p.Cout) continue;
-            float* orow = p.partial + (static_cast<int64_t>(s) * p.Cout + co) * p.ld + n_tile * BN + 2 * (lane & 3u);
+            float* orow = p.partial + (static_cast<int64_t>(s) * p.Cout + co) * p.ld + n_tile * (NB * BN) +
+                          2 * (lane & 3u);
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const float2 f = empty_range ? make_float2(0.f, 0.f)
-                                             : make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-                *reinterpret_cast<float2*>(orow + 8 * j) = f;
+            for (int nb = 0; nb < NB; ++nb) {
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const float2 f = empty_range ? make_float2(0.f, 0.f)
+                                                 : make_float2(acc[nb][4 * j + 2 * i], acc[nb][4 * j + 2 * i + 1]);
+                    *reinterpret_cast<float2*>(orow + nb * BN + 8 * j) = f;
+                }
             }
         }
     }
 }
 
-template <int BN, class P>
+template <int BN, int NB, class P>
 static int launch_wgrad(const P& p, void* stream) {
-    const size_t smem = 1024 + static_cast<size_t>(p.stages) * (2 + BN / 64) * kAtomBytes + 16 * p.stages;
+    const size_t smem = 1024 + static_cast<size_t>(p.stages) * (2 + NB * BN / 64) * kAtomBytes + 16 * p.stages;
     static bool attr_set = false;
     if (!attr_set) {
-        VQB_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VQB_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN, NB, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set = true;
     }
     const int grid = p.total_units < num_sms() ? p.total_units : num_sms();
-    wgrad_gemm_kernel<BN, P><<<grid, kWThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
+    wgrad_gemm_kernel<BN, NB, P><<<grid, kWThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
     VQB_CUDA(cudaGetLastError());
     return VQB_OK;
+}
+
+template <class P>
+static int launch_wgrad_form(int block_n, int tile_n, const P& p, void* stream) {
+    if (tile_n == 256) return launch_wgrad<128, 2>(p, stream);
+    return block_n == 128 ? launch_wgrad<128, 1>(p, stream) : launch_wgrad<64, 1>(p, stream);
 }
 
 static int encode_view(const VqbView& vw, const void* basep, int C, int lbw, int lbh, int lbn, CUtensorMap* m) {
@@ -267,15 +298,15 @@ extern "C" int vqb_wgrad_gemm(const VqbWgradDesc* d, const void* dy, const void*
     p.C64 = ((d->C + 63) / 64) * 64;
     p.Cout = d->Cout;
     const int cols = vqb_wgrad_cols(d->ntaps, d->C);
-    const int block_n = (cols % 128 == 0) ? 128 : 64;  // 64 fp32 accumulator registers per thread at most
+    const int block_n = wgrad_block_n(cols), tile_n = block_n * wgrad_tile_blocks(cols);
     const int m_tiles = (d->Cout + kWM - 1) / kWM;
-    p.n_tiles = cols / block_n;
+    p.n_tiles = cols / tile_n;
     p.ksplit = d->ksplit;
     p.total_units = m_tiles * p.n_tiles * p.ksplit;
     // ld_override / col_offset: several launches may fill column ranges of one partial buffer (folded upsample conv)
     p.ld = d->ld_override > 0 ? d->ld_override : cols;
     p.partial = partial + d->col_offset;
-    const int stage_bytes = (2 + block_n / 64) * static_cast<int>(kAtomBytes);
+    const int stage_bytes = (2 + tile_n / 64) * static_cast<int>(kAtomBytes);
     int stages = (200 * 1024) / stage_bytes;
     if (stages > kWMaxStages) stages = kWMaxStages;
     p.stages = stages;
@@ -291,7 +322,7 @@ extern "C" int vqb_wgrad_gemm(const VqbWgradDesc* d, const void* dy, const void*
         rc = encode_view(d->views[v], x, d->C, p.lbw, p.lbh, p.lbn, &p.xmap[v]);
         if (rc != VQB_OK) return rc;
     }
-    rc = block_n == 128 ? launch_wgrad<128>(p, stream) : launch_wgrad<64>(p, stream);
+    rc = launch_wgrad_form(block_n, tile_n, p, stream);
     if (rc != VQB_OK) return rc;
     count_launch();
     return VQB_OK;
@@ -362,16 +393,16 @@ extern "C" int vqb_wgrad3d_gemm(const VqbWgrad3dDesc* d, const void* dy, const v
     p.C = d->C;
     p.C64 = ((d->C + 63) / 64) * 64;
     p.Cout = d->Cout;
-    const int block_n = (cols % 128 == 0) ? 128 : 64;
+    const int block_n = wgrad_block_n(cols), tile_n = block_n * wgrad_tile_blocks(cols);
     const int m_tiles = (d->Cout + kWM - 1) / kWM;
-    p.n_tiles = cols / block_n;
+    p.n_tiles = cols / tile_n;
     p.ksplit = d->ksplit;
     const int64_t units = static_cast<int64_t>(m_tiles) * p.n_tiles * p.ksplit;
     VQB_CHECK(units < (1ll << 31), "vqb_wgrad3d_gemm: too many work units");
     p.total_units = static_cast<int32_t>(units);
     p.ld = d->ld_override > 0 ? d->ld_override : cols;
     p.partial = partial + d->col_offset;
-    const int stage_bytes = (2 + block_n / 64) * static_cast<int>(kAtomBytes);
+    const int stage_bytes = (2 + tile_n / 64) * static_cast<int>(kAtomBytes);
     int stages = (200 * 1024) / stage_bytes;
     if (stages > kWMaxStages) stages = kWMaxStages;
     p.stages = stages;
@@ -387,7 +418,7 @@ extern "C" int vqb_wgrad3d_gemm(const VqbWgrad3dDesc* d, const void* dy, const v
         rc = encode_view3d(d->views[v], x, d->C, bw, bh, bt, bn, &p.xmap[v]);
         if (rc != VQB_OK) return rc;
     }
-    rc = block_n == 128 ? launch_wgrad<128>(p, stream) : launch_wgrad<64>(p, stream);
+    rc = launch_wgrad_form(block_n, tile_n, p, stream);
     if (rc != VQB_OK) return rc;
     count_launch();
     return VQB_OK;

@@ -299,17 +299,23 @@ def _num_sms() -> int:
 
 
 def _wgrad_block_n(cols: int) -> int:
+    """wgmma column block of csrc/wgrad_gemm.cu."""
     return 128 if cols % 128 == 0 else 64
+
+
+def _wgrad_tile_blocks(cols: int) -> int:
+    """Column blocks per CTA tile of csrc/wgrad_gemm.cu: two (256 columns) when the columns divide by 256."""
+    return 2 if cols % 256 == 0 else 1
 
 
 def choose_ksplit(g: plans.ConvGeom, Cout_pad: int) -> int:
     """Split-K factor of the weight-gradient GEMM: the split count whose (tile, split) unit count best fills whole waves
     of the persistent CTAs (one per SM of an H100 SXM), preferring one wave. Mirrors the tile shape rules of
-    csrc/wgrad_gemm.cu (128 Cout rows x 128 or 64 columns, 64-pixel K blocks; for a 3-D geometry, 64-voxel boxes)."""
+    csrc/wgrad_gemm.cu (128 Cout rows x one or two blocks of 128 or 64 columns, 64-pixel K blocks; for a 3-D geometry, 64-voxel boxes)."""
     cols = len(g.taps) * ((g.C + 63) // 64) * 64
     rows = 128
     kpix = 64
-    tiles = ((Cout_pad + rows - 1) // rows) * (cols // _wgrad_block_n(cols))
+    tiles = ((Cout_pad + rows - 1) // rows) * (cols // (_wgrad_block_n(cols) * _wgrad_tile_blocks(cols)))
 
     def p2(v, cap):
         p = 1
