@@ -6,10 +6,17 @@
 // K = ntaps * C walked in 64-channel chunks. Per K-chunk the TMA producer issues ONE 4-D tiled load of the activation
 // box shifted by the tap offset (out-of-range rows/cols/channels are zero-filled by the TMA unit -> conv padding costs
 // nothing) and ONE 2-D load of the packed weights; both land in 128B-swizzled K-major smem tiles of a multi-stage
-// mbarrier ring. Two consumer warpgroups each own 64 rows of the tile and issue wgmma (M = 64, N = BLOCK_N, K = 16 x4)
-// with fp32 accumulators in registers; their epilogue (bias / residual / ReLU / mask / GroupNorm statistics -> bf16
-// NHWC or strided fp32) runs while the producer already streams the next tile's operands. Persistent: one CTA per SM
-// walks tiles round-robin.
+// mbarrier ring. Persistent: one CTA per SM walks tiles round-robin, and its two consumer warpgroups take turns
+// ("ping-pong"): warpgroup c owns the CTA's tiles of local index = c (mod 2) whole, issuing two wgmma row blocks
+// (M = 64 each, N = BLOCK_N, K = 16 x4) per K-chunk into 2 x BLOCK_N / 2 fp32 accumulators per thread, so one
+// warpgroup's epilogue (bias / residual / ReLU / mask / GroupNorm statistics -> bf16 NHWC or strided fp32) runs while
+// the other warpgroup's MMAs run. 128 accumulators per thread at BLOCK_N = 128 need the register file re-split at the
+// role split (setmaxnreg: producer 40, consumers 232).
+//
+// Math order: a warpgroup starts the K loop of its tile only after the other warpgroup has passed the last `full`
+// wait of the previous tile (the `order` mbarriers). The ring's full barriers are waited by parity alone, so without
+// this a warpgroup two or more fills behind on a stage would take the other warpgroup's chunk for its own; with it,
+// every full barrier a consumer waits on has completed all earlier fills, for any K-chunk count and stage count.
 //
 // Replaces the cuDNN kernels behind nn.Conv2d at reference ae.py:105-117,143-154,160-167 and the
 // torchvision VGG convs reached from utils.py:95-111,150-154 (see include/vqb200.h).
@@ -26,6 +33,8 @@ constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB per stage
 constexpr int kThreads = 384;                   // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue
 constexpr int kMaxStages = 8;
 constexpr int kConsumerWarps = 8;
+constexpr int kProducerRegs = 40;   // setmaxnreg split: 40 * 128 + 232 * 256 <= 64 K registers
+constexpr int kConsumerRegs = 232;
 
 struct alignas(64) ConvParams {
     static constexpr int kRank = 4;  // NHWC activations, 4-D TMA boxes [64 ch][bw][bh][bn]
@@ -92,9 +101,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     // carve shared memory (1024-B aligned for the 128B swizzle atoms)
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t stages = p.stages;
-    float* sStat = reinterpret_cast<float*>(base + stages * kStageBytes);  // [8 consumer warps][BN][2]
+    float* sStat = reinterpret_cast<float*>(base + stages * kStageBytes);  // [2 warpgroups][4 warps][BN][2]
     uint64_t* full = reinterpret_cast<uint64_t*>(sStat + kConsumerWarps * BN * 2);
     uint64_t* empty = full + stages;
+    uint64_t* order = empty + stages;  // [warpgroup]: one phase per tile, completed at its last full wait
     const uint32_t wg = threadIdx.x >> 7;
     const uint32_t warp = (threadIdx.x >> 5) & 3u;  // warp inside its warpgroup
     const uint32_t lane = threadIdx.x & 31u;
@@ -108,15 +118,18 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         tma_prefetch_desc(&p.bmap);
         for (uint32_t i = 0; i < stages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], kConsumerWarps);  // lane 0 of every consumer warp releases the stage
+            mbar_init(&empty[i], 4);  // lane 0 of every warp of the consuming warpgroup releases the stage
         }
+        mbar_init(&order[0], 4);
+        mbar_init(&order[1], 4);
         fence_mbar_init();
     }
     __syncthreads();
 
     const int num_kb = p.ntaps * p.kchunks;
     if (wg == 0) {
-        // ===================== TMA producer (one elected thread) =====================
+        // ===================== TMA producer (one elected thread), tiles in order =====================
+        setmaxnreg_dec<kProducerRegs>();
         if (warp == 0 && elect_one()) {
             uint32_t stage = 0, phase = 0;
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -156,10 +169,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         return;
     }
 
-    // ===================== consumers: warpgroup cw owns rows 64*cw .. 64*cw + 63 of every tile =====================
+    // ===================== consumers: warpgroup cw owns the CTA's tiles 2i + cw, all 128 rows of each ==============
+    setmaxnreg_inc<kConsumerRegs>();
     const uint32_t cw = wg - 1;
     const uint32_t cwarp = cw * 4 + warp;  // 0..7
-    const uint32_t ctid = threadIdx.x - 128;  // 0..255
+    const uint32_t wtid = threadIdx.x & 127u;  // thread inside its warpgroup
     const uint32_t ring = smem_u32(base);
     const bool has_bias = p.flags & VQB_EPI_BIAS, has_res = p.flags & VQB_EPI_RES;
     const bool do_relu = !kR5 && (p.flags & VQB_EPI_RELU), has_mask = !kR5 && (p.flags & VQB_EPI_MASK);
@@ -167,24 +181,42 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const bool reduce = !kR5 && p.do_stats;
     const __nv_bfloat16* res = reinterpret_cast<const __nv_bfloat16*>(p.res);
     const __nv_bfloat16* mask = reinterpret_cast<const __nv_bfloat16*>(p.mask);
-    float acc[BN / 2];
+    float acc[2][BN / 2];  // acc[mb]: rows 64*mb .. 64*mb + 63 of the tile
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[mb][i] = 0.f;
     uint32_t stage = 0, phase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    for (int l = static_cast<int>(cw);; l += 2) {  // l: the CTA's local tile index
+        const int tile = blockIdx.x + l * gridDim.x;
+        if (tile >= p.total_tiles) break;
+        if (l > 0) {
+            // tile l - 1 is the other warpgroup's: skip its K-chunks in the ring, and start only once it has passed
+            // its last full wait (phase (l - 1) / 2 of its order barrier)
+            stage += num_kb;
+            phase ^= (stage / stages) & 1u;
+            stage %= stages;
+            mbar_wait(&order[cw ^ 1u], ((l - 1) >> 1) & 1);
+        }
         uint32_t prev = 0;
         for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(&full[stage], phase);
+            if (kb == num_kb - 1 && lane == 0) mbar_arrive(&order[cw]);
             const uint32_t a = ring + stage * kStageBytes;
-            const uint64_t da = make_smem_desc(a + cw * 8192u, 16, 1024);
+            const uint64_t da0 = make_smem_desc(a, 16, 1024);
+            const uint64_t da1 = make_smem_desc(a + 8192u, 16, 1024);  // rows 64..127: 64 rows x 128 B further
             const uint64_t db = make_smem_desc(a + kABytes, 16, 1024);
-            fence_operands(acc);
+            fence_operands(acc[0]);
+            fence_operands(acc[1]);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k)  // +32 B per K = 16 step inside the swizzle atom
-                wgmma_bf16<BN, 0, 0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+            for (int k = 0; k < kBlockK / 16; ++k) {  // +32 B per K = 16 step inside the swizzle atom
+                wgmma_bf16<BN, 0, 0>(acc[0], da0 + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+                wgmma_bf16<BN, 0, 0>(acc[1], da1 + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+            }
             wgmma_commit();
-            fence_operands(acc);
+            fence_operands(acc[0]);
+            fence_operands(acc[1]);
             // keep this K-chunk's group in flight while the next stage is awaited; the previous one has retired
             wgmma_wait<1>();
             if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
@@ -195,7 +227,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             }
         }
         wgmma_wait<0>();
-        fence_operands(acc);  // the epilogue's reads of acc stay below the wait
+        fence_operands(acc[0]);  // the epilogue's reads of acc stay below the wait
+        fence_operands(acc[1]);
         if (lane == 0) mbar_arrive(&empty[prev]);  // num_kb >= 1 (ntaps >= 1, C > 0)
 
         // ---------------- epilogue straight from the accumulator fragment
@@ -211,23 +244,24 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             tn = m_tile / (p.tiles_w * p.tiles_h);
         }
         const int col0 = n_tile * BN;
-        int64_t pix[2];
-        bool valid[2];
+        // row group r = 2 * mb + i: acc[mb][4j + 2i + e] is row 64 mb + 16 warp + lane / 4 + 8 i, column 8j + 2(lane % 4) + e
+        int64_t pix[4];
+        bool valid[4];
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const uint32_t row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;  // row of the 128-pixel box
+        for (int r = 0; r < 4; ++r) {
+            const uint32_t row = (r >> 1) * 64 + warp * 16 + (lane >> 2) + 8 * (r & 1);  // row of the 128-pixel box
             const int w = (tw << p.lbw) + static_cast<int>(row & ((1u << p.lbw) - 1));
             const int h = (th << p.lbh) + static_cast<int>((row >> p.lbw) & ((1u << p.lbh) - 1));
             if constexpr (kR5) {  // row = w + bw * (h + bh * (t + bt * n)) of the 128-voxel box
                 const int t = (tt << p.lbt) + static_cast<int>((row >> (p.lbw + p.lbh)) & ((1u << p.lbt) - 1));
                 const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh + p.lbt));
-                valid[i] = (w < p.W) && (h < p.H) && (t < p.T) && (n < p.N);
-                pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(t) * p.ot +
+                valid[r] = (w < p.W) && (h < p.H) && (t < p.T) && (n < p.N);
+                pix[r] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(t) * p.ot +
                          static_cast<int64_t>(h) * p.oh + static_cast<int64_t>(w) * p.ow;
             } else {
                 const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh));
-                valid[i] = (w < p.W) && (h < p.H) && (n < p.N);
-                pix[i] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh +
+                valid[r] = (w < p.W) && (h < p.H) && (n < p.N);
+                pix[r] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh +
                          static_cast<int64_t>(w) * p.ow;
             }
         }
@@ -241,28 +275,37 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                 b1 = ok1 ? __ldg(p.bias + col + 1) : 0.f;
             }
             float r1[2] = {0.f, 0.f}, r2[2] = {0.f, 0.f};  // per column: statistics partial sums over this thread's rows
+            if (vec_path && ok1) {
+                // all residual / mask loads of the column group in flight before the first use
+                __nv_bfloat162 rv[4], mv[4];
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                float f[2] = {acc[4 * j + 2 * i] + b0, acc[4 * j + 2 * i + 1] + b1};
-                if (!valid[i]) continue;
-                if (vec_path && ok1) {
-                    const int64_t o = pix[i] + col;  // 4-byte aligned: pixel strides % 8 == 0, col even
+                for (int r = 0; r < 4; ++r) {
+                    rv[r] = mv[r] = __floats2bfloat162_rn(0.f, 0.f);
+                    const int64_t o = pix[r] + col;  // 4-byte aligned: pixel strides % 8 == 0, col even
+                    if (has_res && valid[r]) rv[r] = *reinterpret_cast<const __nv_bfloat162*>(res + o);
+                    if (has_mask && valid[r]) mv[r] = *reinterpret_cast<const __nv_bfloat162*>(mask + o);
+                }
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    if (!valid[r]) continue;
+                    const int a0 = 4 * j + 2 * (r & 1);
+                    float f[2] = {acc[r >> 1][a0] + b0, acc[r >> 1][a0 + 1] + b1};
                     if (has_res) {
-                        const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(res + o));
-                        f[0] += r.x;
-                        f[1] += r.y;
+                        const float2 rf = __bfloat1622float2(rv[r]);
+                        f[0] += rf.x;
+                        f[1] += rf.y;
                     }
                     if (do_relu) {
                         f[0] = fmaxf(f[0], 0.f);
                         f[1] = fmaxf(f[1], 0.f);
                     }
                     if (has_mask) {
-                        const float2 m = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(mask + o));
+                        const float2 m = __bfloat1622float2(mv[r]);
                         if (!(m.x > 0.f)) f[0] = 0.f;
                         if (!(m.y > 0.f)) f[1] = 0.f;
                     }
                     const __nv_bfloat162 ob = __floats2bfloat162_rn(f[0], f[1]);
-                    *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.out) + o) = ob;
+                    *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix[r] + col) = ob;
                     if (reduce) {
                         const float2 v = __bfloat1622float2(ob);  // the bf16 values the consumer will read
                         r1[0] += v.x;
@@ -270,12 +313,18 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                         r1[1] += v.y;
                         r2[1] = fmaf(v.y, v.y, r2[1]);
                     }
-                } else {
-                    // generic strided / ragged path (small or odd Cout, NCHW fp32 outputs)
+                }
+            } else {
+                // generic strided / ragged path (small or odd Cout, NCHW fp32 outputs)
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    if (!valid[r]) continue;
+                    const int a0 = 4 * j + 2 * (r & 1);
+                    const float f[2] = {acc[r >> 1][a0] + b0, acc[r >> 1][a0 + 1] + b1};
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         if (!(e ? ok1 : ok0)) continue;
-                        const int64_t o = pix[i] + static_cast<int64_t>(col + e) * p.oc;
+                        const int64_t o = pix[r] + static_cast<int64_t>(col + e) * p.oc;
                         float x = f[e];
                         if (has_res) x += __bfloat162float(res[o]);
                         if (do_relu) x = fmaxf(x, 0.f);
@@ -304,16 +353,17 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         }
         if (reduce) {
             // the statistics need every row of the tile inside one image (checked on the host: vqb_conv_stats_ok)
-            named_bar_sync(1, 256);
+            named_bar_sync(1 + cw, 128);
             const int n_img = tn << p.lbn;
-            for (uint32_t idx = ctid; idx < BN * 2u; idx += 256u) {
+            const float* sw = sStat + cw * 4 * BN * 2;
+            for (uint32_t idx = wtid; idx < BN * 2u; idx += 128u) {
                 const int c = col0 + static_cast<int>(idx >> 1);
                 float v = 0.f;
 #pragma unroll
-                for (int w8 = 0; w8 < kConsumerWarps; ++w8) v += sStat[w8 * BN * 2 + idx];
+                for (int w4 = 0; w4 < 4; ++w4) v += sw[w4 * BN * 2 + idx];
                 if (c < p.Cout) atomicAdd(p.stats + (static_cast<int64_t>(n_img) * p.Cout + c) * 2 + (idx & 1u), v);
             }
-            named_bar_sync(1, 256);  // sStat is reused by the next tile
+            named_bar_sync(1 + cw, 128);  // this warpgroup's sStat half is reused by its next tile
         }
     }
 }
@@ -337,7 +387,9 @@ static int fill_views(const VqbView* views, int nviews, const void* a, int C, in
 template <int BN, class P>
 static int launch_conv(const P& p, void* stream) {
     constexpr size_t stage_bytes = kABytes + BN * kBlockK * 2;
-    const size_t smem = 1024 + p.stages * stage_bytes + kConsumerWarps * BN * 2 * sizeof(float) + 2 * 8 * p.stages;
+    // ring + statistics staging + full / empty barriers + the two order barriers
+    const size_t smem =
+        1024 + p.stages * stage_bytes + kConsumerWarps * BN * 2 * sizeof(float) + 2 * 8 * p.stages + 2 * 8;
     static bool attr_set = false;
     if (!attr_set) {
         VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -428,7 +480,7 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     p.do_stats = (d->flags & VQB_EPI_STATS) ? 1 : 0;
     if (query_only) return stats_ok ? 1 : 0;
     const int stage_bytes = kABytes + block_n * kBlockK * 2;
-    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages;
+    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages + 2 * 8;
     int stages = (227 * 1024 - fixed) / stage_bytes;
     if (stages > kMaxStages) stages = kMaxStages;
     p.stages = stages;
@@ -542,7 +594,7 @@ static int conv3d_impl(const char* fn, const D* d, const void* a, const void* w_
     VQB_CHECK(total < (1ll << 31), "%s: too many tiles", fn);
     p.total_tiles = static_cast<int32_t>(total);
     const int stage_bytes = kABytes + block_n * kBlockK * 2;
-    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages;
+    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages + 2 * 8;
     int stages = (227 * 1024 - fixed) / stage_bytes;
     if (stages > kMaxStages) stages = kMaxStages;
     p.stages = stages;
