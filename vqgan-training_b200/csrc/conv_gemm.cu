@@ -18,6 +18,20 @@
 // this a warpgroup two or more fills behind on a stage would take the other warpgroup's chunk for its own; with it,
 // every full barrier a consumer waits on has completed all earlier fills, for any K-chunk count and stage count.
 //
+// Staged epilogue (kStaged; NHWC bf16 outputs, Cout % 64 == 0, short K: the rule is in conv_gemm_impl): each consumer
+// warpgroup owns a 128 x BLOCK_N bf16 tile buffer after the ring, BLOCK_N / 64 slabs of [128 rows][128 B] in the ring's
+// 128B swizzle, guarded by epi_full[c] / epi_empty[c] (count 1 each). Tile l of a CTA belongs to warpgroup c = l & 1 and
+// is the (l >> 1)-th use of its buffer; both barriers are waited with parity (l >> 1) & 1, epi_empty with the ring's
+// "previous phase" convention (the first wait passes).
+//   producer, before tile l's K-chunks: wait epi_empty[c], then TMA-load the tile's residual or mask box into the buffer
+//     (complete_tx on epi_full[c]), or arrive on epi_full[c] when there is none. The load lands during the MMAs.
+//   warpgroup c, after its MMAs: wait epi_full[c]; each thread reads its residual / mask and writes the rounded bf16
+//     result in the same place (generic proxy), fence.proxy.async.shared::cta, 128-thread named barrier; one thread
+//     issues one TMA store per slab, commits, and after the statistics waits cp.async.bulk.wait_group.read 0 (the
+//     buffer has been read) before it arrives on epi_empty[c]. It waits for full completion before the CTA exits.
+// So the buffer is written by TMA only after the previous tile's store has read it, and by the threads only after that
+// load (or the producer's plain arrival, which itself followed the read) completed.
+//
 // Replaces the cuDNN kernels behind nn.Conv2d at reference ae.py:105-117,143-154,160-167 and the
 // torchvision VGG convs reached from utils.py:95-111,150-154 (see include/vqb200.h).
 #include "common.cuh"
@@ -35,12 +49,15 @@ constexpr int kMaxStages = 8;
 constexpr int kConsumerWarps = 8;
 constexpr int kProducerRegs = 40;   // setmaxnreg split: 40 * 128 + 232 * 256 <= 64 K registers
 constexpr int kConsumerRegs = 232;
+constexpr int kStagedKChunksPerTensor = 18;  // staged-epilogue rule in conv_gemm_impl (DESIGN.md 3.1)
 
 struct alignas(64) ConvParams {
     static constexpr int kRank = 4;  // NHWC activations, 4-D TMA boxes [64 ch][bw][bh][bn]
     static constexpr int kViews = VQB_MAX_VIEWS;
     CUtensorMap amap[VQB_MAX_VIEWS];
     CUtensorMap bmap;
+    CUtensorMap omap;  // staged epilogue: the output as [Cout][W][H][N], box [64 ch][bw][bh][bn]
+    CUtensorMap emap;  // staged epilogue: the residual or the mask, same extents, strides and box as omap
     int32_t tap_view[VQB_MAX_TAPS];
     int32_t tap_dw[VQB_MAX_TAPS];
     int32_t tap_dh[VQB_MAX_TAPS];
@@ -92,19 +109,28 @@ struct alignas(64) Conv3dParamsT {
 using Conv3dParams = Conv3dParamsT<VQB_MAX_TAPS_3D>;
 using Conv3dDgradParams = Conv3dParamsT<VQB_MAX_TAPS_3D_DGRAD>;
 
-template <int BN, class P>
+template <int BN, class P, bool kStaged>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ P p) {
     constexpr bool kR5 = P::kRank == 5;
+    static_assert(!kStaged || (!kR5 && BN >= 64), "the staged epilogue stores whole 64-channel slabs of 2-D outputs");
     extern __shared__ uint8_t smem_raw[];
     constexpr uint32_t kBBytes = BN * kBlockK * 2;
     constexpr uint32_t kStageBytes = kABytes + kBBytes;  // a multiple of 2 KB: every tile stays 1024-B aligned
     // carve shared memory (1024-B aligned for the 128B swizzle atoms)
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t stages = p.stages;
-    float* sStat = reinterpret_cast<float*>(base + stages * kStageBytes);  // [2 warpgroups][4 warps][BN][2]
+    // staged epilogue: one 128 x BN bf16 tile per consumer warpgroup, as BN / 64 slabs of [128 rows][64 ch] in the
+    // ring's 128B swizzle (what a [64 ch][bw][bh][bn] TMA box writes), after the ring
+    constexpr uint32_t kSlabBytes = kBlockM * kBlockK * 2;
+    constexpr uint32_t kEpiBytes = kBlockM * BN * 2;
+    constexpr uint32_t kRowOff[4] = {0, 8 * 128, 64 * 128, 72 * 128};  // row groups r = 2 mb + i: rows + 64 mb + 8 i
+    uint8_t* epi = base + stages * kStageBytes;
+    float* sStat = reinterpret_cast<float*>(epi + (kStaged ? 2 * kEpiBytes : 0));  // [2 warpgroups][4 warps][BN][2]
     uint64_t* full = reinterpret_cast<uint64_t*>(sStat + kConsumerWarps * BN * 2);
     uint64_t* empty = full + stages;
     uint64_t* order = empty + stages;  // [warpgroup]: one phase per tile, completed at its last full wait
+    uint64_t* epi_full = order + 2;    // [warpgroup]: its tile buffer holds the residual / mask (or is free to write)
+    uint64_t* epi_empty = epi_full + 2;  // [warpgroup]: the TMA store of its previous tile has read the buffer
     const uint32_t wg = threadIdx.x >> 7;
     const uint32_t warp = (threadIdx.x >> 5) & 3u;  // warp inside its warpgroup
     const uint32_t lane = threadIdx.x & 31u;
@@ -116,12 +142,19 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             if (used) tma_prefetch_desc(&p.amap[v]);
         }
         tma_prefetch_desc(&p.bmap);
+        if constexpr (kStaged) {
+            tma_prefetch_desc(&p.omap);
+            if (p.flags & (VQB_EPI_RES | VQB_EPI_MASK)) tma_prefetch_desc(&p.emap);
+        }
         for (uint32_t i = 0; i < stages; ++i) {
             mbar_init(&full[i], 1);
             mbar_init(&empty[i], 4);  // lane 0 of every warp of the consuming warpgroup releases the stage
         }
-        mbar_init(&order[0], 4);
-        mbar_init(&order[1], 4);
+        for (int c = 0; c < 2; ++c) {
+            mbar_init(&order[c], 4);
+            mbar_init(&epi_full[c], 1);
+            mbar_init(&epi_empty[c], 1);
+        }
         fence_mbar_init();
     }
     __syncthreads();
@@ -132,7 +165,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         setmaxnreg_dec<kProducerRegs>();
         if (warp == 0 && elect_one()) {
             uint32_t stage = 0, phase = 0;
-            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+            for (int tile = blockIdx.x, l = 0; tile < p.total_tiles; tile += gridDim.x, ++l) {
                 const int n_tile = tile % p.n_tiles;
                 const int m_tile = tile / p.n_tiles;
                 const int tw = m_tile % p.tiles_w;
@@ -146,6 +179,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                 }
                 const int w0 = tw << p.lbw, h0 = th << p.lbh, n0 = tn << p.lbn;
                 const int ncol0 = n_tile * BN;
+                if constexpr (kStaged) {
+                    // tile l goes to warpgroup l & 1: once its buffer is free (the store of tile l - 2 has read
+                    // it), fill it with this tile's residual or mask; it lands while the tile's MMAs run
+                    const uint32_t c = l & 1;
+                    mbar_wait(&epi_empty[c], ((l >> 1) & 1) ^ 1);
+                    if (p.flags & (VQB_EPI_RES | VQB_EPI_MASK)) {
+                        const int nslab = min(BN, p.Cout - ncol0) / kBlockK;  // Cout % 64 == 0
+                        mbar_arrive_expect_tx(&epi_full[c], nslab * kSlabBytes);
+                        for (int s = 0; s < nslab; ++s)
+                            tma_load_4d(&p.emap, &epi_full[c], epi + c * kEpiBytes + s * kSlabBytes,
+                                        ncol0 + s * kBlockK, w0, h0, n0);
+                    } else {
+                        mbar_arrive(&epi_full[c]);
+                    }
+                }
                 for (int t = 0; t < p.ntaps; ++t) {
                     for (int kc = 0; kc < p.kchunks; ++kc) {
                         mbar_wait(&empty[stage], phase ^ 1);
@@ -231,7 +279,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         fence_operands(acc[1]);
         if (lane == 0) mbar_arrive(&empty[prev]);  // num_kb >= 1 (ntaps >= 1, C > 0)
 
-        // ---------------- epilogue straight from the accumulator fragment
+        // ---------------- epilogue: from the accumulator fragment to global memory, or through the staged tile
         const int n_tile = tile % p.n_tiles;
         const int m_tile = tile / p.n_tiles;
         const int tw = m_tile % p.tiles_w;
@@ -244,25 +292,31 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             tn = m_tile / (p.tiles_w * p.tiles_h);
         }
         const int col0 = n_tile * BN;
+        uint8_t* tbuf = epi + cw * kEpiBytes;  // staged: this warpgroup's tile buffer
+        // staged: this thread's column pair in row group 0 (row % 8 == lane / 4 in all four row groups)
+        const uint32_t trow = smem_u32(tbuf) + (warp * 16 + (lane >> 2)) * 128u + (lane & 3u) * 4u;
+        if (kStaged) mbar_wait(&epi_full[cw], (l >> 1) & 1);
         // row group r = 2 * mb + i: acc[mb][4j + 2i + e] is row 64 mb + 16 warp + lane / 4 + 8 i, column 8j + 2(lane % 4) + e
-        int64_t pix[4];
-        bool valid[4];
+        int64_t pix[4] = {0, 0, 0, 0};
+        bool valid[4] = {true, true, true, true};  // staged: rows outside the tensor are computed, then clipped by TMA
+        if constexpr (!kStaged) {
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const uint32_t row = (r >> 1) * 64 + warp * 16 + (lane >> 2) + 8 * (r & 1);  // row of the 128-pixel box
-            const int w = (tw << p.lbw) + static_cast<int>(row & ((1u << p.lbw) - 1));
-            const int h = (th << p.lbh) + static_cast<int>((row >> p.lbw) & ((1u << p.lbh) - 1));
-            if constexpr (kR5) {  // row = w + bw * (h + bh * (t + bt * n)) of the 128-voxel box
-                const int t = (tt << p.lbt) + static_cast<int>((row >> (p.lbw + p.lbh)) & ((1u << p.lbt) - 1));
-                const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh + p.lbt));
-                valid[r] = (w < p.W) && (h < p.H) && (t < p.T) && (n < p.N);
-                pix[r] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(t) * p.ot +
-                         static_cast<int64_t>(h) * p.oh + static_cast<int64_t>(w) * p.ow;
-            } else {
-                const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh));
-                valid[r] = (w < p.W) && (h < p.H) && (n < p.N);
-                pix[r] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh +
-                         static_cast<int64_t>(w) * p.ow;
+            for (int r = 0; r < 4; ++r) {
+                const uint32_t row = (r >> 1) * 64 + warp * 16 + (lane >> 2) + 8 * (r & 1);  // row of the 128-pixel box
+                const int w = (tw << p.lbw) + static_cast<int>(row & ((1u << p.lbw) - 1));
+                const int h = (th << p.lbh) + static_cast<int>((row >> p.lbw) & ((1u << p.lbh) - 1));
+                if constexpr (kR5) {  // row = w + bw * (h + bh * (t + bt * n)) of the 128-voxel box
+                    const int t = (tt << p.lbt) + static_cast<int>((row >> (p.lbw + p.lbh)) & ((1u << p.lbt) - 1));
+                    const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh + p.lbt));
+                    valid[r] = (w < p.W) && (h < p.H) && (t < p.T) && (n < p.N);
+                    pix[r] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(t) * p.ot +
+                             static_cast<int64_t>(h) * p.oh + static_cast<int64_t>(w) * p.ow;
+                } else {
+                    const int n = (tn << p.lbn) + static_cast<int>(row >> (p.lbw + p.lbh));
+                    valid[r] = (w < p.W) && (h < p.H) && (n < p.N);
+                    pix[r] = static_cast<int64_t>(n) * p.on + static_cast<int64_t>(h) * p.oh +
+                             static_cast<int64_t>(w) * p.ow;
+                }
             }
         }
 #pragma unroll
@@ -275,12 +329,23 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                 b1 = ok1 ? __ldg(p.bias + col + 1) : 0.f;
             }
             float r1[2] = {0.f, 0.f}, r2[2] = {0.f, 0.f};  // per column: statistics partial sums over this thread's rows
-            if (vec_path && ok1) {
+            if (kStaged ? ok1 : vec_path && ok1) {
                 // all residual / mask loads of the column group in flight before the first use
                 __nv_bfloat162 rv[4], mv[4];
+                // staged: 16-byte chunk j % 8 of a 128-B row, XOR row % 8 (128B swizzle). The 8 rows a warp touches
+                // per access fall in 8 different chunks, so these loads and stores are free of bank conflicts.
+                const uint32_t tj = trow + (j >> 3) * kSlabBytes + (((j & 7u) ^ (lane >> 2)) << 4);
 #pragma unroll
                 for (int r = 0; r < 4; ++r) {
                     rv[r] = mv[r] = __floats2bfloat162_rn(0.f, 0.f);
+                    if constexpr (kStaged) {
+                        if (has_res || has_mask) {
+                            const __nv_bfloat162 v = u32_as_bf16x2(ld_shared_u32(tj + kRowOff[r]));
+                            if (has_res) rv[r] = v;
+                            if (has_mask) mv[r] = v;
+                        }
+                        continue;
+                    }
                     const int64_t o = pix[r] + col;  // 4-byte aligned: pixel strides % 8 == 0, col even
                     if (has_res && valid[r]) rv[r] = *reinterpret_cast<const __nv_bfloat162*>(res + o);
                     if (has_mask && valid[r]) mv[r] = *reinterpret_cast<const __nv_bfloat162*>(mask + o);
@@ -305,7 +370,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                         if (!(m.y > 0.f)) f[1] = 0.f;
                     }
                     const __nv_bfloat162 ob = __floats2bfloat162_rn(f[0], f[1]);
-                    *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix[r] + col) = ob;
+                    if constexpr (kStaged)
+                        st_shared_u32(tj + kRowOff[r], bf16x2_as_u32(ob));  // in place of its residual / mask
+                    else
+                        *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix[r] + col) = ob;
                     if (reduce) {
                         const float2 v = __bfloat1622float2(ob);  // the bf16 values the consumer will read
                         r1[0] += v.x;
@@ -314,7 +382,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                         r2[1] = fmaf(v.y, v.y, r2[1]);
                     }
                 }
-            } else {
+            } else if constexpr (!kStaged) {
                 // generic strided / ragged path (small or odd Cout, NCHW fp32 outputs)
 #pragma unroll
                 for (int r = 0; r < 4; ++r) {
@@ -351,6 +419,19 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                 }
             }
         }
+        if constexpr (kStaged) {
+            // the tile's generic-proxy writes, then one thread hands it to the TMA unit: one store per 64-channel slab
+            // inside Cout (rows outside the tensor are clipped by TMA)
+            fence_proxy_async_shared();
+            named_bar_sync(1 + cw, 128);
+            if (wtid == 0) {
+                const int nslab = min(BN, p.Cout - col0) / kBlockK;
+                for (int s = 0; s < nslab; ++s)
+                    tma_store_4d(&p.omap, tbuf + s * kSlabBytes, col0 + s * kBlockK, tw << p.lbw, th << p.lbh,
+                                 tn << p.lbn);
+                bulk_commit_group();
+            }
+        }
         if (reduce) {
             // the statistics need every row of the tile inside one image (checked on the host: vqb_conv_stats_ok)
             named_bar_sync(1 + cw, 128);
@@ -365,7 +446,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             }
             named_bar_sync(1 + cw, 128);  // this warpgroup's sStat half is reused by its next tile
         }
+        if (kStaged && wtid == 0) {
+            bulk_wait_group_read<0>();  // the buffer is free: the producer may load tile l + 2's residual / mask
+            mbar_arrive(&epi_empty[cw]);
+        }
     }
+    if (kStaged && wtid == 0) bulk_wait_group<0>();  // the last tile's stores are complete before the CTA exits
 }
 
 static int fill_views(const VqbView* views, int nviews, const void* a, int C, int lbw, int lbh, int lbn,
@@ -384,20 +470,32 @@ static int fill_views(const VqbView* views, int nviews, const void* a, int C, in
     return VQB_OK;
 }
 
-template <int BN, class P>
+// Dynamic shared memory of one CTA: alignment slack, ring, the two staged epilogue tiles, statistics staging, the
+// full / empty barriers of the ring and the order / epi_full / epi_empty pairs.
+static size_t conv_smem_bytes(int block_n, int stages, bool staged) {
+    return 1024 + static_cast<size_t>(stages) * (kABytes + block_n * kBlockK * 2) +
+           (staged ? 2 * kBlockM * block_n * 2 : 0) + kConsumerWarps * block_n * 2 * sizeof(float) + 8 * (2 * stages + 6);
+}
+
+// The deepest ring (<= kMaxStages) that fits next to the rest: 6 stages at BLOCK_N = 128 and 8 below it, or 4 and 7
+// when the staged epilogue tiles take their 64 / 32 KB.
+static int ring_stages(int block_n, bool staged) {
+    int stages = kMaxStages;
+    while (conv_smem_bytes(block_n, stages, staged) > 227 * 1024) --stages;
+    return stages;
+}
+
+template <int BN, bool kStaged = false, class P>
 static int launch_conv(const P& p, void* stream) {
-    constexpr size_t stage_bytes = kABytes + BN * kBlockK * 2;
-    // ring + statistics staging + full / empty barriers + the two order barriers
-    const size_t smem =
-        1024 + p.stages * stage_bytes + kConsumerWarps * BN * 2 * sizeof(float) + 2 * 8 * p.stages + 2 * 8;
+    const size_t smem = conv_smem_bytes(BN, p.stages, kStaged);
     static bool attr_set = false;
     if (!attr_set) {
-        VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        VQB_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, P, kStaged>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       227 * 1024));
         attr_set = true;
     }
     const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-    conv_gemm_kernel<BN, P><<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
+    conv_gemm_kernel<BN, P, kStaged><<<grid, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
     VQB_CUDA(cudaGetLastError());
     return VQB_OK;
 }
@@ -479,11 +577,18 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     }
     p.do_stats = (d->flags & VQB_EPI_STATS) ? 1 : 0;
     if (query_only) return stats_ok ? 1 : 0;
-    const int stage_bytes = kABytes + block_n * kBlockK * 2;
-    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages + 2 * 8;
-    int stages = (227 * 1024 - fixed) / stage_bytes;
-    if (stages > kMaxStages) stages = kMaxStages;
-    p.stages = stages;
+    // Staged epilogue (kernel header): whole 64-channel slabs of an NHWC bf16 output that TMA can address, and at most
+    // one of residual / mask, 16-byte aligned like the output. It saves per tile in proportion to the tile-sized tensors
+    // the epilogue moves (the output, and the residual or mask), and its two tile buffers cost the ring 2 of its 6
+    // stages at BLOCK_N = 128 (1 of 8 at 64), a loss in proportion to the K-chunks of a tile: it is taken up to
+    // kStagedKChunksPerTensor K-chunks per moved tensor. Everything else stores from the accumulator fragment.
+    const bool has_res = d->flags & VQB_EPI_RES, has_mask = d->flags & VQB_EPI_MASK;
+    const void* eop = has_res ? res : mask;
+    const int moved = (has_res || has_mask) ? 2 : 1;
+    const bool staged = nhwc_bf16 && d->Cout % 64 == 0 && d->on > 0 && d->oh > 0 && d->ow > 0 &&
+                        !(has_res && has_mask) && (reinterpret_cast<uintptr_t>(eop) & 15u) == 0 &&
+                        d->ntaps * ((d->C + kBlockK - 1) / kBlockK) <= kStagedKChunksPerTensor * moved;
+    p.stages = ring_stages(block_n, staged);
     p.ntaps = d->ntaps;
     p.kchunks = (d->C + kBlockK - 1) / kBlockK;
     p.C = d->C;
@@ -511,6 +616,18 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     }
     int rc = fill_views(d->views, d->nviews, a, d->C, p.lbw, p.lbh, p.lbn, p.amap);
     if (rc != VQB_OK) return rc;
+    if (staged) {
+        // the output (and the residual / mask, which share its strides) as 4-D tensors [Cout][W][H][N] in the
+        // activations' box: out-of-range rows are zero-filled on load and clipped on store
+        uint64_t dims[4] = {static_cast<uint64_t>(d->Cout), static_cast<uint64_t>(d->W), static_cast<uint64_t>(d->H),
+                            static_cast<uint64_t>(d->N)};
+        uint64_t str[3] = {static_cast<uint64_t>(d->ow) * 2, static_cast<uint64_t>(d->oh) * 2,
+                           static_cast<uint64_t>(d->on) * 2};
+        uint32_t box[4] = {kBlockK, bw, bh, bn};
+        rc = encode_tmap_bf16(&p.omap, out, 4, dims, str, box, 128);
+        if (rc == VQB_OK && (has_res || has_mask)) rc = encode_tmap_bf16(&p.emap, eop, 4, dims, str, box, 128);
+        if (rc != VQB_OK) return rc;
+    }
     {
         const uint64_t ktot = static_cast<uint64_t>(d->ntaps) * d->C;
         uint64_t dims[2] = {ktot, static_cast<uint64_t>(d->Cout)};
@@ -522,8 +639,8 @@ static int conv_gemm_impl(const VqbConvDesc* d, const void* a, const void* w_pac
     switch (block_n) {
         case 16: rc = launch_conv<16>(p, stream); break;
         case 32: rc = launch_conv<32>(p, stream); break;
-        case 64: rc = launch_conv<64>(p, stream); break;
-        default: rc = launch_conv<128>(p, stream); break;
+        case 64: rc = staged ? launch_conv<64, true>(p, stream) : launch_conv<64>(p, stream); break;
+        default: rc = staged ? launch_conv<128, true>(p, stream) : launch_conv<128>(p, stream); break;
     }
     if (rc != VQB_OK) return rc;
     count_launch();
@@ -593,11 +710,7 @@ static int conv3d_impl(const char* fn, const D* d, const void* a, const void* w_
     const int64_t total = static_cast<int64_t>(p.tiles_w) * p.tiles_h * p.tiles_t * ((d->N + bn - 1) / bn) * p.n_tiles;
     VQB_CHECK(total < (1ll << 31), "%s: too many tiles", fn);
     p.total_tiles = static_cast<int32_t>(total);
-    const int stage_bytes = kABytes + block_n * kBlockK * 2;
-    const int fixed = 1024 + kConsumerWarps * block_n * 2 * 4 + 2 * 8 * kMaxStages + 2 * 8;
-    int stages = (227 * 1024 - fixed) / stage_bytes;
-    if (stages > kMaxStages) stages = kMaxStages;
-    p.stages = stages;
+    p.stages = ring_stages(block_n, false);
     p.ntaps = d->ntaps;
     p.kchunks = (d->C + kBlockK - 1) / kBlockK;
     p.C = d->C;

@@ -122,6 +122,29 @@ __device__ __forceinline__ void tma_load_5d(const void* desc, uint64_t* bar, voi
         : "memory");
 }
 
+// smem -> global tiled store (async proxy); out-of-range box elements are not written. Completion is tracked per thread
+// with bulk groups: commit, then wait_group.read (the smem source may be reused) or wait_group (the writes are done).
+__device__ __forceinline__ void tma_store_4d(const void* desc, const void* smem, int32_t c0, int32_t c1, int32_t c2,
+                                             int32_t c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 :
+                 : "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() {
+    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+// Orders this thread's generic-proxy shared-memory accesses before later async-proxy (TMA) accesses of the CTA.
+__device__ __forceinline__ void fence_proxy_async_shared() {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -262,6 +285,16 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint6
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
     __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ __nv_bfloat162 u32_as_bf16x2(uint32_t u) { return *reinterpret_cast<__nv_bfloat162*>(&u); }
+__device__ __forceinline__ uint32_t bf16x2_as_u32(__nv_bfloat162 h) { return *reinterpret_cast<uint32_t*>(&h); }
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
     __nv_bfloat162 h = *reinterpret_cast<__nv_bfloat162*>(&u);
