@@ -329,6 +329,35 @@ int vqb_gauss_reparam(const void* z, const void* eps, void* out, int N, int Z, i
 int vqb_gauss_reparam_bwd(const float* g, const float* z, const float* eps, float* dz, int N, int Z, int64_t S,
                           void* stream);
 
+/*
+ * Clip boundary of the per-frame image losses (utils.LPIPS / utils.PatchDiscriminator called on a [B][C][T][H][W] clip,
+ * tae_trainer.VideoTrainer): the frames of a clip, folded into the batch in (b, t) order, as per-frame NHWC bf16 images
+ * [B*Tsel][H+2pad][W+2pad][Cpad], with the (x - shift) * inv_scale of vqb_nchw_to_nhwc fused in (the same fp32 arithmetic
+ * and one rounding, so each image equals vqb_nchw_to_nhwc_pad of that frame bit for bit). The clip is read through its
+ * strides (channel T*H*W, frame H*W): no folded copy. frames (device, int32 [B*Tsel], optional): image i is frame
+ * frames[i] of clip i / Tsel; NULL means every frame (Tsel = T). The entries of one clip must be distinct and in [0, T):
+ * the caller checks that on the host (ops.ClipToFrames). pad > 0 writes the interior of a PRE-ZEROED framed buffer.
+ * x is fp32 or (_bf16) bf16; shift / inv_scale both NULL or both given. The non-_pad forms are pad = 0.
+ * Every entry point validates its arguments (VQB_EINVAL) and fails with VQB_ENODEVICE without an sm_90 device.
+ */
+int vqb_ncthw_frames_to_nhwc_pad(const float* x, void* y, int B, int C, int T, int H, int W, int Cpad, int pad,
+                                 const int* frames, int Tsel, const float* shift, const float* inv_scale, void* stream);
+int vqb_ncthw_frames_to_nhwc_pad_bf16(const void* x, void* y, int B, int C, int T, int H, int W, int Cpad, int pad,
+                                      const int* frames, int Tsel, const float* shift, const float* inv_scale,
+                                      void* stream);
+int vqb_ncthw_frames_to_nhwc(const float* x, void* y, int B, int C, int T, int H, int W, int Cpad, const int* frames,
+                             int Tsel, const float* shift, const float* inv_scale, void* stream);
+int vqb_ncthw_frames_to_nhwc_bf16(const void* x, void* y, int B, int C, int T, int H, int W, int Cpad,
+                                  const int* frames, int Tsel, const float* shift, const float* inv_scale,
+                                  void* stream);
+/* The backward: gx [B][C][T][H][W] fp32 = g[image of (b, t)][h][w][c] * inv_scale[c] (inv_scale may be NULL), the
+ * arithmetic of vqb_nhwc_to_nchw_pad; frames not in the selection get exact zeros from the same launch. Every element
+ * of gx is written exactly once. */
+int vqb_nhwc_pad_frames_to_ncthw(const void* g, float* gx, int B, int C, int T, int H, int W, int Cpad, int pad,
+                                 const int* frames, int Tsel, const float* inv_scale, void* stream);
+int vqb_nhwc_frames_to_ncthw(const void* g, float* gx, int B, int C, int T, int H, int W, int Cpad, const int* frames,
+                             int Tsel, const float* inv_scale, void* stream);
+
 /* out[c] = sum over P pixels of x[p][c] : Conv2d bias gradient */
 int vqb_colsum(const void* x, float* out, int64_t P, int C, void* stream);
 

@@ -1,0 +1,141 @@
+"""Times tae_trainer.VideoTrainer.step (the video autoencoder trained against per-frame losses) for three loss stacks:
+MSE only (lpips=None), + LPIPS, and + LPIPS + PatchGAN (hinge, LeCam), each on every frame of the clip and on
+--perceptual-frames frames per clip. Every arm is also run as a bf16-autocast eager peer: the same folded computation
+in plain PyTorch (oracle/tae_oracle.py, oracle/clip_loss_oracle.py: F.conv3d / F.conv2d VGG16 with cuDNN) with
+torch.optim.AdamW.
+
+Usage: python tools/tae_loss_bench.py [--frames 16] [--res 256] [--ch 64] [--batch 1] [--perceptual-frames 4]
+           [--steps 5] [--warmup 2] [--skip-peer]
+
+Prints one JSON line per arm with ms/step, frames/s (clip frames through the autoencoder per second) and peak
+allocated memory, plus the card's name and power limit read in the same run. LPIPS / PatchD weights are torchvision's
+random initialisation (VQB_OFFLINE=1): the timing does not depend on the values.
+"""
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "vqgan-training_b200"))
+sys.path.insert(1, ROOT)
+sys.path.insert(2, os.path.join(ROOT, "tools"))
+os.environ.setdefault("VQB_OFFLINE", "1")
+
+import torch  # noqa: E402
+import torch.nn.functional as F  # noqa: E402
+
+from infer_bench import card, timed  # noqa: E402
+from oracle import clip_loss_oracle as CO  # noqa: E402
+from oracle import loss_oracle as LO  # noqa: E402
+from oracle import tae_oracle as TO  # noqa: E402
+
+STACKS = ("mse", "lpips", "lpips+gan")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=16)
+    ap.add_argument("--res", type=int, default=256)
+    ap.add_argument("--ch", type=int, default=64)
+    ap.add_argument("--batch", type=int, default=1)
+    ap.add_argument("--perceptual-frames", type=int, default=4)
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--skip-peer", action="store_true")
+    a = ap.parse_args()
+
+    import tae
+    import tae_trainer
+    import utils
+
+    cfg = TO.TAEConfig(ch=a.ch)
+    N, T = a.batch, a.frames
+    info = card()
+    torch.manual_seed(0)
+    x = torch.rand(N, 3, T, a.res, a.res, device="cuda") * 2 - 1
+    torch.manual_seed(1)
+    tsd = tae.TVAE(**cfg.kwargs()).state_dict()
+    lsd = utils.LPIPS().state_dict()
+    psd = utils.PatchDiscriminator().state_dict()
+
+    def report(arm, stack, k, ms, peak):
+        print(json.dumps({"arm": arm, "loss": stack, "perceptual_frames": k or T, "frames": T, "res": a.res,
+                          "ch": a.ch, "batch": N, "ms_per_step": round(ms, 2),
+                          "frames_per_s": round(N * T * 1e3 / ms, 1), "peak_alloc_gb": round(peak / 2 ** 30, 2),
+                          "gpu": info}), flush=True)
+
+    def native(stack, k):
+        m = tae.TVAE(**cfg.kwargs())
+        m.load_state_dict(tsd)
+        lp = pd = None
+        if stack != "mse":
+            lp = utils.LPIPS()
+            lp.load_state_dict(lsd)
+            lp = lp.cuda().eval()
+        if stack == "lpips+gan":
+            pd = utils.PatchDiscriminator()
+            pd.load_state_dict(psd)
+            pd = pd.cuda()
+        tr = tae_trainer.VideoTrainer(m.cuda(), lp, pd, disc_type="hinge", use_lecam=True, perceptual_frames=k,
+                                      lr_vae=1e-4, lr_disc=2e-4)
+        ms, peak, _ = timed(lambda: tr.step(x), a.steps, a.warmup)
+        report("native", stack, k, ms, peak)
+        del tr, m, lp, pd
+        torch.cuda.empty_cache()
+
+    def peer(stack, k):
+        tp = {n: v.cuda().clone().requires_grad_(True) for n, v in tsd.items()}
+        ls = {n: v.cuda() for n, v in lsd.items()}
+        dp = {n: v.cuda().clone().requires_grad_("scaling_layer" not in n) for n, v in psd.items()}
+        kw = dict(weight_decay=1e-3, betas=(0.9, 0.95))
+        opt_g = torch.optim.AdamW(tp.values(), lr=1e-4, **kw)
+        opt_d = torch.optim.AdamW([v for v in dp.values() if v.requires_grad], lr=2e-4, **kw)
+        anchors = [torch.zeros((), device="cuda"), torch.zeros((), device="cuda")]
+        ac = lambda: torch.autocast("cuda", dtype=torch.bfloat16)  # noqa: E731
+
+        def step():
+            sel = None if k is None else torch.stack([torch.randperm(T)[:k] for _ in range(N)])
+            with ac():
+                z = TO.encoder_forward(tp, x, cfg)
+                decz = TO.decoder_forward(tp, TO.reg(z, torch.randn_like(z[:, :cfg.z_channels])), cfg)
+            decz, z = decz.float(), z.float()
+            if stack == "lpips+gan":
+                with ac():
+                    real = CO.patchd_clip(dp, x, sel).float()
+                    fake = CO.patchd_clip(dp, decz.detach(), sel).float()
+                d_loss = (F.relu(1 - real).mean() + F.relu(1 + fake).mean()) * 0.5
+                anchors[0] = 0.9 * anchors[0] + 0.1 * real.detach().mean()
+                anchors[1] = 0.9 * anchors[1] + 0.1 * fake.detach().mean()
+                d_loss = d_loss + 0.1 * LO.lecam_loss(real, fake, anchors[0], anchors[1])
+                opt_d.zero_grad(set_to_none=True)
+                d_loss.backward()
+                opt_d.step()
+            with ac():
+                if stack == "mse":
+                    rec = F.mse_loss(CO.fold_frames(decz, sel), CO.fold_frames(x, sel))
+                else:
+                    rec = CO.lpips_clip(ls, LO.gradnorm(decz), x, sel).float().mean()
+                loss = rec + 0.1 * z.pow(2).mean()
+                if stack == "lpips+gan":
+                    frozen = {n: v.detach() for n, v in dp.items()}
+                    loss = loss - CO.patchd_clip(frozen, LO.gradnorm(decz, 1.0), sel).float().mean()
+            opt_g.zero_grad(set_to_none=True)
+            loss.backward()
+            opt_g.step()
+            return loss
+
+        ms, peak, _ = timed(step, a.steps, a.warmup)
+        report("bf16-autocast eager peer", stack, k, ms, peak)
+        del tp, dp, opt_g, opt_d
+        torch.cuda.empty_cache()
+
+    for k in (None, a.perceptual_frames):
+        for stack in STACKS:
+            native(stack, k)
+            if not a.skip_peer:
+                peer(stack, k)
+
+
+if __name__ == "__main__":
+    main()

@@ -168,6 +168,76 @@ __global__ void nhwc_to_nchw_kernel(const __nv_bfloat16* __restrict__ g, Out* __
     }
 }
 
+// ------------------------------------------------------------------ clip <-> per-frame layout
+// Clips are NCTHW: channel stride T*HW, frame stride HW. Image i of the per-frame NHWC buffer is frame frames[i] (all
+// frames: i % Tsel) of clip i / Tsel. grid (pixel blocks, images); per element the arithmetic of nchw_to_nhwc_kernel.
+template <typename In>
+__global__ void clip_to_frames_kernel(const In* __restrict__ x, __nv_bfloat16* __restrict__ y, int C, int T, int HW,
+                                      int W, int Cpad, int pad, const int* __restrict__ frames, int Tsel,
+                                      const float* __restrict__ shift, const float* __restrict__ inv_scale) {
+    const int img = blockIdx.y;
+    const int t = frames ? frames[img] : img % Tsel;
+    const int H = HW / W;
+    const In* xb = x + (static_cast<int64_t>(img / Tsel) * C * T + t) * HW;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += gridDim.x * blockDim.x) {
+        const int h = p / W, w = p % W;
+        const int64_t opix = (static_cast<int64_t>(img) * (H + 2 * pad) + h + pad) * (W + 2 * pad) + w + pad;
+        __nv_bfloat16* yp = y + opix * Cpad;
+        for (int c0 = 0; c0 < Cpad; c0 += 8) {
+            float f[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int c = c0 + j;
+                float v = 0.f;
+                if (c < C && static_cast<unsigned>(t) < static_cast<unsigned>(T)) {
+                    v = to_f32(xb[static_cast<int64_t>(c) * T * HW + p]);
+                    if (shift) v = (v - shift[c]) * inv_scale[c];
+                }
+                f[j] = v;
+            }
+            store8(yp + c0, f);
+        }
+    }
+}
+
+// gx[b,c,t,h,w] = g[img,h,w,c] * inv_scale[c] where frames[img] == t within clip b, else 0: grid (pixel blocks, B*T clip
+// frames), so every element of the clip gradient is written exactly once by one launch.
+__global__ void frames_to_clip_kernel(const __nv_bfloat16* __restrict__ g, float* __restrict__ gx, int C, int T, int HW,
+                                      int W, int Cpad, int pad, const int* __restrict__ frames, int Tsel,
+                                      const float* __restrict__ inv_scale) {
+    __shared__ int s_img;
+    const int b = blockIdx.y / T, t = blockIdx.y % T;
+    if (threadIdx.x == 0) {
+        int img = -1;
+        if (frames) {
+            for (int j = 0; j < Tsel; ++j)
+                if (frames[b * Tsel + j] == t) img = b * Tsel + j;
+        } else {
+            img = b * Tsel + t;
+        }
+        s_img = img;
+    }
+    __syncthreads();
+    const int img = s_img;
+    const int H = HW / W;
+    float* xb = gx + (static_cast<int64_t>(b) * C * T + t) * HW;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += gridDim.x * blockDim.x) {
+        float* xp = xb + p;
+        if (img < 0) {
+            for (int c = 0; c < C; ++c) xp[static_cast<int64_t>(c) * T * HW] = 0.f;
+            continue;
+        }
+        const int h = p / W, w = p % W;
+        const int64_t ipix = (static_cast<int64_t>(img) * (H + 2 * pad) + h + pad) * (W + 2 * pad) + w + pad;
+        const __nv_bfloat16* gp = g + ipix * Cpad;
+        for (int c = 0; c < C; ++c) {
+            float v = __bfloat162float(gp[c]);
+            if (inv_scale) v *= inv_scale[c];
+            xp[static_cast<int64_t>(c) * T * HW] = v;
+        }
+    }
+}
+
 // ------------------------------------------------------------------ GroupNorm forward
 // grid (chunks, N); thread t owns channel vector cv = t % V (V = C/8) and pixel rows t / V + k*R.
 // The R row partials of a block are summed in a fixed order (no shared-memory float atomics), so the fp32 chunk sums do
@@ -693,6 +763,55 @@ __global__ void gauss_reparam_bwd_kernel(const float* __restrict__ g, const floa
     }
 }
 
+// Clip boundary (per-frame LPIPS / PatchGAN on NCTHW clips): frames of a clip <-> per-frame NHWC images. `images` is
+// the grid's y extent (B*Tsel forward, B*T backward). Every argument is checked before the device.
+int check_clip_args(const char* fn, const void* in, const void* out, int B, int C, int T, int H, int W, int Cpad,
+                    int pad, const int* frames, int Tsel, const float* shift, const float* inv_scale, int64_t images) {
+    VQB_CHECK(in, "%s: null input pointer", fn);
+    VQB_CHECK(out, "%s: null output pointer", fn);
+    VQB_CHECK(B > 0 && C > 0 && T > 0 && H > 0 && W > 0, "%s: bad clip size (B=%d C=%d T=%d H=%d W=%d)", fn, B, C, T, H,
+              W);
+    VQB_CHECK(Cpad % 8 == 0 && Cpad >= C, "%s: bad Cpad=%d for C=%d", fn, Cpad, C);
+    VQB_CHECK(pad >= 0, "%s: bad pad=%d", fn, pad);
+    VQB_CHECK(Tsel > 0 && Tsel <= T, "%s: bad Tsel=%d for T=%d", fn, Tsel, T);
+    VQB_CHECK(frames != nullptr || Tsel == T, "%s: Tsel=%d without a frame list must equal T=%d", fn, Tsel, T);
+    VQB_CHECK((shift == nullptr) == (inv_scale == nullptr), "%s: shift and inv_scale must both be given or null", fn);
+    VQB_CHECK(images <= 65535, "%s: %lld frames in one launch exceed 65535", fn, static_cast<long long>(images));
+    VQB_CHECK(static_cast<int64_t>(H) * W <= INT32_MAX / 2, "%s: frame of %dx%d too large", fn, H, W);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "%s: current device is not sm_90", fn);
+    return VQB_OK;
+}
+
+inline dim3 clip_grid(int HW, int images) {
+    const int bx = (HW + 255) / 256;
+    return dim3(static_cast<unsigned>(bx < 64 ? bx : 64), static_cast<unsigned>(images));
+}
+
+template <typename In>
+int clip_to_frames(const char* fn, const In* x, void* y, int B, int C, int T, int H, int W, int Cpad, int pad,
+                   const int* frames, int Tsel, const float* shift, const float* inv_scale, void* stream) {
+    const int rc = check_clip_args(fn, x, y, B, C, T, H, W, Cpad, pad, frames, Tsel, shift, inv_scale,
+                                   static_cast<int64_t>(B) * Tsel);
+    if (rc != VQB_OK) return rc;
+    clip_to_frames_kernel<In><<<clip_grid(H * W, B * Tsel), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        x, static_cast<__nv_bfloat16*>(y), C, T, H * W, W, Cpad, pad, frames, Tsel, shift, inv_scale);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+int frames_to_clip(const char* fn, const void* g, float* gx, int B, int C, int T, int H, int W, int Cpad, int pad,
+                   const int* frames, int Tsel, const float* inv_scale, void* stream) {
+    const int rc = check_clip_args(fn, g, gx, B, C, T, H, W, Cpad, pad, frames, Tsel, inv_scale, inv_scale,
+                                   static_cast<int64_t>(B) * T);
+    if (rc != VQB_OK) return rc;
+    frames_to_clip_kernel<<<clip_grid(H * W, B * T), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(g), gx, C, T, H * W, W, Cpad, pad, frames, Tsel, inv_scale);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
 }  // namespace vqb
 
 using namespace vqb;
@@ -849,6 +968,44 @@ int vqb_nhwc_to_nchw(const void* g, float* gx, int N, int C, int H, int W, int C
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
+}
+
+int vqb_ncthw_frames_to_nhwc_pad(const float* x, void* y, int B, int C, int T, int H, int W, int Cpad, int pad,
+                                 const int* frames, int Tsel, const float* shift, const float* inv_scale,
+                                 void* stream) {
+    return clip_to_frames("vqb_ncthw_frames_to_nhwc_pad", x, y, B, C, T, H, W, Cpad, pad, frames, Tsel, shift,
+                          inv_scale, stream);
+}
+
+int vqb_ncthw_frames_to_nhwc_pad_bf16(const void* x, void* y, int B, int C, int T, int H, int W, int Cpad, int pad,
+                                      const int* frames, int Tsel, const float* shift, const float* inv_scale,
+                                      void* stream) {
+    return clip_to_frames("vqb_ncthw_frames_to_nhwc_pad_bf16", static_cast<const __nv_bfloat16*>(x), y, B, C, T, H, W,
+                          Cpad, pad, frames, Tsel, shift, inv_scale, stream);
+}
+
+int vqb_ncthw_frames_to_nhwc(const float* x, void* y, int B, int C, int T, int H, int W, int Cpad, const int* frames,
+                             int Tsel, const float* shift, const float* inv_scale, void* stream) {
+    return clip_to_frames("vqb_ncthw_frames_to_nhwc", x, y, B, C, T, H, W, Cpad, 0, frames, Tsel, shift, inv_scale,
+                          stream);
+}
+
+int vqb_ncthw_frames_to_nhwc_bf16(const void* x, void* y, int B, int C, int T, int H, int W, int Cpad,
+                                  const int* frames, int Tsel, const float* shift, const float* inv_scale,
+                                  void* stream) {
+    return clip_to_frames("vqb_ncthw_frames_to_nhwc_bf16", static_cast<const __nv_bfloat16*>(x), y, B, C, T, H, W,
+                          Cpad, 0, frames, Tsel, shift, inv_scale, stream);
+}
+
+int vqb_nhwc_pad_frames_to_ncthw(const void* g, float* gx, int B, int C, int T, int H, int W, int Cpad, int pad,
+                                 const int* frames, int Tsel, const float* inv_scale, void* stream) {
+    return frames_to_clip("vqb_nhwc_pad_frames_to_ncthw", g, gx, B, C, T, H, W, Cpad, pad, frames, Tsel, inv_scale,
+                          stream);
+}
+
+int vqb_nhwc_frames_to_ncthw(const void* g, float* gx, int B, int C, int T, int H, int W, int Cpad, const int* frames,
+                             int Tsel, const float* inv_scale, void* stream) {
+    return frames_to_clip("vqb_nhwc_frames_to_ncthw", g, gx, B, C, T, H, W, Cpad, 0, frames, Tsel, inv_scale, stream);
 }
 
 // GroupNorm(+SiLU) forward. ws: >= N*C*2 doubles (zeroed here); mr: [N][G][2] floats (mean, rstd) kept for backward.

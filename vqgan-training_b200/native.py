@@ -156,6 +156,12 @@ def load():
         "vqb_attn_bwd_hd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
         "vqb_gauss_reparam_bwd": (i32, [vp, vp, vp, vp, i32, i32, i64, vp]),
         "vqb_gn_silu_apply": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+        "vqb_ncthw_frames_to_nhwc_pad": (i32, [vp, vp] + [i32] * 7 + [vp, i32, vp, vp, vp]),
+        "vqb_ncthw_frames_to_nhwc_pad_bf16": (i32, [vp, vp] + [i32] * 7 + [vp, i32, vp, vp, vp]),
+        "vqb_ncthw_frames_to_nhwc": (i32, [vp, vp] + [i32] * 6 + [vp, i32, vp, vp, vp]),
+        "vqb_ncthw_frames_to_nhwc_bf16": (i32, [vp, vp] + [i32] * 6 + [vp, i32, vp, vp, vp]),
+        "vqb_nhwc_pad_frames_to_ncthw": (i32, [vp, vp] + [i32] * 7 + [vp, i32, vp, vp]),
+        "vqb_nhwc_frames_to_ncthw": (i32, [vp, vp] + [i32] * 6 + [vp, i32, vp, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)

@@ -536,6 +536,83 @@ def to_nhwc(x, shift=None, inv_scale=None, frame=False):
     return ToNHWC.apply(x, shift, inv_scale, frame)
 
 
+def clip_frame_selection(frames, B: int, T: int):
+    """Host-side check of a frame selection for [B, C, T, H, W] clips: None (every frame) or a [B, T'] integer tensor or
+    nested list holding T' distinct frames in [0, T) per clip. -> (int32 CPU tensor [B*T'] or None, T'). Raises before
+    anything is launched; a CUDA tensor is copied to the host (one synchronisation)."""
+    if frames is None:
+        return None, T
+    f = torch.as_tensor(frames)
+    if f.is_floating_point() or f.is_complex() or f.dtype == torch.bool:
+        raise ValueError(f"frames must be integers, got {f.dtype}")
+    if f.dim() != 2 or f.shape[0] != B or not 1 <= f.shape[1] <= T:
+        raise ValueError(f"frames must be a [B, T'] selection with B = {B} and 1 <= T' <= T = {T}, got shape "
+                         f"{tuple(f.shape)}")
+    f = f.to("cpu", torch.int64)
+    if bool(((f < 0) | (f >= T)).any()):
+        raise ValueError(f"frames holds a frame outside [0, {T}): {f.tolist()}")
+    if bool((f.sort(dim=1).values.diff(dim=1) == 0).any()):
+        raise ValueError(f"frames holds a duplicate frame within a clip: {f.tolist()}")
+    return f.to(torch.int32).reshape(-1), f.shape[1]
+
+
+class ClipToFrames(torch.autograd.Function):
+    """The clip counterpart of ToNHWC: [B,C,T,H,W] fp32 or bf16 -> [B*T', H, W, Cp] bf16 (zero-framed [B*T', H+2, W+2,
+    Cp] with frame=True), frames folded into the batch in (b, t) order, optional (x - shift) * inv_scale. `sel` is the
+    int32 CPU [B*T'] selection of clip_frame_selection (None: every frame). The clip is read through its strides, with
+    no folded copy; each image is bit-identical to ToNHWC of that frame. Backward: the NCTHW fp32 clip gradient
+    (* inv_scale), exact zeros in frames outside the selection, from one launch."""
+
+    @staticmethod
+    def forward(ctx, x, shift, inv_scale, frame, sel, Tsel):
+        require_cuda(x)
+        x = x.detach()
+        bf16 = x.dtype == torch.bfloat16
+        if bf16:
+            x = x.contiguous()
+        elif x.dtype != torch.float32 or not x.is_contiguous():
+            x = x.float().contiguous()
+        B, C, T, H, W = x.shape
+        Cp = plans.cpad(C)
+        # pinned + non_blocking: a pageable host-to-device copy would wait for the stream to drain
+        sel_dev = None if sel is None else sel.pin_memory().to(x.device, non_blocking=True)
+        if frame:
+            y = alloc_framed(B * Tsel, H, W, Cp, x.device)
+            fn = _L().vqb_ncthw_frames_to_nhwc_pad_bf16 if bf16 else _L().vqb_ncthw_frames_to_nhwc_pad
+            check(fn(ptr(x), ptr(y), B, C, T, H, W, Cp, 1, ptr(sel_dev), Tsel, ptr(shift), ptr(inv_scale),
+                     stream_ptr()), "ncthw_frames_to_nhwc_pad")
+        else:
+            y = torch.empty(B * Tsel, H, W, Cp, device=x.device, dtype=torch.bfloat16)
+            fn = _L().vqb_ncthw_frames_to_nhwc_bf16 if bf16 else _L().vqb_ncthw_frames_to_nhwc
+            check(fn(ptr(x), ptr(y), B, C, T, H, W, Cp, ptr(sel_dev), Tsel, ptr(shift), ptr(inv_scale), stream_ptr()),
+                  "ncthw_frames_to_nhwc")
+        ctx.shape = (B, C, T, H, W, Cp, Tsel)
+        ctx.inv_scale, ctx.frame, ctx.sel_dev = inv_scale, frame, sel_dev
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        B, C, T, H, W, Cp, Tsel = ctx.shape
+        gy = gy.contiguous()
+        gx = torch.empty(B, C, T, H, W, device=gy.device, dtype=torch.float32)
+        if ctx.frame:
+            check(_L().vqb_nhwc_pad_frames_to_ncthw(ptr(gy), ptr(gx), B, C, T, H, W, Cp, 1, ptr(ctx.sel_dev), Tsel,
+                                                    ptr(ctx.inv_scale), stream_ptr()), "nhwc_pad_frames_to_ncthw")
+        else:
+            check(_L().vqb_nhwc_frames_to_ncthw(ptr(gy), ptr(gx), B, C, T, H, W, Cp, ptr(ctx.sel_dev), Tsel,
+                                                ptr(ctx.inv_scale), stream_ptr()), "nhwc_frames_to_ncthw")
+        return gx, None, None, None, None, None
+
+
+def clip_to_frames(x, shift=None, inv_scale=None, frame=False, frames=None):
+    """[B,C,T,H,W] clip -> per-frame NHWC bf16 images of the selected frames (ClipToFrames; frames as in
+    clip_frame_selection)."""
+    if x.dim() != 5:
+        raise ValueError(f"clip_to_frames: expected a [B, C, T, H, W] clip, got shape {tuple(x.shape)}")
+    sel, Tsel = clip_frame_selection(frames, x.shape[0], x.shape[2])
+    return ClipToFrames.apply(x, shift, inv_scale, frame, sel, Tsel)
+
+
 class ToNCHW(torch.autograd.Function):
     """[N,H,W,Cp] bf16 -> [N,C,H,W] fp32, or bf16 for a bf16 module (module-boundary output when a caller wants the
     reference layout)."""

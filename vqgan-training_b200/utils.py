@@ -140,17 +140,21 @@ class LPIPS(nn.Module):
                                    "(tests / benchmarks only)") from e
         self.load_state_dict(data, strict=False)
 
-    def forward(self, input, target):
+    def forward(self, input, target, *, frames=None):
+        """input, target: [B, 3, H, W] images -> [B, 1, 1, 1]; or [B, 3, T, H, W] clips -> [B*T', 1, 1, 1], the metric of
+        every selected frame, frames folded into the batch in (b, t) order. frames: optional [B, T'] integer tensor or
+        list of distinct frames per clip (default: every frame, T' = T)."""
         from ae import Act
 
+        clip = _clip_selection(input, frames, target)
         # SURVEY.md fact 5: the reference never calls .eval() on LPIPS, so its nn.Dropout(0.5) in front of every lin layer
         # is live during training. Honoured here: in train mode (and when the lin layer has a Dropout) the fused tail
         # applies a counter-based keep mask; the per-call seed comes from torch's CPU generator (torch.manual_seed
         # reproducible, no device sync). `dropout_seeds` (test hook) pins the five per-layer seeds.
         fat = ops.fat_conv_enabled()
-        a0 = Act(self.scaling_layer.to_act(input, fat), 3, framed=fat)
+        a0 = Act(self.scaling_layer.to_act(input, fat, clip), 3, framed=fat)
         with torch.no_grad():
-            a1 = Act(self.scaling_layer.to_act(target, fat), 3, framed=fat)
+            a1 = Act(self.scaling_layer.to_act(target, fat, clip), 3, framed=fat)
             outs1 = self.net.forward_acts(a1)
         outs0 = self.net.forward_acts(a0)
         lins = [self.lin0, self.lin1, self.lin2, self.lin3, self.lin4]
@@ -176,12 +180,32 @@ class ScalingLayer(nn.Module):
     def forward(self, inp):
         return (inp - self.shift) / self.scale
 
-    def to_act(self, inp, frame=False):
+    def to_act(self, inp, frame=False, clip=None):
         """(inp - shift) / scale fused into the NCHW fp32 -> NHWC bf16 layout kernel (optionally zero-framed for the
-        fat-pixel first VGG conv)."""
+        fat-pixel first VGG conv). clip: the checked (selection, T') of _clip_selection for a [B, 3, T, H, W] clip,
+        whose selected frames become the batch (ops.ClipToFrames)."""
         shift = self.shift.reshape(-1).float().contiguous()
         inv = (1.0 / self.scale.reshape(-1).float()).contiguous()
+        if clip is not None:
+            return ops.ClipToFrames.apply(inp, shift, inv, frame, *clip)
         return ops.to_nhwc(inp, shift, inv, frame)
+
+
+def _clip_selection(x, frames, target=None):
+    """Checks a call of LPIPS / PatchDiscriminator before anything is launched. A 4-D image batch -> None (the image
+    path). A [B, 3, T, H, W] clip (and a target of the same shape) -> (int32 CPU selection or None, T') from
+    ops.clip_frame_selection."""
+    if x.dim() != 5:
+        if frames is not None:
+            raise ValueError(f"frames= selects frames of [B, 3, T, H, W] clips; the input has shape {tuple(x.shape)}")
+        if target is not None and target.dim() == 5:
+            raise ValueError(f"target shape {tuple(target.shape)} differs from input shape {tuple(x.shape)}")
+        return None
+    if x.shape[1] != 3:
+        raise ValueError(f"expected a [B, 3, T, H, W] clip, got {x.shape[1]} channels (shape {tuple(x.shape)})")
+    if target is not None and tuple(target.shape) != tuple(x.shape):
+        raise ValueError(f"target shape {tuple(target.shape)} differs from input shape {tuple(x.shape)}")
+    return ops.clip_frame_selection(frames, x.shape[0], x.shape[2])
 
 
 class NetLinLayer(nn.Module):
@@ -299,11 +323,14 @@ class PatchDiscriminator(nn.Module):
             return seq[2].forward_act(h, input_is_relu=True, nchw_out=True)
         return seq[0].forward_act(feat, input_is_relu=True, nchw_out=True)
 
-    def forward(self, x):
+    def forward(self, x, *, frames=None):
+        """x: [B, 3, H, W] images -> logits [B, (H/16)(W/16)]; or a [B, 3, T, H, W] clip -> [B*T', (H/16)(W/16)], the
+        logits of every selected frame, frames folded into the batch in (b, t) order (frames as in LPIPS.forward)."""
         from ae import Act
 
+        clip = _clip_selection(x, frames)
         fat = ops.fat_conv_enabled()
-        a = Act(self.scaling_layer.to_act(x, fat), 3, framed=fat)
+        a = Act(self.scaling_layer.to_act(x, fat, clip), 3, framed=fat)
         f1 = _run_trunk_slice(self.slice1[0], a, False)
         f2 = _run_trunk_slice(self.slice2[0], f1, False)
         f3 = _run_trunk_slice(self.slice3[0], f2, False)
