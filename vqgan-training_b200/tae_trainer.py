@@ -1,4 +1,5 @@
-"""Training step of the video autoencoder (tae.TVAE) against the image autoencoder's loss stack, applied per frame.
+"""Training of the video autoencoder (tae.TVAE) against the image autoencoder's loss stack, applied per frame, in one
+process or data-parallel over ranks.
 
 The reference has no video trainer. A clip [B, 3, T, H, W] is scored by the reference image losses on its frames folded
 into the batch in (b, t) order (DESIGN.md section 7): LPIPS and the PatchGAN discriminator see the B*T' frames of the
@@ -9,25 +10,39 @@ utils.PatchDiscriminator take the clip directly (ops.ClipToFrames): no folded co
                       disc_type="hinge", use_lecam=True, perceptual_frames=4, lr_vae=1e-4, lr_disc=2e-4)
     out = tr.step(clip)        # clip: fp32 [B, 3, T, H, W] on cuda
 
-Out of scope: DDP / NCCL (one process), CUDA-graph capture (the step runs eagerly), the latent flip and crop
-augmentations, and HR decoding of the image Trainer.
+Data parallel, as the image Trainer (vae_trainer.py): when a process group of more than one rank exists, each rank
+trains on its own clips and the TVAE and discriminator gradients are averaged over ranks (one all-reduce each on the
+flat gradient buffer of FlatAdamW), the LeCam anchors are fed by rank-averaged logits, GradNorm divides by the
+rank-averaged norm, and LPIPS scores with rank 0's weights. The torchrun entry point (`train_video`, below):
+
+    torchrun --nproc_per_node=8 tae_trainer.py --vae_ch 64 --clip_frames 16 --resolution 256 --batch_size 1 \
+        --do_ganloss --disc_type hinge --use_lecam True --perceptual_frames 4
+
+Out of scope: CUDA-graph capture (the step runs eagerly), the latent flip and crop augmentations, HR decoding of the
+image Trainer, and real video datasets (the entry point trains on a seeded synthetic clip stream).
 """
 from __future__ import annotations
 
+import logging
 import os
 import sys
+import time
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 if _HERE not in sys.path:
     sys.path.insert(0, _HERE)
 
+import click
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F
 
 import tae
 from flat import FlatAdamW
-from vae_trainer import gan_disc_loss, gradnorm, vae_loss_function
+from utils import broadcast_module_state
+from vae_trainer import (FlatAllReduceDDP, SyntheticLoader, _dist_on, avg_scalar_over_nodes, cleanup,
+                         cosine_with_warmup, gan_disc_loss, gradnorm, vae_loss_function)
 
 
 def fold_frames(x: torch.Tensor, frames=None) -> torch.Tensor:
@@ -43,7 +58,7 @@ def fold_frames(x: torch.Tensor, frames=None) -> torch.Tensor:
 
 
 class VideoTrainer:
-    """Trainer._step_body (vae_trainer.py) on frames folded into the batch, in one process.
+    """Trainer._step_body (vae_trainer.py) on frames folded into the batch, in one process or data-parallel.
 
     vae: a float32 tae.TVAE; it is opted into training here (tae.enable_training; `recompute` passes through).
     lpips: utils.LPIPS (frozen; its train/eval mode is kept as given), or None for the MSE-only baseline, whose
@@ -61,6 +76,20 @@ class VideoTrainer:
       3. LPIPS(gradnorm(decz), clip).mean() over the selected frames, vae_loss_function(clip, gradnorm(decz, 0.001),
          z) with z the NCTHW encoder output (0.1 * mean(z^2)), and the generator loss of D on gradnorm(decz, 1.0) with
          D's parameters frozen for that pass; one backward, AdamW step of the TVAE.
+
+    Data parallel (a process group of more than one rank exists when the trainer is built): the constructor wraps the
+    TVAE and the discriminator in vae_trainer.FlatAllReduceDDP, which broadcasts rank 0's parameters and buffers,
+    before FlatAdamW re-homes them into its flat buffers, so every cached bf16 operand is packed from rank 0's weights;
+    LPIPS is broadcast from rank 0 too. Each step then averages D's flat gradient over ranks before D's AdamW step and
+    the TVAE's before the TVAE's (in place, in FlatAdamW's gradient buffer; VQB_DDP_OVERLAP as in Trainer), feeds the
+    LeCam anchors with rank-averaged logits (avg_scalar_over_nodes), and GradNorm divides by the rank-averaged norm.
+    Every rank therefore holds the same weights, optimizer moments and anchors after every step. Without a process
+    group the wrappers issue no collective and the step is the single-process step.
+    `vae` and `disc` are the unwrapped modules.
+
+    Randomness: the frame selection comes from torch's CPU generator and ε from torch's CUDA generator, so ranks draw
+    their own frames and noise when their caller seeds them per rank (train_video: torch.manual_seed(seed + rank));
+    their weights agree anyway because of the constructor broadcast.
     """
 
     def __init__(self, vae: nn.Module, lpips, discriminator=None, *, disc_type="hinge", use_lecam=False,
@@ -74,14 +103,23 @@ class VideoTrainer:
         self.vae = tae.enable_training(vae, recompute=recompute)
         self.lpips, self.disc = lpips, discriminator
         self.disc_type, self.use_lecam, self.perceptual_frames = disc_type, use_lecam, perceptual_frames
+        # the order of Trainer.__init__: broadcast (in the wrappers' constructors) before FlatAdamW re-homes the weights
+        self._vae_dp = FlatAllReduceDDP(vae)
+        self._disc_dp = None
+        if discriminator is not None:
+            discriminator.requires_grad_(True)
+            self._disc_dp = FlatAllReduceDDP(discriminator)
         self.optimizer_G = FlatAdamW([{"params": [p for p in vae.parameters() if p.requires_grad], "lr": lr_vae}],
                                      weight_decay=1e-3, betas=(0.9, 0.95))
+        self._vae_dp.attach_store(self.optimizer_G.store)
         self.optimizer_D = None
         device = next(vae.parameters()).device
         if discriminator is not None:
-            discriminator.requires_grad_(True)
             self.optimizer_D = FlatAdamW([{"params": list(discriminator.parameters()), "lr": lr_disc}],
                                          weight_decay=1e-3, betas=(0.9, 0.95))
+            self._disc_dp.attach_store(self.optimizer_D.store)
+        if lpips is not None:
+            broadcast_module_state(lpips)  # frozen, not wrapped: every rank scores with rank 0's weights
         self.lecam_loss_weight, self.lecam_beta = 0.1, 0.9
         self.lecam_anchor_real_logits = torch.zeros((), device=device)
         self.lecam_anchor_fake_logits = torch.zeros((), device=device)
@@ -101,14 +139,18 @@ class VideoTrainer:
             raise ValueError(f"expected a [B, 3, T, H, W] clip, got shape {tuple(clip.shape)}")
         sel = self.draw_frames(clip.shape[0], clip.shape[2])
         self.last_frames = sel
-        disc = self.disc
-        decz, z = self.vae(clip)
+        vae_dp, disc_dp = self._vae_dp, self._disc_dp
+        disc = None if disc_dp is None else disc_dp.module
+        decz, z = vae_dp.module(clip)
 
         out = {}
         if disc is not None:
             real_preds = disc(clip, frames=sel)
             fake_preds = disc(decz.detach(), frames=sel)
             d_loss, avg_real_logits, avg_fake_logits, disc_acc = gan_disc_loss(real_preds, fake_preds, self.disc_type)
+            if _dist_on():  # one process uses the local means as they are: no copy is launched
+                avg_real_logits = avg_scalar_over_nodes(avg_real_logits, clip.device)
+                avg_fake_logits = avg_scalar_over_nodes(avg_fake_logits, clip.device)
             self.lecam_anchor_real_logits.mul_(self.lecam_beta).add_(avg_real_logits, alpha=1 - self.lecam_beta)
             self.lecam_anchor_fake_logits.mul_(self.lecam_beta).add_(avg_fake_logits, alpha=1 - self.lecam_beta)
             total_d_loss = d_loss.mean()
@@ -121,6 +163,7 @@ class VideoTrainer:
                 total_d_loss = total_d_loss + lecam_loss * self.lecam_loss_weight
             self.optimizer_D.zero_grad(set_to_none=True)
             total_d_loss.backward()
+            disc_dp.allreduce_grads()
             self.optimizer_D.step()
             out.update(avg_real_logits=avg_real_logits, avg_fake_logits=avg_fake_logits, disc_acc=disc_acc,
                        lecam_loss=lecam_loss_item)
@@ -148,7 +191,118 @@ class VideoTrainer:
 
         self.optimizer_G.zero_grad(set_to_none=True)
         overall_vae_loss.backward()
+        vae_dp.allreduce_grads()
         self.optimizer_G.step()
         out.update(overall_vae_loss=overall_vae_loss.detach(), perceptual_loss=recon_loss.detach(),
                    loss_data=loss_data, z=z.detach(), reconstructed=decz.detach())
         return out
+
+
+@click.command()
+@click.option("--batch_size", type=int, default=1, help="Clips per rank per step")
+@click.option("--clip_frames", type=int, default=16, help="Frames per clip")
+@click.option("--resolution", type=int, default=256, help="Height and width of the clips")
+@click.option("--perceptual_frames", type=int, default=None,
+              help="Frames per clip the losses score each step, drawn at random (default: every frame)")
+@click.option("--do_ganloss", is_flag=True, help="Whether to use GAN loss")
+@click.option("--disc_type", type=click.Choice(["bce", "hinge"]), default="bce", help="Discriminator type")
+@click.option("--use_lecam", type=bool, default=False, help="Whether to use Lecam")
+@click.option("--no_lpips", is_flag=True, help="Train with the MSE of the scored frames instead of LPIPS")
+@click.option("--recompute", is_flag=True, help="Recompute ResnetBlock activations in the backward (less memory)")
+@click.option("--learning_rate_vae", type=float, default=1e-4, help="Learning rate for the TVAE")
+@click.option("--learning_rate_disc", type=float, default=2e-4, help="Learning rate for discriminator")
+@click.option("--vae_ch", type=int, default=64, help="Base channel size for the TVAE")
+@click.option("--vae_ch_mult", type=str, default="1,2,4,4", help="Channel multipliers for the TVAE")
+@click.option("--vae_num_res_blocks", type=int, default=2, help="Number of residual blocks for the TVAE")
+@click.option("--vae_z_channels", type=int, default=16, help="Number of latent channels for the TVAE")
+@click.option("--max_steps", type=int, default=1000, help="Maximum number of steps to train for")
+@click.option("--evaluate_every_n_steps", type=int, default=250, help="Save a checkpoint every n steps")
+@click.option("--load_path", type=str, default=None, help="TVAE state_dict to start from (a saved checkpoint)")
+@click.option("--run_name", type=str, default="run", help="Checkpoints are saved under ./ckpt/<run_name>/")
+@click.option("--seed", type=int, default=42, help="Rank r seeds torch with seed + r (frame selection and noise)")
+def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam, no_lpips,
+                recompute, learning_rate_vae, learning_rate_disc, vae_ch, vae_ch_mult, vae_num_res_blocks,
+                vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed):
+    """Trains tae.TVAE on a seeded synthetic clip stream, data-parallel under torchrun (one process per GPU, NCCL) or in
+    one process. Rank 0 logs every 5 steps and saves the TVAE's state_dict every --evaluate_every_n_steps steps."""
+    # arguments are checked before anything touches a device
+    if perceptual_frames is not None and not 1 <= perceptual_frames <= clip_frames:
+        raise click.BadParameter(f"must be between 1 and --clip_frames ({clip_frames}), got {perceptual_frames}",
+                                 param_hint="--perceptual_frames")
+    try:
+        ch_mult = [int(c) for c in vae_ch_mult.split(",")]
+    except ValueError:
+        raise click.BadParameter(f"expected comma-separated integers, got {vae_ch_mult!r}", param_hint="--vae_ch_mult")
+    div = 2 ** (len(ch_mult) - 1)
+    if clip_frames % div or resolution % div:
+        raise click.BadParameter(f"--clip_frames ({clip_frames}) and --resolution ({resolution}) must be multiples of "
+                                 f"{div} for {len(ch_mult)} levels", param_hint="--vae_ch_mult")
+
+    assert torch.cuda.is_available(), "CUDA is required"
+    rank = int(os.environ.get("RANK", "0"))
+    device = torch.device(f"cuda:{int(os.environ.get('LOCAL_RANK', '0'))}")
+    torch.cuda.set_device(device)
+    if "RANK" in os.environ:
+        dist.init_process_group(backend="nccl", device_id=device)
+    try:
+        _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type,
+                     use_lecam, no_lpips, recompute, learning_rate_vae, learning_rate_disc, vae_ch, ch_mult,
+                     vae_num_res_blocks, vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed)
+    finally:
+        cleanup()
+
+
+def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam,
+                 no_lpips, recompute, learning_rate_vae, learning_rate_disc, vae_ch, ch_mult, vae_num_res_blocks,
+                 vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed):
+    import utils
+
+    torch.manual_seed(seed + rank)  # each rank draws its own frames and noise (the weights come from rank 0)
+    torch.cuda.manual_seed(seed + rank)
+    vae = tae.TVAE(resolution=resolution, in_channels=3, ch=vae_ch, out_ch=3, ch_mult=ch_mult,
+                   num_res_blocks=vae_num_res_blocks, z_channels=vae_z_channels)
+    if load_path is not None:
+        vae.load_state_dict(torch.load(load_path, map_location="cpu"), strict=True)
+    lpips = None if no_lpips else utils.LPIPS().to(device)  # train mode: dropout live, as train_ddp runs it
+    disc = utils.PatchDiscriminator().to(device) if do_ganloss else None
+    tr = VideoTrainer(vae.to(device), lpips, disc, disc_type=disc_type, use_lecam=use_lecam,
+                      perceptual_frames=perceptual_frames, lr_vae=learning_rate_vae, lr_disc=learning_rate_disc,
+                      recompute=recompute)
+    lr_scheduler = cosine_with_warmup(tr.optimizer_G, 200, max_steps)
+    clips = iter(SyntheticLoader(batch_size, resolution, frames=clip_frames))  # seed 42 + rank
+
+    logger = logging.getLogger(__name__)
+    logger.setLevel(logging.INFO)
+    if rank == 0:
+        handler = logging.StreamHandler()
+        handler.setFormatter(logging.Formatter("%(asctime)s - %(name)s - %(levelname)s - %(message)s"))
+        logger.addHandler(handler)
+    t_log, step_log = time.time(), 0
+    for step in range(max_steps):
+        out = tr.step(next(clips)[0].to(device, non_blocking=True))
+        lr_scheduler.step()
+        if rank == 0 and step % 5 == 0:  # the only host synchronisations of the loop
+            ld = out["loss_data"]
+            items = [("overall_vae_loss", out["overall_vae_loss"]), ("perceptual_loss", out["perceptual_loss"]),
+                     ("kl_loss", ld["kl_loss"])]
+            if do_ganloss:
+                items += [("d_loss", out["d_loss"]), ("gan_loss", out["g_gan_loss"]),
+                          ("avg_real_logits", out["avg_real_logits"]), ("avg_fake_logits", out["avg_fake_logits"]),
+                          ("discriminator_accuracy", out["disc_acc"]), ("lecam_loss", out["lecam_loss"]),
+                          ("lecam_anchor_real_logits", tr.lecam_anchor_real_logits),
+                          ("lecam_anchor_fake_logits", tr.lecam_anchor_fake_logits)]
+            items = [(k, float(v)) for k, v in items]
+            now = time.time()
+            items.append(("ms_per_step", (now - t_log) * 1e3 / (step + 1 - step_log)))
+            t_log, step_log = now, step + 1
+            logger.info(f"step {step} - " + "\n\t".join(f"{k}: {v:.4f}" for k, v in items))
+        if evaluate_every_n_steps > 0 and (step + 1) % evaluate_every_n_steps == 0 and rank == 0:
+            os.makedirs(f"./ckpt/{run_name}", exist_ok=True)
+            ck = f"./ckpt/{run_name}/tvae_step_{step + 1}.pt"
+            torch.save({k: v.detach().cpu() for k, v in tr.vae.state_dict().items()}, ck)
+            logger.info(f"Saved checkpoint to {ck}")
+
+
+if __name__ == "__main__":
+    # Example: torchrun --nproc_per_node=8 tae_trainer.py --vae_ch 64 --clip_frames 16 --resolution 256 --batch_size 1
+    train_video()

@@ -134,12 +134,14 @@ def create_dataloader(url, batch_size, num_workers, do_shuffle=True, just_resize
 
 
 class SyntheticLoader:
-    """Endless seeded stream of pinned host batches in [-1, 1) (the range of Normalize(.5,.5), vae_trainer.py:98)."""
+    """Endless seeded stream of pinned host batches in [-1, 1) (the range of Normalize(.5,.5), vae_trainer.py:98):
+    images [B, 3, R, R], or clips [B, 3, frames, R, R] for the video trainer (tae_trainer.py)."""
 
-    def __init__(self, batch_size, resolution, seed=None, n_distinct=4):
+    def __init__(self, batch_size, resolution, seed=None, n_distinct=4, frames=None):
         rank = int(os.environ.get("RANK", "0"))
         g = torch.Generator().manual_seed(42 + rank if seed is None else seed)
-        self.batches = [(torch.rand(batch_size, 3, resolution, resolution, generator=g) * 2 - 1) for _ in range(n_distinct)]
+        shape = (batch_size, 3) + (() if frames is None else (frames,)) + (resolution, resolution)
+        self.batches = [(torch.rand(shape, generator=g) * 2 - 1) for _ in range(n_distinct)]
         if torch.cuda.is_available():
             self.batches = [b.pin_memory() for b in self.batches]
 
