@@ -149,6 +149,9 @@ int vqb_nhwc_to_nchw_pad(const void* g, float* gx, int N, int C, int H, int W, i
  * FP32GroupNorm (+ swish) forward / backward on bf16 NHWC: 32 groups, biased variance, eps inside the sqrt, fp32
  * statistics (ae.py:41-53 + ae.py:13-14). mr = [N][G][2] (mean, rstd) kept for the backward.
  * fwd workspace ws: N*C*2 doubles; bwd workspace ws: N*C*2 + N*G*2 floats. `add` (optional) is summed into dx.
+ * `silu` is an activation code: 0 none, 1 swish, 2 LeakyReLU(0.2) (the 3-D PatchGAN of tae_disc.py; its backward
+ * recomputes the pre-activation from x, gamma, beta and mr as the swish backward does); any other value is VQB_EINVAL.
+ * vqb_gn_silu_apply takes codes 0 and 1 only (its caller is the ResnetBlock recompute).
  */
 int vqb_gn_silu_fwd(const void* x, void* y, const float* gamma, const float* beta, float* mr, double* ws, int N,
                     int HW, int C, int G, float eps, int silu, void* stream);
@@ -164,6 +167,15 @@ int vqb_gn_silu_apply(const void* x, void* y, const float* gamma, const float* b
 int vqb_gn_silu_bwd(const void* x, const void* dy, const void* add, void* dx, const float* gamma, const float* beta,
                     const float* mr, float* dgamma, float* dbeta, float* ws, int N, int HW, int C, int G, int silu,
                     float* dx_colsum, void* stream);
+
+/*
+ * LeakyReLU(0.2) over n bf16 elements (an NTHWC activation; n a positive multiple of 8, pointers 16-byte aligned):
+ * forward y = x > 0 ? x : 0.2 x (rounded once); backward dx = dy * (y > 0 ? 1 : 0.2), gated on the saved forward
+ * output (y > 0 exactly where x > 0, so the gradient at 0 is torch's). Validates (VQB_EINVAL), then VQB_ENODEVICE
+ * without an sm_90 device. The conv_in activation of tae_disc.PatchDiscriminator3D.
+ */
+int vqb_leaky_relu_fwd(const void* x, void* y, int64_t n, void* stream);
+int vqb_leaky_relu_bwd(const void* y, const void* dy, void* dx, int64_t n, void* stream);
 
 /*
  * Wavelet front-end of the encoder (--use_wavelet; utils.py:229-247): F.pad(x, 2) + grouped 6x6 stride-2 conv with the

@@ -4,8 +4,13 @@ MSE only (lpips=None), + LPIPS, and + LPIPS + PatchGAN (hinge, LeCam), each on e
 in plain PyTorch (oracle/tae_oracle.py, oracle/clip_loss_oracle.py: F.conv3d / F.conv2d VGG16 with cuDNN) with
 torch.optim.AdamW.
 
+With --clip-disc it times instead the 3-D PatchGAN leg: LPIPS + clip discriminator (tae_disc.PatchDiscriminator3D,
+--clip-disc-ch 64, --clip-disc-layers 3, hinge + LeCam) on every frame, without and with the per-frame PatchGAN, and
+the peer with the oracle module (oracle/clip_disc_oracle.py, F.conv3d on cuDNN); it also prints the discriminator's
+FLOPs counted from the plan shapes.
+
 Usage: python tools/tae_loss_bench.py [--frames 16] [--res 256] [--ch 64] [--batch 1] [--perceptual-frames 4]
-           [--steps 5] [--warmup 2] [--skip-peer]
+           [--steps 5] [--warmup 2] [--skip-peer] [--clip-disc [--clip-disc-ch 64] [--clip-disc-layers 3]]
 
 Prints one JSON line per arm with ms/step, frames/s (clip frames through the autoencoder per second) and peak
 allocated memory, plus the card's name and power limit read in the same run. LPIPS / PatchD weights are torchvision's
@@ -26,6 +31,7 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
 from infer_bench import card, timed  # noqa: E402
+from oracle import clip_disc_oracle as CDO  # noqa: E402
 from oracle import clip_loss_oracle as CO  # noqa: E402
 from oracle import loss_oracle as LO  # noqa: E402
 from oracle import tae_oracle as TO  # noqa: E402
@@ -43,9 +49,13 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--skip-peer", action="store_true")
+    ap.add_argument("--clip-disc", action="store_true")
+    ap.add_argument("--clip-disc-ch", type=int, default=64)
+    ap.add_argument("--clip-disc-layers", type=int, default=3)
     a = ap.parse_args()
 
     import tae
+    import tae_disc
     import tae_trainer
     import utils
 
@@ -58,6 +68,8 @@ def main():
     tsd = tae.TVAE(**cfg.kwargs()).state_dict()
     lsd = utils.LPIPS().state_dict()
     psd = utils.PatchDiscriminator().state_dict()
+    nl = a.clip_disc_layers
+    csd = CDO.PatchDiscriminator3D(ch=a.clip_disc_ch, n_layers=nl).state_dict()
 
     def report(arm, stack, k, ms, peak):
         print(json.dumps({"arm": arm, "loss": stack, "perceptual_frames": k or T, "frames": T, "res": a.res,
@@ -68,20 +80,24 @@ def main():
     def native(stack, k):
         m = tae.TVAE(**cfg.kwargs())
         m.load_state_dict(tsd)
-        lp = pd = None
+        lp = pd = d3 = None
         if stack != "mse":
             lp = utils.LPIPS()
             lp.load_state_dict(lsd)
             lp = lp.cuda().eval()
-        if stack == "lpips+gan":
+        if stack.startswith("lpips+gan"):
             pd = utils.PatchDiscriminator()
             pd.load_state_dict(psd)
             pd = pd.cuda()
+        if stack.endswith("clipd"):
+            d3 = tae_disc.PatchDiscriminator3D(ch=a.clip_disc_ch, n_layers=nl)
+            d3.load_state_dict(csd)
+            d3 = d3.cuda()
         tr = tae_trainer.VideoTrainer(m.cuda(), lp, pd, disc_type="hinge", use_lecam=True, perceptual_frames=k,
-                                      lr_vae=1e-4, lr_disc=2e-4)
+                                      lr_vae=1e-4, lr_disc=2e-4, clip_discriminator=d3, lr_clip_disc=2e-4)
         ms, peak, _ = timed(lambda: tr.step(x), a.steps, a.warmup)
         report("native", stack, k, ms, peak)
-        del tr, m, lp, pd
+        del tr, m, lp, pd, d3
         torch.cuda.empty_cache()
 
     def peer(stack, k):
@@ -92,6 +108,20 @@ def main():
         opt_g = torch.optim.AdamW(tp.values(), lr=1e-4, **kw)
         opt_d = torch.optim.AdamW([v for v in dp.values() if v.requires_grad], lr=2e-4, **kw)
         anchors = [torch.zeros((), device="cuda"), torch.zeros((), device="cuda")]
+        cp = {n: v.cuda().clone().requires_grad_(True) for n, v in csd.items()}
+        opt_c = torch.optim.AdamW(cp.values(), lr=2e-4, **kw)
+        canchors = [torch.zeros((), device="cuda"), torch.zeros((), device="cuda")]
+
+        def d_step(fwd, params, opt, anc, fake_in):
+            with ac():
+                real, fake = fwd(params, x).float(), fwd(params, fake_in).float()
+            d_loss = (F.relu(1 - real).mean() + F.relu(1 + fake).mean()) * 0.5
+            anc[0] = 0.9 * anc[0] + 0.1 * real.detach().mean()
+            anc[1] = 0.9 * anc[1] + 0.1 * fake.detach().mean()
+            d_loss = d_loss + 0.1 * LO.lecam_loss(real, fake, anc[0], anc[1])
+            opt.zero_grad(set_to_none=True)
+            d_loss.backward()
+            opt.step()
         ac = lambda: torch.autocast("cuda", dtype=torch.bfloat16)  # noqa: E731
 
         def step():
@@ -100,26 +130,24 @@ def main():
                 z = TO.encoder_forward(tp, x, cfg)
                 decz = TO.decoder_forward(tp, TO.reg(z, torch.randn_like(z[:, :cfg.z_channels])), cfg)
             decz, z = decz.float(), z.float()
-            if stack == "lpips+gan":
-                with ac():
-                    real = CO.patchd_clip(dp, x, sel).float()
-                    fake = CO.patchd_clip(dp, decz.detach(), sel).float()
-                d_loss = (F.relu(1 - real).mean() + F.relu(1 + fake).mean()) * 0.5
-                anchors[0] = 0.9 * anchors[0] + 0.1 * real.detach().mean()
-                anchors[1] = 0.9 * anchors[1] + 0.1 * fake.detach().mean()
-                d_loss = d_loss + 0.1 * LO.lecam_loss(real, fake, anchors[0], anchors[1])
-                opt_d.zero_grad(set_to_none=True)
-                d_loss.backward()
-                opt_d.step()
+            patchd = lambda p, v: CO.patchd_clip(p, v, sel)  # noqa: E731
+            clipd = lambda p, v: CDO.forward(p, v, nl)  # noqa: E731
+            if stack.startswith("lpips+gan"):
+                d_step(patchd, dp, opt_d, anchors, decz.detach())
+            if stack.endswith("clipd"):
+                d_step(clipd, cp, opt_c, canchors, decz.detach())
             with ac():
                 if stack == "mse":
                     rec = F.mse_loss(CO.fold_frames(decz, sel), CO.fold_frames(x, sel))
                 else:
                     rec = CO.lpips_clip(ls, LO.gradnorm(decz), x, sel).float().mean()
                 loss = rec + 0.1 * z.pow(2).mean()
-                if stack == "lpips+gan":
+                if stack.startswith("lpips+gan"):
                     frozen = {n: v.detach() for n, v in dp.items()}
                     loss = loss - CO.patchd_clip(frozen, LO.gradnorm(decz, 1.0), sel).float().mean()
+                if stack.endswith("clipd"):
+                    frozen = {n: v.detach() for n, v in cp.items()}
+                    loss = loss - CDO.forward(frozen, LO.gradnorm(decz, 1.0), nl).float().mean()
             opt_g.zero_grad(set_to_none=True)
             loss.backward()
             opt_g.step()
@@ -127,9 +155,22 @@ def main():
 
         ms, peak, _ = timed(step, a.steps, a.warmup)
         report("bf16-autocast eager peer", stack, k, ms, peak)
-        del tp, dp, opt_g, opt_d
+        del tp, dp, opt_g, opt_d, cp, opt_c
         torch.cuda.empty_cache()
 
+    if a.clip_disc:
+        # one forward of D3 per clip; a step runs it 3 times (real, fake, G pass), the weight gradient twice (real and
+        # fake of the D step) and the data gradient of every conv but conv_in twice and of all convs once (G pass)
+        fwd = CDO.flops(a.clip_disc_ch, nl, N, T, a.res, a.res)
+        first = CDO.flops(a.clip_disc_ch, nl, N, T, a.res, a.res, only_first=True)
+        print(json.dumps({"clip_disc": {"ch": a.clip_disc_ch, "n_layers": nl, "fwd_gflop": round(fwd / 1e9, 2),
+                                        "step_gflop": round((3 * fwd + 2 * fwd + 2 * (fwd - first) + fwd) / 1e9, 2)},
+                          "gpu": info}), flush=True)
+        for stack in ("lpips+clipd", "lpips+gan+clipd"):
+            native(stack, None)
+            if not a.skip_peer:
+                peer(stack, None)
+        return
     for k in (None, a.perceptual_frames):
         for stack in STACKS:
             native(stack, k)

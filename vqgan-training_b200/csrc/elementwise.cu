@@ -1,5 +1,5 @@
 // HBM-bound kernels of the VAE path: layout conversion at the module boundary, weight packing,
-// fused GroupNorm(+SiLU) forward / backward, bias gradients, wgrad split
+// fused GroupNorm(+SiLU / LeakyReLU) forward / backward, LeakyReLU, bias gradients, wgrad split
 // reduction. All activations are NHWC bf16 with C % 8 == 0; every thread moves 16-byte vectors and
 // owns a FIXED 8-channel slot (its channel vector index never changes while it strides over pixels),
 // so per-channel affine terms / reductions stay in registers.
@@ -44,6 +44,11 @@ __device__ __forceinline__ float sigmoidf_(float x) {
     return fmaf(0.5f, t, 0.5f);
 #endif
 }
+
+// activation codes of the GroupNorm entry points (their `int silu` argument)
+constexpr int kActNone = 0, kActLeaky = 2;  // 1: swish
+// negative slope of the LeakyReLU of the 3-D PatchGAN discriminator (tae_disc.py)
+constexpr float kLeakySlope = 0.2f;
 
 // tanh for the swish derivative: MUFU.TANH by default; with -DVQB_EXACT_SIGMOID the exact form through exp
 __device__ __forceinline__ float tanh_fast(float x) {
@@ -332,6 +337,8 @@ __global__ void gn_finalize_f32_kernel(const float* __restrict__ sums, float* __
     mr[i * 2 + 1] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
 }
 
+// LEAKY: y = LeakyReLU(0.2)(u) (activation code 2); otherwise `silu` selects swish (1) or none (0)
+template <bool LEAKY>
 __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                 const float* __restrict__ mr, const float* __restrict__ gamma,
                                 const float* __restrict__ beta, int HW, int C, int G, int pix_per_chunk, int silu) {
@@ -362,7 +369,7 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 float u = fmaf(a[j], f[j], b[j]);
-                f[j] = silu ? u * sigmoidf_(u) : u;
+                f[j] = LEAKY ? (u > 0.f ? u : kLeakySlope * u) : (silu ? u * sigmoidf_(u) : u);
             }
             store8(y + base + static_cast<int64_t>(p + k * R) * C, f);
         }
@@ -373,14 +380,16 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             float u = fmaf(a[j], f[j], b[j]);
-            f[j] = silu ? u * sigmoidf_(u) : u;
+            f[j] = LEAKY ? (u > 0.f ? u : kLeakySlope * u) : (silu ? u * sigmoidf_(u) : u);
         }
         store8(y + base + static_cast<int64_t>(p) * C, f);
     }
 }
 
 // ------------------------------------------------------------------ GroupNorm backward
-// per-(n,channel) sums of du and du*xhat, du = dy * silu'(u), u = xhat*gamma + beta
+// per-(n,channel) sums of du and du*xhat, du = dy * act'(u), u = xhat*gamma + beta (LEAKY: act'(u) = u > 0 ? 1 : 0.2,
+// with u > 0 tested on the recomputed h = u/2)
+template <bool LEAKY>
 __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
                                      const float* __restrict__ mr, const float* __restrict__ gamma,
                                      const float* __restrict__ beta, float* __restrict__ cs /* [N][C][2] */, int HW,
@@ -428,7 +437,9 @@ __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, const 
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     float du2 = 2.f * d[j];
-                    if (silu) {
+                    if (LEAKY) {
+                        if (!(fmaf(f[j], a2[j], b2[j]) > 0.f)) du2 *= kLeakySlope;
+                    } else if (silu) {
                         const float h = fmaf(f[j], a2[j], b2[j]);
                         const float t = tanh_fast(h);
                         const float r = fmaf(-h, t, h + 1.f);
@@ -478,7 +489,7 @@ __global__ void gn_bwd_finalize_kernel(const float* __restrict__ cs, const float
 }
 
 // dx = rstd * (du*gamma - S1 - xhat*S2) (+ add)
-template <bool ADD, int U>
+template <bool ADD, int U, bool LEAKY>
 __global__ void __launch_bounds__(256, 2)
 gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
                     const __nv_bfloat16* __restrict__ add, __nv_bfloat16* __restrict__ dx,
@@ -532,7 +543,9 @@ gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     float du2 = 2.f * d[j];
-                    if (silu) {
+                    if (LEAKY) {
+                        if (!(fmaf(f[j], a2[j], b2[j]) > 0.f)) du2 *= kLeakySlope;
+                    } else if (silu) {
                         const float h = fmaf(f[j], a2[j], b2[j]);
                         const float t = tanh_fast(h);
                         const float rr = fmaf(-h, t, h + 1.f);
@@ -555,6 +568,34 @@ gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __
     if (colsum) {
         __syncthreads();
         for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(&colsum[i], sm[i]);
+    }
+}
+
+// ------------------------------------------------------------------ LeakyReLU(0.2)
+// y = x > 0 ? x : 0.2 x over n/8 16-byte vectors of bf16 (one rounding of 0.2 x)
+__global__ void leaky_relu_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
+                                      int64_t nvec) {
+    for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < nvec;
+         i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        float f[8];
+        cvt8(ldg16(x + i * 8), f);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] = f[j] > 0.f ? f[j] : kLeakySlope * f[j];
+        store8(y + i * 8, f);
+    }
+}
+
+// dx = dy * (y > 0 ? 1 : 0.2), gated on the saved output: the slope is positive, so y > 0 exactly where x > 0
+__global__ void leaky_relu_bwd_kernel(const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ dy,
+                                      __nv_bfloat16* __restrict__ dx, int64_t nvec) {
+    for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < nvec;
+         i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        float fy[8], f[8];
+        cvt8(ldg16(y + i * 8), fy);
+        cvt8(ldg16(dy + i * 8), f);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] = fy[j] > 0.f ? f[j] : kLeakySlope * f[j];
+        store8(dx + i * 8, f);
     }
 }
 
@@ -1008,11 +1049,30 @@ int vqb_nhwc_frames_to_ncthw(const void* g, float* gx, int B, int C, int T, int 
     return frames_to_clip("vqb_nhwc_frames_to_ncthw", g, gx, B, C, T, H, W, Cpad, 0, frames, Tsel, inv_scale, stream);
 }
 
+// the apply pass of every GroupNorm forward entry point; act: a validated activation code
+static void launch_gn_apply(const void* x, void* y, const float* mr, const float* gamma, const float* beta, int N,
+                            int HW, int C, int G, int act, cudaStream_t st) {
+    int chunks, ppc;
+    const int T = cv_threads(C);
+    const auto* xb = static_cast<const __nv_bfloat16*>(x);
+    auto* yb = static_cast<__nv_bfloat16*>(y);
+    if (act == kActLeaky) {
+        cv_grid(HW, C, N, gn_apply_kernel<true>, 0, chunks, ppc);
+        gn_apply_kernel<true><<<dim3(chunks, N), T, 0, st>>>(xb, yb, mr, gamma, beta, HW, C, G, ppc, act);
+    } else {
+        cv_grid(HW, C, N, gn_apply_kernel<false>, 0, chunks, ppc);
+        gn_apply_kernel<false><<<dim3(chunks, N), T, 0, st>>>(xb, yb, mr, gamma, beta, HW, C, G, ppc, act);
+    }
+}
+
 // GroupNorm(+SiLU) forward. ws: >= N*C*2 doubles (zeroed here); mr: [N][G][2] floats (mean, rstd) kept for backward.
 int vqb_gn_silu_fwd(const void* x, void* y, const float* gamma, const float* beta, float* mr, double* ws, int N,
                     int HW, int C, int G, float eps, int silu, void* stream) {
     VQB_CHECK(x && y && gamma && beta && mr && ws, "vqb_gn_silu_fwd: null pointer");
     VQB_CHECK(C % 8 == 0 && C % G == 0 && C <= 2048, "vqb_gn_silu_fwd: C=%d G=%d unsupported", C, G);
+    VQB_CHECK(silu >= kActNone && silu <= kActLeaky,
+              "vqb_gn_silu_fwd: activation code %d unsupported (0 none, 1 swish, 2 LeakyReLU(0.2))", silu);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_gn_silu_fwd: current device is not sm_90");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     VQB_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * 2 * N * C, st));
     int chunks, ppc;
@@ -1022,10 +1082,7 @@ int vqb_gn_silu_fwd(const void* x, void* y, const float* gamma, const float* bet
     gn_stats_kernel<<<dim3(chunks, N), T, stats_smem, st>>>(static_cast<const __nv_bfloat16*>(x), ws, HW, C,
                                                                         ppc);
     gn_finalize_kernel<<<(N * G + 127) / 128, 128, 0, st>>>(ws, mr, N, C, G, HW, eps);
-    cv_grid(HW, C, N, gn_apply_kernel, 0, chunks, ppc);
-    gn_apply_kernel<<<dim3(chunks, N), T, 0, st>>>(static_cast<const __nv_bfloat16*>(x),
-                                                   static_cast<__nv_bfloat16*>(y), mr, gamma, beta, HW, C, G, ppc,
-                                                   silu);
+    launch_gn_apply(x, y, mr, gamma, beta, N, HW, C, G, silu, st);
     VQB_CUDA(cudaGetLastError());
     count_launch(3);
     return VQB_OK;
@@ -1043,11 +1100,7 @@ int vqb_gn_silu_apply(const void* x, void* y, const float* gamma, const float* b
                     reinterpret_cast<uintptr_t>(mr)) & 3u) == 0,
               "vqb_gn_silu_apply: x and y must be 16-byte aligned, gamma, beta and mr 4-byte aligned");
     if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_gn_silu_apply: current device is not sm_90");
-    int chunks, ppc;
-    const int T = cv_threads(C);
-    cv_grid(HW, C, N, gn_apply_kernel, 0, chunks, ppc);
-    gn_apply_kernel<<<dim3(chunks, N), T, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), mr, gamma, beta, HW, C, G, ppc, silu);
+    launch_gn_apply(x, y, mr, gamma, beta, N, HW, C, G, silu, static_cast<cudaStream_t>(stream));
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
@@ -1059,14 +1112,12 @@ int vqb_gn_silu_fwd_pre(const void* x, void* y, const float* gamma, const float*
                         int N, int HW, int C, int G, float eps, int silu, void* stream) {
     VQB_CHECK(x && y && gamma && beta && mr && chsums, "vqb_gn_silu_fwd_pre: null pointer");
     VQB_CHECK(C % 8 == 0 && C % G == 0 && C <= 2048, "vqb_gn_silu_fwd_pre: C=%d G=%d unsupported", C, G);
+    VQB_CHECK(silu >= kActNone && silu <= kActLeaky,
+              "vqb_gn_silu_fwd_pre: activation code %d unsupported (0 none, 1 swish, 2 LeakyReLU(0.2))", silu);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_gn_silu_fwd_pre: current device is not sm_90");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     gn_finalize_f32_kernel<<<(N * G + 127) / 128, 128, 0, st>>>(chsums, mr, N, C, G, HW, eps);
-    int chunks, ppc;
-    const int T = cv_threads(C);
-    cv_grid(HW, C, N, gn_apply_kernel, 0, chunks, ppc);
-    gn_apply_kernel<<<dim3(chunks, N), T, 0, st>>>(static_cast<const __nv_bfloat16*>(x),
-                                                   static_cast<__nv_bfloat16*>(y), mr, gamma, beta, HW, C, G, ppc,
-                                                   silu);
+    launch_gn_apply(x, y, mr, gamma, beta, N, HW, C, G, silu, st);
     VQB_CUDA(cudaGetLastError());
     count_launch(2);
     return VQB_OK;
@@ -1080,35 +1131,85 @@ int vqb_gn_silu_bwd(const void* x, const void* dy, const void* add, void* dx, co
                     float* dx_colsum, void* stream) {
     VQB_CHECK(x && dy && dx && gamma && beta && mr && dgamma && dbeta && ws, "vqb_gn_silu_bwd: null pointer");
     VQB_CHECK(C % 8 == 0 && C % G == 0 && C <= 2048, "vqb_gn_silu_bwd: C=%d G=%d unsupported", C, G);
+    VQB_CHECK(silu >= kActNone && silu <= kActLeaky,
+              "vqb_gn_silu_bwd: activation code %d unsupported (0 none, 1 swish, 2 LeakyReLU(0.2))", silu);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_gn_silu_bwd: current device is not sm_90");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int chunks, ppc;
     const int T = cv_threads(C);
     float* cs = ws;                                      // [N][C][2]
     float* gsum = ws + static_cast<int64_t>(N) * C * 2;  // [N][G][2]
     VQB_CUDA(cudaMemsetAsync(cs, 0, sizeof(float) * 2 * N * C, st));
-    cv_grid(HW, C, N, gn_bwd_reduce_kernel, 2 * C * sizeof(float), chunks, ppc);
-    gn_bwd_reduce_kernel<<<dim3(chunks, N), T, 2 * C * sizeof(float), st>>>(
-        static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(dy), mr, gamma, beta, cs, HW, C, G,
-        ppc, silu);
+    const bool leaky = silu == kActLeaky;
+    const auto* xb = static_cast<const __nv_bfloat16*>(x);
+    const auto* dyb = static_cast<const __nv_bfloat16*>(dy);
+    if (leaky) {
+        cv_grid(HW, C, N, gn_bwd_reduce_kernel<true>, 2 * C * sizeof(float), chunks, ppc);
+        gn_bwd_reduce_kernel<true><<<dim3(chunks, N), T, 2 * C * sizeof(float), st>>>(xb, dyb, mr, gamma, beta, cs,
+                                                                                       HW, C, G, ppc, silu);
+    } else {
+        cv_grid(HW, C, N, gn_bwd_reduce_kernel<false>, 2 * C * sizeof(float), chunks, ppc);
+        gn_bwd_reduce_kernel<false><<<dim3(chunks, N), T, 2 * C * sizeof(float), st>>>(xb, dyb, mr, gamma, beta, cs,
+                                                                                        HW, C, G, ppc, silu);
+    }
     count_launch();
     const int fin = (N * G > C ? N * G : C);
     gn_bwd_finalize_kernel<<<(fin + 127) / 128, 128, 0, st>>>(cs, gamma, gsum, dgamma, dbeta, N, C, G, HW);
     const size_t cs_smem = dx_colsum ? C * sizeof(float) : 0;
     if (dx_colsum) VQB_CUDA(cudaMemsetAsync(dx_colsum, 0, sizeof(float) * C, st));
-    if (add) {
-        cv_grid(HW, C, N, gn_bwd_apply_kernel<true, 2>, cs_smem, chunks, ppc);
-        gn_bwd_apply_kernel<true, 2><<<dim3(chunks, N), T, cs_smem, st>>>(
-            static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(dy),
-            static_cast<const __nv_bfloat16*>(add), static_cast<__nv_bfloat16*>(dx), mr, gsum, gamma, beta, HW, C, G,
-            ppc, silu, dx_colsum);
+    const auto* ab = static_cast<const __nv_bfloat16*>(add);
+    auto* dxb = static_cast<__nv_bfloat16*>(dx);
+    if (add && leaky) {
+        cv_grid(HW, C, N, gn_bwd_apply_kernel<true, 2, true>, cs_smem, chunks, ppc);
+        gn_bwd_apply_kernel<true, 2, true><<<dim3(chunks, N), T, cs_smem, st>>>(
+            xb, dyb, ab, dxb, mr, gsum, gamma, beta, HW, C, G, ppc, silu, dx_colsum);
+    } else if (add) {
+        cv_grid(HW, C, N, gn_bwd_apply_kernel<true, 2, false>, cs_smem, chunks, ppc);
+        gn_bwd_apply_kernel<true, 2, false><<<dim3(chunks, N), T, cs_smem, st>>>(
+            xb, dyb, ab, dxb, mr, gsum, gamma, beta, HW, C, G, ppc, silu, dx_colsum);
+    } else if (leaky) {
+        cv_grid(HW, C, N, gn_bwd_apply_kernel<false, 3, true>, cs_smem, chunks, ppc);
+        gn_bwd_apply_kernel<false, 3, true><<<dim3(chunks, N), T, cs_smem, st>>>(
+            xb, dyb, nullptr, dxb, mr, gsum, gamma, beta, HW, C, G, ppc, silu, dx_colsum);
     } else {
-        cv_grid(HW, C, N, gn_bwd_apply_kernel<false, 3>, cs_smem, chunks, ppc);
-        gn_bwd_apply_kernel<false, 3><<<dim3(chunks, N), T, cs_smem, st>>>(
-            static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(dy), nullptr,
-            static_cast<__nv_bfloat16*>(dx), mr, gsum, gamma, beta, HW, C, G, ppc, silu, dx_colsum);
+        cv_grid(HW, C, N, gn_bwd_apply_kernel<false, 3, false>, cs_smem, chunks, ppc);
+        gn_bwd_apply_kernel<false, 3, false><<<dim3(chunks, N), T, cs_smem, st>>>(
+            xb, dyb, nullptr, dxb, mr, gsum, gamma, beta, HW, C, G, ppc, silu, dx_colsum);
     }
     VQB_CUDA(cudaGetLastError());
     count_launch(2);
+    return VQB_OK;
+}
+
+static int leaky_check(const char* fn, const void* a, const void* b, const void* c, int64_t n) {
+    VQB_CHECK(a && b && c, "%s: null pointer", fn);
+    VQB_CHECK(n > 0 && n % 8 == 0, "%s: n=%lld must be a positive multiple of 8", fn, static_cast<long long>(n));
+    VQB_CHECK(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) &
+               15u) == 0,
+              "%s: pointers must be 16-byte aligned", fn);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "%s: current device is not sm_90", fn);
+    return VQB_OK;
+}
+
+// LeakyReLU(0.2) forward over n bf16 elements (see include/vqb200.h)
+int vqb_leaky_relu_fwd(const void* x, void* y, int64_t n, void* stream) {
+    const int rc = leaky_check("vqb_leaky_relu_fwd", x, y, y, n);
+    if (rc != VQB_OK) return rc;
+    leaky_relu_fwd_kernel<<<gs_blocks(n / 8, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), n / 8);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+int vqb_leaky_relu_bwd(const void* y, const void* dy, void* dx, int64_t n, void* stream) {
+    const int rc = leaky_check("vqb_leaky_relu_bwd", y, dy, dx, n);
+    if (rc != VQB_OK) return rc;
+    leaky_relu_bwd_kernel<<<gs_blocks(n / 8, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(y), static_cast<const __nv_bfloat16*>(dy), static_cast<__nv_bfloat16*>(dx),
+        n / 8);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
     return VQB_OK;
 }
 

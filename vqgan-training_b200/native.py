@@ -162,6 +162,8 @@ def load():
         "vqb_ncthw_frames_to_nhwc_bf16": (i32, [vp, vp] + [i32] * 6 + [vp, i32, vp, vp, vp]),
         "vqb_nhwc_pad_frames_to_ncthw": (i32, [vp, vp] + [i32] * 7 + [vp, i32, vp, vp]),
         "vqb_nhwc_frames_to_ncthw": (i32, [vp, vp] + [i32] * 6 + [vp, i32, vp, vp]),
+        "vqb_leaky_relu_fwd": (i32, [vp, vp, i64, vp]),
+        "vqb_leaky_relu_bwd": (i32, [vp, vp, vp, i64, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)

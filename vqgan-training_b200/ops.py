@@ -901,9 +901,14 @@ def upsample_conv(x, weight, bias, cache, want_stats=False):
     return UpConvFn.apply(x, weight, bias, cache, False)
 
 
+# activation codes of the GroupNorm kernels (the `silu` argument of vqb_gn_silu_*): a bool passes as 0 / 1
+ACT_NONE, ACT_SWISH, ACT_LEAKY = 0, 1, 2
+
+
 class GroupNormSiLUFn(torch.autograd.Function):
     """FP32GroupNorm (32 groups, eps 1e-6, biased variance, fp32 statistics; ae.py:41-53) fused with swish
     (ae.py:13-14): one statistics pass + one apply pass over bf16 NHWC, instead of cast/GN/cast/sigmoid/mul.
+    `silu` is an activation code (ACT_NONE, ACT_SWISH, ACT_LEAKY = LeakyReLU(0.2)); False / True are codes 0 / 1.
 
     with_skip=True additionally returns the input itself as a second output (the ResnetBlock skip connection): the
     gradient arriving through that output is summed into dx INSIDE the backward apply kernel instead of by a separate
@@ -943,7 +948,7 @@ def gn_silu_fwd(x, gamma, beta, groups, eps, silu):
     ga, be = gamma.detach().float(), beta.detach().float()
     ws = torch.empty(N * C * 2, device=x.device, dtype=torch.float64)
     check(_L().vqb_gn_silu_fwd(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), ptr(ws), N, H * W, C, groups, eps,
-                               1 if silu else 0, stream_ptr()), "gn_silu_fwd")
+                               int(silu), stream_ptr()), "gn_silu_fwd")
     return y, mr
 
 
@@ -955,7 +960,7 @@ def gn_silu_fwd_pre(x, gamma, beta, chsums, groups, eps, silu):
     mr = torch.empty(N, groups, 2, device=x.device, dtype=torch.float32)
     ga, be = gamma.detach().float(), beta.detach().float()
     check(_L().vqb_gn_silu_fwd_pre(ptr(x), ptr(y), ptr(ga), ptr(be), ptr(mr), ptr(chsums), N, H * W, C, groups, eps,
-                                   1 if silu else 0, stream_ptr()), "gn_silu_fwd_pre")
+                                   int(silu), stream_ptr()), "gn_silu_fwd_pre")
     return y, mr
 
 
@@ -982,7 +987,7 @@ def gn_silu_bwd(x, gy, gskip, gamma, beta, mr, groups, silu):
     ga, be = gamma.detach().float(), beta.detach().float()
     cs = torch.empty(C, device=x.device, dtype=torch.float32)
     check(_L().vqb_gn_silu_bwd(ptr(x), ptr(gy), ptr(add), ptr(dx), ptr(ga), ptr(be), ptr(mr), ptr(dg), ptr(db),
-                               ptr(ws), N, H * W, C, groups, 1 if silu else 0, ptr(cs), stream_ptr()), "gn_silu_bwd")
+                               ptr(ws), N, H * W, C, groups, int(silu), ptr(cs), stream_ptr()), "gn_silu_bwd")
     _dx_colsum_slot[0] = (dx, dx._version, cs)
     return dx, dg, db
 
@@ -1247,11 +1252,43 @@ def upsample_conv3d(x, weight, bias, cache):
 
 
 def group_norm_silu3d(x, gamma, beta, groups=32, eps=1e-6, silu=True):
-    """GroupNorm(+swish) over the T*H*W voxels of an NTHWC activation (tae.py:63-71): the 2-D kernels on the
-    [N][T*H][W][C] view, deterministic statistics pass."""
+    """GroupNorm(+activation) over the T*H*W voxels of an NTHWC activation (tae.py:63-71): the 2-D kernels on the
+    [N][T*H][W][C] view, deterministic statistics pass. silu: an activation code (ACT_*) or a bool (swish or none)."""
     N, T, H, W, C = x.shape
     y = group_norm_silu(x.reshape(N, T * H, W, C), gamma, beta, groups, eps, silu)
     return y.view(N, T, H, W, C)
+
+
+def _leaky_relu(x):
+    x = x.contiguous()
+    y = torch.empty_like(x)
+    check(_L().vqb_leaky_relu_fwd(ptr(x), ptr(y), x.numel(), stream_ptr()), "leaky_relu_fwd")
+    return y
+
+
+class LeakyReLUFn(torch.autograd.Function):
+    """LeakyReLU(0.2) of a bf16 NTHWC activation (vqb_leaky_relu_fwd / _bwd): the conv_in activation of
+    tae_disc.PatchDiscriminator3D, which has no GroupNorm to fuse it into. The backward is gated on the saved output."""
+
+    @staticmethod
+    def forward(ctx, x):
+        y = _leaky_relu(x)
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        (y,) = ctx.saved_tensors
+        gy = gy.contiguous()
+        dx = torch.empty_like(y)
+        check(_L().vqb_leaky_relu_bwd(ptr(y), ptr(gy), ptr(dx), y.numel(), stream_ptr()), "leaky_relu_bwd")
+        return dx
+
+
+def leaky_relu(x):
+    """LeakyReLU(0.2) of a bf16 NTHWC activation: the autograd function when grad is enabled, else one kernel."""
+    require_cuda(x)
+    return LeakyReLUFn.apply(x) if torch.is_grad_enabled() else _leaky_relu(x)
 
 
 # head dimensions of the native attention forward and backward (vqb_attn_fwd_hd / vqb_attn_bwd_hd)

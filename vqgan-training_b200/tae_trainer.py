@@ -10,13 +10,18 @@ utils.PatchDiscriminator take the clip directly (ops.ClipToFrames): no folded co
                       disc_type="hinge", use_lecam=True, perceptual_frames=4, lr_vae=1e-4, lr_disc=2e-4)
     out = tr.step(clip)        # clip: fp32 [B, 3, T, H, W] on cuda
 
+Every term above scores frames one at a time. `clip_discriminator=tae_disc.PatchDiscriminator3D(...)` adds a 3-D
+PatchGAN that convolves over time as well: its D step runs after the per-frame one on the whole clip (real: the clip,
+fake: the detached reconstruction; `perceptual_frames` does not apply), with the same loss type and LeCam but its own
+anchors and AdamW, and the G pass adds its generator loss on gradnorm(decz, clip_disc_weight).
+
 Data parallel, as the image Trainer (vae_trainer.py): when a process group of more than one rank exists, each rank
 trains on its own clips and the TVAE and discriminator gradients are averaged over ranks (one all-reduce each on the
 flat gradient buffer of FlatAdamW), the LeCam anchors are fed by rank-averaged logits, GradNorm divides by the
 rank-averaged norm, and LPIPS scores with rank 0's weights. The torchrun entry point (`train_video`, below):
 
     torchrun --nproc_per_node=8 tae_trainer.py --vae_ch 64 --clip_frames 16 --resolution 256 --batch_size 1 \
-        --do_ganloss --disc_type hinge --use_lecam True --perceptual_frames 4
+        --do_ganloss --disc_type hinge --use_lecam True --perceptual_frames 4 [--do_clip_ganloss]
 
 Out of scope: CUDA-graph capture (the step runs eagerly), the latent flip and crop augmentations, HR decoding of the
 image Trainer, and real video datasets (the entry point trains on a seeded synthetic clip stream).
@@ -69,23 +74,28 @@ class VideoTrainer:
         runs reproducible); LPIPS, the MSE term and both GAN passes use that one selection. None: every frame.
     lr_vae, lr_disc: learning rates of the fused AdamW (vqb_adamw_flat; betas (0.9, 0.95), weight decay 1e-3, as in
         Trainer) over the TVAE and the discriminator.
+    clip_discriminator: tae_disc.PatchDiscriminator3D or None; it is opted into training here. lr_clip_disc: its AdamW
+        learning rate (same betas and weight decay); clip_disc_weight: the GradNorm weight of its generator pass.
 
     step(clip) per step:
       1. decz, z = vae(clip) (the reparameterisation draws its noise from torch's CUDA generator);
       2. with a discriminator: D on real and detached fake frames, hinge / BCE loss (+ LeCam), AdamW step of D;
-      3. LPIPS(gradnorm(decz), clip).mean() over the selected frames, vae_loss_function(clip, gradnorm(decz, 0.001),
-         z) with z the NCTHW encoder output (0.1 * mean(z^2)), and the generator loss of D on gradnorm(decz, 1.0) with
-         D's parameters frozen for that pass; one backward, AdamW step of the TVAE.
+      3. with a clip discriminator D3: D3 on the whole real and detached fake clip, the same loss (+ LeCam with the
+         clip_lecam_anchor_{real,fake}_logits), AdamW step of D3;
+      4. LPIPS(gradnorm(decz), clip).mean() over the selected frames, vae_loss_function(clip, gradnorm(decz, 0.001),
+         z) with z the NCTHW encoder output (0.1 * mean(z^2)), the generator loss of D on gradnorm(decz, 1.0) with
+         D's parameters frozen for that pass, and that of D3 on gradnorm(decz, clip_disc_weight) with D3 frozen; one
+         backward, AdamW step of the TVAE.
 
     Data parallel (a process group of more than one rank exists when the trainer is built): the constructor wraps the
-    TVAE and the discriminator in vae_trainer.FlatAllReduceDDP, which broadcasts rank 0's parameters and buffers,
+    TVAE and the discriminators in vae_trainer.FlatAllReduceDDP, which broadcasts rank 0's parameters and buffers,
     before FlatAdamW re-homes them into its flat buffers, so every cached bf16 operand is packed from rank 0's weights;
-    LPIPS is broadcast from rank 0 too. Each step then averages D's flat gradient over ranks before D's AdamW step and
-    the TVAE's before the TVAE's (in place, in FlatAdamW's gradient buffer; VQB_DDP_OVERLAP as in Trainer), feeds the
+    LPIPS is broadcast from rank 0 too. Each step then averages D's (and D3's) flat gradient over ranks before its AdamW
+    step and the TVAE's before the TVAE's (in place, in FlatAdamW's gradient buffer; VQB_DDP_OVERLAP as in Trainer), feeds the
     LeCam anchors with rank-averaged logits (avg_scalar_over_nodes), and GradNorm divides by the rank-averaged norm.
     Every rank therefore holds the same weights, optimizer moments and anchors after every step. Without a process
     group the wrappers issue no collective and the step is the single-process step.
-    `vae` and `disc` are the unwrapped modules.
+    `vae`, `disc` and `clip_disc` are the unwrapped modules.
 
     Randomness: the frame selection comes from torch's CPU generator and ε from torch's CUDA generator, so ranks draw
     their own frames and noise when their caller seeds them per rank (train_video: torch.manual_seed(seed + rank));
@@ -93,11 +103,14 @@ class VideoTrainer:
     """
 
     def __init__(self, vae: nn.Module, lpips, discriminator=None, *, disc_type="hinge", use_lecam=False,
-                 perceptual_frames=None, lr_vae, lr_disc=None, recompute=False):
+                 perceptual_frames=None, lr_vae, lr_disc=None, recompute=False, clip_discriminator=None,
+                 lr_clip_disc=None, clip_disc_weight=1.0):
         if disc_type not in ("hinge", "bce"):
             raise ValueError(f"unknown disc_type {disc_type!r}")
         if discriminator is not None and lr_disc is None:
             raise ValueError("lr_disc is required with a discriminator")
+        if clip_discriminator is not None and lr_clip_disc is None:
+            raise ValueError("lr_clip_disc is required with a clip discriminator")
         if perceptual_frames is not None and perceptual_frames < 1:
             raise ValueError(f"perceptual_frames must be >= 1, got {perceptual_frames}")
         self.vae = tae.enable_training(vae, recompute=recompute)
@@ -124,6 +137,16 @@ class VideoTrainer:
         self.lecam_anchor_real_logits = torch.zeros((), device=device)
         self.lecam_anchor_fake_logits = torch.zeros((), device=device)
         self.last_frames = None
+        self.clip_disc, self._clip_disc_dp, self.optimizer_clip_D = None, None, None
+        if clip_discriminator is not None:
+            self.clip_disc = tae.enable_training(clip_discriminator.requires_grad_(True))
+            self._clip_disc_dp = FlatAllReduceDDP(clip_discriminator)  # broadcast before FlatAdamW re-homes the weights
+            self.optimizer_clip_D = FlatAdamW([{"params": list(clip_discriminator.parameters()), "lr": lr_clip_disc}],
+                                              weight_decay=1e-3, betas=(0.9, 0.95))
+            self._clip_disc_dp.attach_store(self.optimizer_clip_D.store)
+            self.clip_disc_weight = clip_disc_weight
+            self.clip_lecam_anchor_real_logits = torch.zeros((), device=device)
+            self.clip_lecam_anchor_fake_logits = torch.zeros((), device=device)
 
     def draw_frames(self, B: int, T: int):
         """[B, k] int64 CPU tensor of k distinct frames per clip (torch's CPU generator), or None for every frame."""
@@ -167,6 +190,8 @@ class VideoTrainer:
             self.optimizer_D.step()
             out.update(avg_real_logits=avg_real_logits, avg_fake_logits=avg_fake_logits, disc_acc=disc_acc,
                        lecam_loss=lecam_loss_item)
+        if self.clip_disc is not None:
+            out.update(self._clip_disc_step(clip, decz))
 
         if self.lpips is not None:
             recon_loss = self.lpips(gradnorm(decz), clip, frames=sel).mean()
@@ -188,6 +213,19 @@ class VideoTrainer:
                 g_gan_loss = -fake_preds.mean()
             overall_vae_loss = overall_vae_loss + g_gan_loss
             out["g_gan_loss"] = g_gan_loss.detach()
+        if self.clip_disc is not None:
+            clip_disc = self.clip_disc
+            clip_disc.requires_grad_(False)  # the G pass needs D3's data gradient only
+            try:
+                fake_preds = clip_disc(gradnorm(decz, weight=self.clip_disc_weight))
+            finally:
+                clip_disc.requires_grad_(True)
+            if self.disc_type == "bce":
+                clip_g_gan_loss = F.binary_cross_entropy_with_logits(fake_preds, torch.ones_like(fake_preds))
+            else:
+                clip_g_gan_loss = -fake_preds.mean()
+            overall_vae_loss = overall_vae_loss + clip_g_gan_loss
+            out["clip_g_gan_loss"] = clip_g_gan_loss.detach()
 
         self.optimizer_G.zero_grad(set_to_none=True)
         overall_vae_loss.backward()
@@ -195,6 +233,33 @@ class VideoTrainer:
         self.optimizer_G.step()
         out.update(overall_vae_loss=overall_vae_loss.detach(), perceptual_loss=recon_loss.detach(),
                    loss_data=loss_data, z=z.detach(), reconstructed=decz.detach())
+        return out
+
+    def _clip_disc_step(self, clip, decz) -> dict:
+        """The D step of the clip discriminator on the whole clip (real: clip, fake: decz.detach()), with its own LeCam
+        anchors and AdamW; the same loss as the per-frame D step."""
+        real_preds = self.clip_disc(clip)
+        fake_preds = self.clip_disc(decz.detach())
+        d_loss, avg_real_logits, avg_fake_logits, disc_acc = gan_disc_loss(real_preds, fake_preds, self.disc_type)
+        if _dist_on():
+            avg_real_logits = avg_scalar_over_nodes(avg_real_logits, clip.device)
+            avg_fake_logits = avg_scalar_over_nodes(avg_fake_logits, clip.device)
+        self.clip_lecam_anchor_real_logits.mul_(self.lecam_beta).add_(avg_real_logits, alpha=1 - self.lecam_beta)
+        self.clip_lecam_anchor_fake_logits.mul_(self.lecam_beta).add_(avg_fake_logits, alpha=1 - self.lecam_beta)
+        total_d_loss = d_loss.mean()
+        out = {"clip_d_loss": total_d_loss.detach()}
+        lecam_loss_item = torch.zeros((), device=clip.device)
+        if self.use_lecam:
+            lecam_loss = (real_preds - self.clip_lecam_anchor_fake_logits).pow(2).mean() + \
+                (fake_preds - self.clip_lecam_anchor_real_logits).pow(2).mean()
+            lecam_loss_item = lecam_loss.detach()
+            total_d_loss = total_d_loss + lecam_loss * self.lecam_loss_weight
+        self.optimizer_clip_D.zero_grad(set_to_none=True)
+        total_d_loss.backward()
+        self._clip_disc_dp.allreduce_grads()
+        self.optimizer_clip_D.step()
+        out.update(clip_avg_real_logits=avg_real_logits, clip_avg_fake_logits=avg_fake_logits,
+                   clip_disc_acc=disc_acc, clip_lecam_loss=lecam_loss_item)
         return out
 
 
@@ -220,9 +285,15 @@ class VideoTrainer:
 @click.option("--load_path", type=str, default=None, help="TVAE state_dict to start from (a saved checkpoint)")
 @click.option("--run_name", type=str, default="run", help="Checkpoints are saved under ./ckpt/<run_name>/")
 @click.option("--seed", type=int, default=42, help="Rank r seeds torch with seed + r (frame selection and noise)")
+@click.option("--do_clip_ganloss", is_flag=True, help="Also train against a 3-D PatchGAN on whole clips (tae_disc)")
+@click.option("--clip_disc_ch", type=int, default=64, help="Base channels of the clip discriminator (multiple of 32)")
+@click.option("--clip_disc_layers", type=int, default=3, help="Stride-2 layers of the clip discriminator")
+@click.option("--learning_rate_clip_disc", type=float, default=None,
+              help="Learning rate for the clip discriminator (default: --learning_rate_disc)")
 def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam, no_lpips,
                 recompute, learning_rate_vae, learning_rate_disc, vae_ch, vae_ch_mult, vae_num_res_blocks,
-                vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed):
+                vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed, do_clip_ganloss,
+                clip_disc_ch, clip_disc_layers, learning_rate_clip_disc):
     """Trains tae.TVAE on a seeded synthetic clip stream, data-parallel under torchrun (one process per GPU, NCCL) or in
     one process. Rank 0 logs every 5 steps and saves the TVAE's state_dict every --evaluate_every_n_steps steps."""
     # arguments are checked before anything touches a device
@@ -237,6 +308,19 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
     if clip_frames % div or resolution % div:
         raise click.BadParameter(f"--clip_frames ({clip_frames}) and --resolution ({resolution}) must be multiples of "
                                  f"{div} for {len(ch_mult)} levels", param_hint="--vae_ch_mult")
+    clip_disc = {}  # the clip discriminator's settings, passed only when one is trained
+    if do_clip_ganloss:
+        if clip_disc_ch <= 0 or clip_disc_ch % 32 or clip_disc_ch > 256:
+            raise click.BadParameter(f"must be a multiple of 32 up to 256, got {clip_disc_ch}",
+                                     param_hint="--clip_disc_ch")
+        if clip_disc_layers < 1:
+            raise click.BadParameter(f"must be >= 1, got {clip_disc_layers}", param_hint="--clip_disc_layers")
+        f = 2 ** clip_disc_layers
+        if clip_frames % f or resolution % f:
+            raise click.BadParameter(f"--clip_frames ({clip_frames}) and --resolution ({resolution}) must be multiples "
+                                     f"of {f} for {clip_disc_layers} layers", param_hint="--clip_disc_layers")
+        lr = learning_rate_disc if learning_rate_clip_disc is None else learning_rate_clip_disc
+        clip_disc = {"clip_disc": (clip_disc_ch, clip_disc_layers, lr)}
 
     assert torch.cuda.is_available(), "CUDA is required"
     rank = int(os.environ.get("RANK", "0"))
@@ -247,14 +331,17 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
     try:
         _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type,
                      use_lecam, no_lpips, recompute, learning_rate_vae, learning_rate_disc, vae_ch, ch_mult,
-                     vae_num_res_blocks, vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed)
+                     vae_num_res_blocks, vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed,
+                     **clip_disc)
     finally:
         cleanup()
 
 
 def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam,
                  no_lpips, recompute, learning_rate_vae, learning_rate_disc, vae_ch, ch_mult, vae_num_res_blocks,
-                 vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed):
+                 vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed, clip_disc=None):
+    """clip_disc: (ch, n_layers, learning rate) of a tae_disc.PatchDiscriminator3D to train against, or None."""
+    import tae_disc
     import utils
 
     torch.manual_seed(seed + rank)  # each rank draws its own frames and noise (the weights come from rank 0)
@@ -265,9 +352,14 @@ def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_f
         vae.load_state_dict(torch.load(load_path, map_location="cpu"), strict=True)
     lpips = None if no_lpips else utils.LPIPS().to(device)  # train mode: dropout live, as train_ddp runs it
     disc = utils.PatchDiscriminator().to(device) if do_ganloss else None
+    clip_kw = {}
+    if clip_disc is not None:
+        ch, n_layers, lr = clip_disc
+        clip_kw = dict(clip_discriminator=tae_disc.PatchDiscriminator3D(ch=ch, n_layers=n_layers).to(device),
+                       lr_clip_disc=lr)
     tr = VideoTrainer(vae.to(device), lpips, disc, disc_type=disc_type, use_lecam=use_lecam,
                       perceptual_frames=perceptual_frames, lr_vae=learning_rate_vae, lr_disc=learning_rate_disc,
-                      recompute=recompute)
+                      recompute=recompute, **clip_kw)
     lr_scheduler = cosine_with_warmup(tr.optimizer_G, 200, max_steps)
     clips = iter(SyntheticLoader(batch_size, resolution, frames=clip_frames))  # seed 42 + rank
 
@@ -291,6 +383,12 @@ def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_f
                           ("discriminator_accuracy", out["disc_acc"]), ("lecam_loss", out["lecam_loss"]),
                           ("lecam_anchor_real_logits", tr.lecam_anchor_real_logits),
                           ("lecam_anchor_fake_logits", tr.lecam_anchor_fake_logits)]
+            if clip_disc is not None:
+                items += [("clip_d_loss", out["clip_d_loss"]), ("clip_gan_loss", out["clip_g_gan_loss"]),
+                          ("clip_avg_real_logits", out["clip_avg_real_logits"]),
+                          ("clip_avg_fake_logits", out["clip_avg_fake_logits"]),
+                          ("clip_discriminator_accuracy", out["clip_disc_acc"]),
+                          ("clip_lecam_loss", out["clip_lecam_loss"])]
             items = [(k, float(v)) for k, v in items]
             now = time.time()
             items.append(("ms_per_step", (now - t_log) * 1e3 / (step + 1 - step_log)))
