@@ -413,7 +413,8 @@ int vqb_attn_bwd(const void* qkv, const void* out, const void* dout, const float
 /*
  * VQ codebook nearest neighbour (BASELINE.json config 4; the reference has no VQ — semantics pinned by
  * oracle/vq_oracle.py): idx[i] = argmin_j sum_c (z[i][c]-e[j][c])^2 in canonical fp32 order (bit-exact vs the oracle,
- * first index on ties), zq = e[idx], *sqerr += sum (zq - z)^2 when sqerr != NULL.
+ * first index on ties), zq = e[idx], *sqerr += sum (zq - z)^2 when sqerr != NULL. Non-finite distances follow
+ * np.argmin: the first NaN distance wins, and a row whose distances are all +inf gets 0, so idx is always in [0, K).
  */
 int vqb_vq_argmin(const float* z, const float* e, long long* idx, float* zq, float* sqerr, int M, int K, int D,
                   void* stream);

@@ -309,14 +309,23 @@ int vqb_maxpool2_bwd(const void* x, const void* dy, const void* add, void* dx, i
     return VQB_OK;
 }
 
+// Both directions serve exactly the widths whose C/8 channel vectors split over G = min(32, C/8) lanes (a power of two)
+// of VPL = 1 or 2 vectors each: C = 64, 128, 256, 512. Sizes are checked before anything divides by them.
+static int lpips_tail_check(const char* fn, int N, int HW, int C) {
+    VQB_CHECK(N > 0 && HW > 0, "%s: bad sizes N=%d HW=%d", fn, N, HW);
+    VQB_CHECK(C == 64 || C == 128 || C == 256 || C == 512, "%s: C=%d unsupported (64, 128, 256 or 512)", fn, C);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "%s: current device is not sm_90", fn);
+    return VQB_OK;
+}
+
 // out[n] += (1/HW) sum_p sum_c w_c (f0/(|f0|+eps) - f1/(|f1|+eps))^2 ; out must be initialised by the caller
 // (the five LPIPS layers accumulate into the same [N] vector, utils.py:54-57).
-static int lpips_tail_fwd_impl(const void* f0, const void* f1, const float* w, float* out, int N, int HW, int C,
-                               bool drop, uint64_t seed, void* stream) {
-    VQB_CHECK(f0 && f1 && w && out, "vqb_lpips_tail_fwd: null pointer");
-    VQB_CHECK(C % 64 == 0 && C <= 512 && ((C / 8) <= 32 || (C / 8) % 32 == 0), "vqb_lpips_tail_fwd: C=%d unsupported", C);
+static int lpips_tail_fwd_impl(const char* fn, const void* f0, const void* f1, const float* w, float* out, int N,
+                               int HW, int C, bool drop, uint64_t seed, void* stream) {
+    VQB_CHECK(f0 && f1 && w && out, "%s: null pointer", fn);
+    const int rc = lpips_tail_check(fn, N, HW, C);
+    if (rc != VQB_OK) return rc;
     const int V = C / 8, G = V < 32 ? V : 32, VPL = V / G;
-    VQB_CHECK((G & (G - 1)) == 0, "vqb_lpips_tail_fwd: C/8 must be a power of two");
     int ppb = (HW + 132 * 4 - 1) / (132 * 4);
     const int per_pass = 8 * (32 / G);
     if (ppb < per_pass * 2) ppb = per_pass * 2;
@@ -334,21 +343,22 @@ static int lpips_tail_fwd_impl(const void* f0, const void* f1, const float* w, f
     else if (VPL == 2)
         lpips_tail_fwd_kernel<2, true><<<grid, 256, 0, st>>>(a, b, w, out, HW, C, G, ppb, inv, seed);
     else
-        return set_error(VQB_EINVAL, "vqb_lpips_tail_fwd: C=%d unsupported", C);
+        return set_error(VQB_EINVAL, "%s: C=%d unsupported", fn, C);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
 }
 
 int vqb_lpips_tail_fwd(const void* f0, const void* f1, const float* w, float* out, int N, int HW, int C, void* stream) {
-    return lpips_tail_fwd_impl(f0, f1, w, out, N, HW, C, false, 0, stream);
+    return lpips_tail_fwd_impl("vqb_lpips_tail_fwd", f0, f1, w, out, N, HW, C, false, 0, stream);
 }
 int vqb_lpips_tail_fwd_dropout(const void* f0, const void* f1, const float* w, float* out, int N, int HW, int C,
                                uint64_t seed, void* stream) {
-    return lpips_tail_fwd_impl(f0, f1, w, out, N, HW, C, true, seed, stream);
+    return lpips_tail_fwd_impl("vqb_lpips_tail_fwd_dropout", f0, f1, w, out, N, HW, C, true, seed, stream);
 }
 int vqb_lpips_dropout_mask(uint64_t seed, int N, int HW, int C, uint8_t* mask, void* stream) {
-    VQB_CHECK(mask && C % 8 == 0, "vqb_lpips_dropout_mask: bad arguments");
+    VQB_CHECK(mask && N > 0 && HW > 0 && C > 0 && C % 8 == 0, "vqb_lpips_dropout_mask: bad arguments");
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_lpips_dropout_mask: current device is not sm_90");
     const int64_t total8 = static_cast<int64_t>(N) * HW * C / 8;
     lpips_dropout_mask_kernel<<<gs_blocks2(total8, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(seed, total8, mask);
     VQB_CUDA(cudaGetLastError());
@@ -356,12 +366,12 @@ int vqb_lpips_dropout_mask(uint64_t seed, int N, int HW, int C, uint8_t* mask, v
     return VQB_OK;
 }
 
-static int lpips_tail_bwd_impl(const void* f0, const void* f1, const float* w, const float* g, void* df0, int N, int HW,
-                               int C, bool drop, uint64_t seed, void* stream) {
-    VQB_CHECK(f0 && f1 && w && g && df0, "vqb_lpips_tail_bwd: null pointer");
-    VQB_CHECK(C % 64 == 0 && C <= 512, "vqb_lpips_tail_bwd: C=%d unsupported", C);
+static int lpips_tail_bwd_impl(const char* fn, const void* f0, const void* f1, const float* w, const float* g,
+                               void* df0, int N, int HW, int C, bool drop, uint64_t seed, void* stream) {
+    VQB_CHECK(f0 && f1 && w && g && df0, "%s: null pointer", fn);
+    const int rc = lpips_tail_check(fn, N, HW, C);
+    if (rc != VQB_OK) return rc;
     const int V = C / 8, G = V < 32 ? V : 32, VPL = V / G;
-    VQB_CHECK((G & (G - 1)) == 0, "vqb_lpips_tail_bwd: C/8 must be a power of two");
     int ppb = (HW + 132 * 4 - 1) / (132 * 4);
     const int per_pass = 8 * (32 / G);
     if (ppb < per_pass * 2) ppb = per_pass * 2;
@@ -380,7 +390,7 @@ static int lpips_tail_bwd_impl(const void* f0, const void* f1, const float* w, c
     else if (VPL == 2)
         lpips_tail_bwd_kernel<2, true><<<grid, 256, 0, st>>>(a, b, w, g, d, HW, C, G, ppb, inv, seed);
     else
-        return set_error(VQB_EINVAL, "vqb_lpips_tail_bwd: C=%d unsupported", C);
+        return set_error(VQB_EINVAL, "%s: C=%d unsupported", fn, C);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
@@ -388,11 +398,11 @@ static int lpips_tail_bwd_impl(const void* f0, const void* f1, const float* w, c
 
 int vqb_lpips_tail_bwd(const void* f0, const void* f1, const float* w, const float* g, void* df0, int N, int HW, int C,
                        void* stream) {
-    return lpips_tail_bwd_impl(f0, f1, w, g, df0, N, HW, C, false, 0, stream);
+    return lpips_tail_bwd_impl("vqb_lpips_tail_bwd", f0, f1, w, g, df0, N, HW, C, false, 0, stream);
 }
 int vqb_lpips_tail_bwd_dropout(const void* f0, const void* f1, const float* w, const float* g, void* df0, int N, int HW,
                                int C, uint64_t seed, void* stream) {
-    return lpips_tail_bwd_impl(f0, f1, w, g, df0, N, HW, C, true, seed, stream);
+    return lpips_tail_bwd_impl("vqb_lpips_tail_bwd_dropout", f0, f1, w, g, df0, N, HW, C, true, seed, stream);
 }
 
 }  // extern "C"

@@ -181,6 +181,7 @@ int vqb_adamw_flat(float* params, const float* grads, float* exp_avg, float* exp
         h.bc1[i] = static_cast<float>(1.0 - pow(static_cast<double>(s.beta1), static_cast<double>(s.step)));
         h.bc2_sqrt[i] = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(s.beta2), static_cast<double>(s.step))));
     }
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_adamw_flat: current device is not sm_90");
     int64_t blocks = nchunks;
     const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (blocks > cap) blocks = cap;
@@ -216,6 +217,7 @@ int vqb_adamw_flat_dev(float* params, const float* grads, float* exp_avg, float*
                reinterpret_cast<uintptr_t>(exp_avg) | reinterpret_cast<uintptr_t>(exp_avg_sq)) % 16 == 0,
               "vqb_adamw_flat_dev: buffers must be 16-byte aligned");
     if (nchunks <= 0) return VQB_OK;
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_adamw_flat_dev: current device is not sm_90");
     int64_t blocks = nchunks;
     const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (blocks > cap) blocks = cap;

@@ -1,7 +1,10 @@
 // VQ codebook nearest-neighbour search (BASELINE.json config 4; absent from the reference — semantics pinned by
 // oracle/vq_oracle.py): idx[i] = argmin_j sum_c (z[i][c] - e[j][c])^2 with the CANONICAL fp32 evaluation order
 // (c ascending, separate rounded subtract / multiply / add, no FMA contraction) so that indices are bit-reproducible
-// against the NumPy oracle; ties resolve to the smallest index (torch.argmin / np.argmin rule).
+// against the NumPy oracle; ties resolve to the smallest index (torch.argmin / np.argmin rule). Non-finite distances
+// follow np.argmin too: the first NaN distance wins (a NaN in z[i] or in a code), and a row whose distances are all
+// +inf (|z - e|^2 overflows) gets index 0, so the index is always in [0, K). Both the per-lane scan and the warp
+// reduction compare the key (NaN -> -1, else d; distances are never negative) lexicographically with the index.
 //
 // One warp per row of z; the 32 lanes split the codebook (lane l scans codes l, l+32, ...), codebook chunks are staged
 // in shared memory with a +1 word row pitch (conflict-free), the per-lane (distance, index) minima are combined with a
@@ -52,8 +55,11 @@ __global__ void __launch_bounds__(256) vq_argmin_kernel(const float* __restrict_
                         const float diff = __fsub_rn(zr[c], ej[c]);
                         d = __fadd_rn(d, __fmul_rn(diff, diff));
                     }
-                    if (d < best_d[r]) {  // strict: the first (smallest-index) minimum of this lane's subsequence wins
-                        best_d[r] = d;
+                    // the first (smallest-index) minimum of this lane's subsequence wins; the index clause only takes
+                    // the lane's first code when every key so far is +inf (the sentinel index is larger than any j)
+                    const float key = d != d ? -1.f : d;
+                    if (key < best_d[r] || (key == best_d[r] && k0 + j < best_j[r])) {
+                        best_d[r] = key;
                         best_j[r] = k0 + j;
                     }
                 }
@@ -106,6 +112,7 @@ int vqb_vq_argmin(const float* z, const float* e, long long* idx, float* zq, flo
         kVqChunk >>= 1;
     const size_t smem = (static_cast<size_t>(kVqRowsPerBlock) * D + static_cast<size_t>(kVqChunk) * (D + 1)) * sizeof(float);
     VQB_CHECK(smem <= 200 * 1024, "vqb_vq_argmin: D=%d too large for the shared-memory chunk", D);
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_vq_argmin: current device is not sm_90");
     static size_t attr_set = 0;
     if (smem > 48 * 1024 && smem > attr_set) {
         VQB_CUDA(cudaFuncSetAttribute(vq_argmin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
