@@ -459,6 +459,19 @@ typedef struct VqbPackJob {
 } VqbPackJob;
 int vqb_pack_weights_multi(const VqbPackJob* jobs_dev, int njobs, int total_blocks, void* stream);
 
+/*
+ * Reconstruction metrics (DESIGN.md section 7 row 25; the reference has none): per-item PSNR and SSIM of x against y,
+ * both contiguous [B][C][T][H][W] (images: T = 1), fp32 (bf16 = 0) or bf16 (bf16 = 1). An item is (b, t); psnr and ssim
+ * are fp32 [B * T] in (b, t) order. Every value v is mapped to u = fminf(fmaxf((v - lo) * inv, 0), 1) with inv =
+ * 1 / (hi - lo) rounded once to fp32. PSNR = 10 log10(1 / mean (u_x - u_y)^2) over the item's C*H*W values (+inf when
+ * the mean is 0). SSIM (Wang et al. 2004, no padding, no downsampling) is the mean over channels and the (H-10)(W-10)
+ * valid positions of the 11x11 Gaussian window (sigma 1.5, normalised), C1 = 0.01^2, C2 = 0.03^2.
+ * work: fp32 scratch of work_elems >= 2 * B * T * C * ceil((H-10)/32) * ceil((W-10)/32) floats. H, W >= 11, lo < hi
+ * (finite). Two launches, no atomics: results are bit-reproducible.
+ */
+int vqb_psnr_ssim(const void* x, const void* y, int bf16, int B, int C, int T, int H, int W, float lo, float hi,
+                  float* psnr, float* ssim, float* work, int64_t work_elems, void* stream);
+
 /* library / device info */
 const char* vqb_last_error(void);
 int vqb_version(void);

@@ -164,6 +164,7 @@ def load():
         "vqb_nhwc_frames_to_ncthw": (i32, [vp, vp] + [i32] * 6 + [vp, i32, vp, vp]),
         "vqb_leaky_relu_fwd": (i32, [vp, vp, i64, vp]),
         "vqb_leaky_relu_bwd": (i32, [vp, vp, vp, i64, vp]),
+        "vqb_psnr_ssim": (i32, [vp, vp] + [i32] * 6 + [f32, f32, vp, vp, vp, i64, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)

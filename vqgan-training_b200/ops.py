@@ -1166,6 +1166,58 @@ def vq_argmin(z_flat: torch.Tensor, codebook: torch.Tensor):
     return idx, zq, sq
 
 
+METRICS_TILE = 32  # SSIM positions per tile side of vqb_psnr_ssim (kMTile in csrc/metrics.cu); sizes the workspace
+
+
+def psnr_ssim(x: torch.Tensor, y: torch.Tensor, value_range=(0.0, 1.0)):
+    """Per-item PSNR (dB) and SSIM of x against y (DESIGN.md section 7 row 25): images [B, C, H, W] -> two fp32 [B],
+    clips [B, C, T, H, W] -> two fp32 [B, T], one value per frame in (b, t) order.
+
+    x and y: contiguous CUDA tensors of one shape and dtype (float32 or bfloat16), C >= 1, H and W >= 11. Values are
+    mapped to [0, 1] by value_range=(lo, hi) and clamped: (0, 1) for images, (-1, 1) for the TVAE's clips. PSNR is +inf
+    for identical items. Not differentiable: inputs that require grad under grad mode are refused, so that the result
+    cannot be mistaken for a loss. Every refusal raises before anything launches."""
+    if not isinstance(x, torch.Tensor) or not isinstance(y, torch.Tensor):
+        raise TypeError("psnr_ssim: x and y must be tensors")
+    if torch.is_grad_enabled() and (x.requires_grad or y.requires_grad):
+        raise RuntimeError("psnr_ssim is not differentiable: call it under torch.no_grad() or on detached tensors")
+    if x.dim() not in (4, 5):
+        raise ValueError(f"psnr_ssim: expected [B, C, H, W] images or [B, C, T, H, W] clips, got shape "
+                         f"{tuple(x.shape)}")
+    if x.shape != y.shape:
+        raise ValueError(f"psnr_ssim: shapes differ: {tuple(x.shape)} vs {tuple(y.shape)}")
+    if x.dtype != y.dtype or x.dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"psnr_ssim: x and y must both be float32 or both bfloat16, got {x.dtype} and {y.dtype}")
+    B, C = x.shape[:2]
+    T = x.shape[2] if x.dim() == 5 else 1
+    H, W = x.shape[-2:]
+    if min(B, C, T) < 1 or H < 11 or W < 11:
+        raise ValueError(f"psnr_ssim: need non-empty B, C, T and H, W >= 11 (the SSIM window), got shape "
+                         f"{tuple(x.shape)}")
+    try:
+        lo, hi = (float(v) for v in value_range)
+    except (TypeError, ValueError):
+        raise ValueError(f"psnr_ssim: value_range must be a pair (lo, hi), got {value_range!r}") from None
+    lo32, hi32 = (torch.tensor(v, dtype=torch.float32).item() for v in (lo, hi))  # the kernel's fp32 bounds
+    if not (math.isfinite(lo32) and math.isfinite(hi32) and hi32 > lo32):
+        raise ValueError(f"psnr_ssim: value_range must be finite with lo < hi in float32, got {value_range!r}")
+    require_cuda(x)
+    require_cuda(y)
+    if x.device != y.device:
+        raise ValueError(f"psnr_ssim: x is on {x.device}, y on {y.device}")
+    if not (x.is_contiguous() and y.is_contiguous()):
+        raise ValueError("psnr_ssim: x and y must be contiguous (the kernel reads NCHW / NCTHW in place)")
+    tiles = -(-(H - 10) // METRICS_TILE) * -(-(W - 10) // METRICS_TILE)
+    work = torch.empty(2 * B * T * C * tiles, device=x.device, dtype=torch.float32)
+    psnr = torch.empty(B, T, device=x.device, dtype=torch.float32)
+    ssim = torch.empty(B, T, device=x.device, dtype=torch.float32)
+    check(_L().vqb_psnr_ssim(ptr(x), ptr(y), int(x.dtype == torch.bfloat16), B, C, T, H, W, lo32, hi32, ptr(psnr),
+                             ptr(ssim), ptr(work), work.numel(), stream_ptr()), "psnr_ssim")
+    if x.dim() == 4:
+        return psnr.view(B), ssim.view(B)
+    return psnr, ssim
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # Video autoencoder (tae.py): ops over NTHWC bf16 activations [N, T, H, W, Cp]. The plain functions are the no-grad
 # inference path; the autograd functions after them (Conv3dFn, UpConv3dFn, AttentionHdFn, GaussReparamFn) are the

@@ -50,6 +50,9 @@ from vae_trainer import (FlatAllReduceDDP, SyntheticLoader, _dist_on, avg_scalar
                          cosine_with_warmup, gan_disc_loss, gradnorm, vae_loss_function)
 
 
+EVAL_SEED = 20040101  # seed of train_video's held-out clips (--eval_clips), fixed across runs and ranks
+
+
 def fold_frames(x: torch.Tensor, frames=None) -> torch.Tensor:
     """[B, C, T, H, W] -> [B*T', C, H, W] in (b, t) order (frames: [B, T'] selection, None = every frame). An ATen
     copy, for the terms that take images rather than clips (the MSE of the lpips=None baseline)."""
@@ -262,6 +265,49 @@ class VideoTrainer:
                    clip_disc_acc=disc_acc, clip_lecam_loss=lecam_loss_item)
         return out
 
+    @torch.no_grad()
+    def evaluate(self, clips) -> dict:
+        """Reconstruction quality of held-out clips: `clips` is an iterable of fp32 [B, 3, T, H, W] clips in [-1, 1).
+
+        Each clip is encoded by the TVAE and its posterior mean (the first half of the encoder's channels; nothing is
+        sampled, so a checkpoint's score does not depend on the RNG) decoded. The frames are scored with
+        ops.psnr_ssim(decz, clip, value_range=(-1, 1)) and, when the trainer has an LPIPS, with
+        lpips(decz.clamp(-1, 1), clip) in eval mode (dropout off; its previous mode is restored).
+
+        Returns psnr, ssim (and lpips) as Python floats, the means over every frame, and psnr_frames, ssim_frames (and
+        lpips_frames) as fp32 [N, T] tensors, N the clips' batch rows in order. Weights, packed operands, optimizer
+        moments, LeCam anchors, module modes and RNG states are left as they were, and no collective is issued."""
+        import ops
+
+        vae, lpips = self.vae, self.lpips
+        was_training = lpips.training if lpips is not None else None
+        scores = {"psnr": [], "ssim": [], "lpips": []}
+        try:
+            if lpips is not None:
+                lpips.eval()
+            for clip in clips:
+                if clip.dim() != 5 or clip.shape[1] != 3:
+                    raise ValueError(f"expected [B, 3, T, H, W] clips, got shape {tuple(clip.shape)}")
+                z = vae.encoder(clip)
+                decz = vae.decoder(z[:, :z.shape[1] // 2])
+                p, s = ops.psnr_ssim(decz, clip, value_range=(-1.0, 1.0))
+                scores["psnr"].append(p)
+                scores["ssim"].append(s)
+                if lpips is not None:
+                    scores["lpips"].append(lpips(decz.clamp(-1, 1), clip).view(p.shape))
+        finally:
+            if lpips is not None:
+                lpips.train(was_training)
+        if not scores["psnr"]:
+            raise ValueError("evaluate: no clips")
+        out = {}
+        for k, v in scores.items():
+            if v:
+                frames = torch.cat(v)
+                out[k] = float(frames.double().mean())
+                out[f"{k}_frames"] = frames
+        return out
+
 
 @click.command()
 @click.option("--batch_size", type=int, default=1, help="Clips per rank per step")
@@ -290,13 +336,19 @@ class VideoTrainer:
 @click.option("--clip_disc_layers", type=int, default=3, help="Stride-2 layers of the clip discriminator")
 @click.option("--learning_rate_clip_disc", type=float, default=None,
               help="Learning rate for the clip discriminator (default: --learning_rate_disc)")
+@click.option("--eval_clips", type=int, default=0,
+              help="Held-out clips rank 0 reconstructs and scores (PSNR, SSIM, LPIPS) at every checkpoint (0: none)")
 def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam, no_lpips,
                 recompute, learning_rate_vae, learning_rate_disc, vae_ch, vae_ch_mult, vae_num_res_blocks,
                 vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed, do_clip_ganloss,
-                clip_disc_ch, clip_disc_layers, learning_rate_clip_disc):
+                clip_disc_ch, clip_disc_layers, learning_rate_clip_disc, eval_clips):
     """Trains tae.TVAE on a seeded synthetic clip stream, data-parallel under torchrun (one process per GPU, NCCL) or in
-    one process. Rank 0 logs every 5 steps and saves the TVAE's state_dict every --evaluate_every_n_steps steps."""
+    one process. Rank 0 logs every 5 steps and saves the TVAE's state_dict every --evaluate_every_n_steps steps; with
+    --eval_clips K it first scores K held-out clips (VideoTrainer.evaluate) and logs eval_psnr, eval_ssim and
+    eval_lpips."""
     # arguments are checked before anything touches a device
+    if eval_clips < 0:
+        raise click.BadParameter(f"must be >= 0, got {eval_clips}", param_hint="--eval_clips")
     if perceptual_frames is not None and not 1 <= perceptual_frames <= clip_frames:
         raise click.BadParameter(f"must be between 1 and --clip_frames ({clip_frames}), got {perceptual_frames}",
                                  param_hint="--perceptual_frames")
@@ -308,7 +360,7 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
     if clip_frames % div or resolution % div:
         raise click.BadParameter(f"--clip_frames ({clip_frames}) and --resolution ({resolution}) must be multiples of "
                                  f"{div} for {len(ch_mult)} levels", param_hint="--vae_ch_mult")
-    clip_disc = {}  # the clip discriminator's settings, passed only when one is trained
+    extra = {}  # the clip discriminator's settings and eval_clips, passed only when used
     if do_clip_ganloss:
         if clip_disc_ch <= 0 or clip_disc_ch % 32 or clip_disc_ch > 256:
             raise click.BadParameter(f"must be a multiple of 32 up to 256, got {clip_disc_ch}",
@@ -320,7 +372,9 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
             raise click.BadParameter(f"--clip_frames ({clip_frames}) and --resolution ({resolution}) must be multiples "
                                      f"of {f} for {clip_disc_layers} layers", param_hint="--clip_disc_layers")
         lr = learning_rate_disc if learning_rate_clip_disc is None else learning_rate_clip_disc
-        clip_disc = {"clip_disc": (clip_disc_ch, clip_disc_layers, lr)}
+        extra["clip_disc"] = (clip_disc_ch, clip_disc_layers, lr)
+    if eval_clips:
+        extra["eval_clips"] = eval_clips
 
     assert torch.cuda.is_available(), "CUDA is required"
     rank = int(os.environ.get("RANK", "0"))
@@ -332,15 +386,17 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
         _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type,
                      use_lecam, no_lpips, recompute, learning_rate_vae, learning_rate_disc, vae_ch, ch_mult,
                      vae_num_res_blocks, vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed,
-                     **clip_disc)
+                     **extra)
     finally:
         cleanup()
 
 
 def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam,
                  no_lpips, recompute, learning_rate_vae, learning_rate_disc, vae_ch, ch_mult, vae_num_res_blocks,
-                 vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed, clip_disc=None):
-    """clip_disc: (ch, n_layers, learning rate) of a tae_disc.PatchDiscriminator3D to train against, or None."""
+                 vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed, clip_disc=None,
+                 eval_clips=0):
+    """clip_disc: (ch, n_layers, learning rate) of a tae_disc.PatchDiscriminator3D to train against, or None.
+    eval_clips: the number of held-out clips rank 0 scores at every checkpoint."""
     import tae_disc
     import utils
 
@@ -362,6 +418,9 @@ def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_f
                       recompute=recompute, **clip_kw)
     lr_scheduler = cosine_with_warmup(tr.optimizer_G, 200, max_steps)
     clips = iter(SyntheticLoader(batch_size, resolution, frames=clip_frames))  # seed 42 + rank
+    held_out = []
+    if eval_clips and rank == 0:  # the same clips on every run, whatever --seed: scores compare across runs
+        held_out = SyntheticLoader(1, resolution, seed=EVAL_SEED, n_distinct=eval_clips, frames=clip_frames).batches
 
     logger = logging.getLogger(__name__)
     logger.setLevel(logging.INFO)
@@ -395,6 +454,10 @@ def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_f
             t_log, step_log = now, step + 1
             logger.info(f"step {step} - " + "\n\t".join(f"{k}: {v:.4f}" for k, v in items))
         if evaluate_every_n_steps > 0 and (step + 1) % evaluate_every_n_steps == 0 and rank == 0:
+            if held_out:
+                ev = tr.evaluate(c.to(device, non_blocking=True) for c in held_out)
+                logger.info(f"step {step + 1} - " + "\n\t".join(f"eval_{k}: {ev[k]:.4f}" for k in
+                                                                  ("psnr", "ssim", "lpips") if k in ev))
             os.makedirs(f"./ckpt/{run_name}", exist_ok=True)
             ck = f"./ckpt/{run_name}/tvae_step_{step + 1}.pt"
             torch.save({k: v.detach().cpu() for k, v in tr.vae.state_dict().items()}, ck)
