@@ -440,6 +440,14 @@ int vqb_adamw_flat(float* params, const float* grads, float* exp_avg, float* exp
 int vqb_adamw_fill_record(int ngroups, const VqbAdamwGroup* groups_host, float* record_host);
 int vqb_adamw_flat_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const uint8_t* chunk_group,
                        int64_t nchunks, const float* record_dev, float grad_scale, void* stream);
+/* vqb_adamw_flat_dev plus an exponential moving average of the parameters in the same pass: after the AdamW update,
+ * every element of the flat buffer (chunks of group 255 and zero pads included) gets ema -= r * (ema - params), with
+ * r = 1 - d_n read as one fp32 from DEVICE memory (ema_rate_dev) at kernel run time, so graph replays follow the
+ * schedule without re-capture. params, exp_avg and exp_avg_sq are bit-identical to vqb_adamw_flat_dev's. ema must be
+ * 16-byte aligned like the other buffers. */
+int vqb_adamw_ema_flat_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, float* ema,
+                           const uint8_t* chunk_group, int64_t nchunks, const float* record_dev,
+                           const float* ema_rate_dev, float grad_scale, void* stream);
 
 /*
  * Re-pack every cached bf16 GEMM operand of the fp32 OIHW master weights in one launch (after an optimizer step).

@@ -3,6 +3,8 @@
 //   vqb_adamw_flat          AdamW over ONE flat fp32 parameter/gradient/moment buffer holding every tensor of a model
 //                           (two learning-rate groups + cosine schedule of vae_trainer.py:455-475,486-490 arrive as
 //                           per-group scalars), replacing ~250 per-tensor ATen multi_tensor_apply chunks.
+//   vqb_adamw_ema_flat_dev  the same AdamW pass that also moves an exponential moving average of the parameters (one
+//                           more fp32 read and write per element, no extra launch).
 //   vqb_pack_weights_multi  re-packs EVERY cached bf16 GEMM operand (forward, data-gradient, folded up-sample and
 //                           fat-pixel layouts) of the just-updated fp32 OIHW master weights in one launch driven by a
 //                           device-resident job table (what torch.autocast's per-step weight casts do in the reference,
@@ -25,16 +27,36 @@ struct AdamwGroups {
 };
 
 // hyper-parameters either by value (h) or, hdev != nullptr, from DEVICE memory (one AdamwGroups record the host refreshes
-// before every launch / CUDA-graph replay: learning-rate schedules and bias corrections then need no re-capture)
+// before every launch / CUDA-graph replay: learning-rate schedules and bias corrections then need no re-capture).
+// kEma additionally keeps an exponential moving average of the parameters in the same pass over the chunks: after the
+// AdamW update of a chunk (or, group 255, with its parameters unchanged) e -= r * (e - p'), r = 1 - d_n read from the
+// device scalar ema_rate (vqb_adamw_ema_flat_dev). The AdamW arithmetic is the same code in both instances, so p, m and v
+// are bit-identical with and without the average.
+template <bool kEma>
 __global__ void __launch_bounds__(256) adamw_flat_kernel(float* __restrict__ p, const float* __restrict__ g,
                                                          float* __restrict__ m, float* __restrict__ v,
                                                          const uint8_t* __restrict__ chunk_group, int64_t nchunks,
                                                          AdamwGroups h, const AdamwGroups* __restrict__ hdev,
-                                                         float grad_scale) {
+                                                         float grad_scale, float* __restrict__ ema,
+                                                         const float* __restrict__ ema_rate) {
     if (hdev) h = *hdev;
+    float rate = 0.f;
+    if constexpr (kEma) rate = *ema_rate;
     for (int64_t c = blockIdx.x; c < nchunks; c += gridDim.x) {
         const int grp = chunk_group[c];
-        if (grp >= VQB_ADAMW_MAX_GROUPS) continue;
+        if (grp >= VQB_ADAMW_MAX_GROUPS) {
+            if constexpr (kEma) {  // no gradient: AdamW skips the chunk, its average still moves toward the unchanged p
+                const int64_t i = c * 1024 + threadIdx.x * 4;
+                const float4 pp = *reinterpret_cast<const float4*>(p + i);
+                float4 ee = *reinterpret_cast<const float4*>(ema + i);
+                ee.x = ee.x - rate * (ee.x - pp.x);
+                ee.y = ee.y - rate * (ee.y - pp.y);
+                ee.z = ee.z - rate * (ee.z - pp.z);
+                ee.w = ee.w - rate * (ee.w - pp.w);
+                *reinterpret_cast<float4*>(ema + i) = ee;
+            }
+            continue;
+        }
         const float lr = h.lr[grp], b1 = h.beta1[grp], b2 = h.beta2[grp], eps = h.eps[grp];
         const float decay = 1.f - lr * h.wd[grp], step = lr / h.bc1[grp], bc2s = h.bc2_sqrt[grp];
         const int64_t i = c * 1024 + threadIdx.x * 4;
@@ -58,6 +80,13 @@ __global__ void __launch_bounds__(256) adamw_flat_kernel(float* __restrict__ p, 
         *reinterpret_cast<float4*>(p + i) = pp;
         *reinterpret_cast<float4*>(m + i) = mm;
         *reinterpret_cast<float4*>(v + i) = vv;
+        if constexpr (kEma) {
+            float4 ee = *reinterpret_cast<const float4*>(ema + i);
+            float* E = reinterpret_cast<float*>(&ee);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) E[j] = E[j] - rate * (E[j] - P[j]);
+            *reinterpret_cast<float4*>(ema + i) = ee;
+        }
     }
 }
 
@@ -185,8 +214,8 @@ int vqb_adamw_flat(float* params, const float* grads, float* exp_avg, float* exp
     int64_t blocks = nchunks;
     const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (blocks > cap) blocks = cap;
-    adamw_flat_kernel<<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        params, grads, exp_avg, exp_avg_sq, chunk_group, nchunks, h, nullptr, grad_scale);
+    adamw_flat_kernel<false><<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        params, grads, exp_avg, exp_avg_sq, chunk_group, nchunks, h, nullptr, grad_scale, nullptr, nullptr);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;
@@ -222,9 +251,32 @@ int vqb_adamw_flat_dev(float* params, const float* grads, float* exp_avg, float*
     const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
     if (blocks > cap) blocks = cap;
     AdamwGroups dummy = {};
-    adamw_flat_kernel<<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    adamw_flat_kernel<false><<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         params, grads, exp_avg, exp_avg_sq, chunk_group, nchunks, dummy,
-        reinterpret_cast<const AdamwGroups*>(record_dev), grad_scale);
+        reinterpret_cast<const AdamwGroups*>(record_dev), grad_scale, nullptr, nullptr);
+    VQB_CUDA(cudaGetLastError());
+    count_launch();
+    return VQB_OK;
+}
+
+int vqb_adamw_ema_flat_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, float* ema,
+                           const uint8_t* chunk_group, int64_t nchunks, const float* record_dev,
+                           const float* ema_rate_dev, float grad_scale, void* stream) {
+    VQB_CHECK(params && grads && exp_avg && exp_avg_sq && ema && chunk_group && record_dev && ema_rate_dev,
+              "vqb_adamw_ema_flat_dev: null pointer");
+    VQB_CHECK((reinterpret_cast<uintptr_t>(params) | reinterpret_cast<uintptr_t>(grads) |
+               reinterpret_cast<uintptr_t>(exp_avg) | reinterpret_cast<uintptr_t>(exp_avg_sq) |
+               reinterpret_cast<uintptr_t>(ema)) % 16 == 0,
+              "vqb_adamw_ema_flat_dev: buffers must be 16-byte aligned");
+    if (nchunks <= 0) return VQB_OK;
+    if (!device_is_sm90()) return set_error(VQB_ENODEVICE, "vqb_adamw_ema_flat_dev: current device is not sm_90");
+    int64_t blocks = nchunks;
+    const int64_t cap = static_cast<int64_t>(num_sms() > 0 ? num_sms() : 132) * 16;
+    if (blocks > cap) blocks = cap;
+    AdamwGroups dummy = {};
+    adamw_flat_kernel<true><<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        params, grads, exp_avg, exp_avg_sq, chunk_group, nchunks, dummy,
+        reinterpret_cast<const AdamwGroups*>(record_dev), grad_scale, ema, ema_rate_dev);
     VQB_CUDA(cudaGetLastError());
     count_launch();
     return VQB_OK;

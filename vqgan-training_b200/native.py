@@ -142,6 +142,7 @@ def load():
         "vqb_pack_weights_multi": (i32, [vp, i32, i32, vp]),
         "vqb_adamw_fill_record": (i32, [i32, C.POINTER(VqbAdamwGroup), vp]),
         "vqb_adamw_flat_dev": (i32, [vp, vp, vp, vp, vp, i64, vp, f32, vp]),
+        "vqb_adamw_ema_flat_dev": (i32, [vp, vp, vp, vp, vp, vp, i64, vp, vp, f32, vp]),
         "vqb_pack_weights_bf16": (i32, [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp]),
         "vqb_pack_weights_fold_bf16": (i32, [vp, vp, i32, i32, i32, i32, vp, i32, i32, vp]),
         "vqb_nchw_to_nhwc_bf16": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]),

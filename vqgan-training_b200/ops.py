@@ -131,6 +131,7 @@ PACK_MULTI_MAX_TAPS = 16
 # every live pack entry, by the data_ptr of the master weight it was packed from (weak: caches own the entries)
 _pack_registry = {}
 _pack_tables = {}
+_captured_pack_tables = []
 
 
 def _new_pack_entry(weight, tapmap, transpose, Kpad, fold, fat=False) -> _PackEntry:
@@ -180,6 +181,10 @@ def _run_pack(entries):
             _pack_tables.clear()
         tab = (dev, len(jobs), nb, [weakref.ref(e) for e in entries])
         _pack_tables[key] = tab
+    if torch.cuda.is_current_stream_capturing():
+        # a captured launch reads this job table on every replay: keep it alive even if the cache above is cleared
+        # later (another trainer's first steps add entries), or its memory would be handed to other tensors
+        _captured_pack_tables.append(tab)
     check(_L().vqb_pack_weights_multi(tab[0].data_ptr(), tab[1], tab[2], stream_ptr()), "pack_weights_multi")
     for e in entries:
         w = e.wref()

@@ -44,10 +44,10 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 import tae
-from flat import FlatAdamW
+from flat import FlatAdamW, check_ema_decay
 from utils import broadcast_module_state
 from vae_trainer import (FlatAllReduceDDP, SyntheticLoader, _dist_on, avg_scalar_over_nodes, cleanup,
-                         cosine_with_warmup, gan_disc_loss, gradnorm, vae_loss_function)
+                         cosine_with_warmup, gan_disc_loss, gradnorm, restart_ema, vae_loss_function)
 
 
 EVAL_SEED = 20040101  # seed of train_video's held-out clips (--eval_clips), fixed across runs and ranks
@@ -79,6 +79,9 @@ class VideoTrainer:
         Trainer) over the TVAE and the discriminator.
     clip_discriminator: tae_disc.PatchDiscriminator3D or None; it is opted into training here. lr_clip_disc: its AdamW
         learning rate (same betas and weight decay); clip_disc_weight: the GradNorm weight of its generator pass.
+    ema_decay: None, or 0 < d < 1 to keep an exponential moving average of the TVAE's trained weights in its fused
+        AdamW launch (flat.FlatAdamW; not of the discriminators). `vae_ema` is a tae.TVAE over the average (None
+        without one); evaluate(clips, ema=True) scores it.
 
     step(clip) per step:
       1. decz, z = vae(clip) (the reparameterisation draws its noise from torch's CUDA generator);
@@ -107,7 +110,9 @@ class VideoTrainer:
 
     def __init__(self, vae: nn.Module, lpips, discriminator=None, *, disc_type="hinge", use_lecam=False,
                  perceptual_frames=None, lr_vae, lr_disc=None, recompute=False, clip_discriminator=None,
-                 lr_clip_disc=None, clip_disc_weight=1.0):
+                 lr_clip_disc=None, clip_disc_weight=1.0, ema_decay=None):
+        if ema_decay is not None:
+            ema_decay = check_ema_decay(ema_decay)
         if disc_type not in ("hinge", "bce"):
             raise ValueError(f"unknown disc_type {disc_type!r}")
         if discriminator is not None and lr_disc is None:
@@ -126,8 +131,12 @@ class VideoTrainer:
             discriminator.requires_grad_(True)
             self._disc_dp = FlatAllReduceDDP(discriminator)
         self.optimizer_G = FlatAdamW([{"params": [p for p in vae.parameters() if p.requires_grad], "lr": lr_vae}],
-                                     weight_decay=1e-3, betas=(0.9, 0.95))
+                                     weight_decay=1e-3, betas=(0.9, 0.95), ema_decay=ema_decay)
         self._vae_dp.attach_store(self.optimizer_G.store)
+        self.vae_ema = None
+        if ema_decay is not None:  # started after the broadcast, from the weights every rank holds
+            self.vae_ema = self.optimizer_G.averaged_copy(vae)
+            self._vae_dp.after_load = lambda: restart_ema(self.optimizer_G, self.vae, self.vae_ema)
         self.optimizer_D = None
         device = next(vae.parameters()).device
         if discriminator is not None:
@@ -266,7 +275,7 @@ class VideoTrainer:
         return out
 
     @torch.no_grad()
-    def evaluate(self, clips) -> dict:
+    def evaluate(self, clips, ema=False) -> dict:
         """Reconstruction quality of held-out clips: `clips` is an iterable of fp32 [B, 3, T, H, W] clips in [-1, 1).
 
         Each clip is encoded by the TVAE and its posterior mean (the first half of the encoder's channels; nothing is
@@ -276,10 +285,13 @@ class VideoTrainer:
 
         Returns psnr, ssim (and lpips) as Python floats, the means over every frame, and psnr_frames, ssim_frames (and
         lpips_frames) as fp32 [N, T] tensors, N the clips' batch rows in order. Weights, packed operands, optimizer
-        moments, LeCam anchors, module modes and RNG states are left as they were, and no collective is issued."""
+        moments, LeCam anchors, module modes and RNG states are left as they were, and no collective is issued.
+        ema=True scores the averaged weights (vae_ema) instead of the trained ones."""
         import ops
 
-        vae, lpips = self.vae, self.lpips
+        if ema and self.vae_ema is None:
+            raise ValueError("evaluate(ema=True): this trainer keeps no weight EMA (ema_decay=None)")
+        vae, lpips = (self.vae_ema if ema else self.vae), self.lpips
         was_training = lpips.training if lpips is not None else None
         scores = {"psnr": [], "ssim": [], "lpips": []}
         try:
@@ -338,15 +350,21 @@ class VideoTrainer:
               help="Learning rate for the clip discriminator (default: --learning_rate_disc)")
 @click.option("--eval_clips", type=int, default=0,
               help="Held-out clips rank 0 reconstructs and scores (PSNR, SSIM, LPIPS) at every checkpoint (0: none)")
+@click.option("--ema_decay", type=float, default=None,
+              help="Keep an EMA of the TVAE weights with this decay (0 < D < 1, warmed up over the first updates) and "
+                   "save it beside every checkpoint (default: none)")
 def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam, no_lpips,
                 recompute, learning_rate_vae, learning_rate_disc, vae_ch, vae_ch_mult, vae_num_res_blocks,
                 vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed, do_clip_ganloss,
-                clip_disc_ch, clip_disc_layers, learning_rate_clip_disc, eval_clips):
+                clip_disc_ch, clip_disc_layers, learning_rate_clip_disc, eval_clips, ema_decay):
     """Trains tae.TVAE on a seeded synthetic clip stream, data-parallel under torchrun (one process per GPU, NCCL) or in
     one process. Rank 0 logs every 5 steps and saves the TVAE's state_dict every --evaluate_every_n_steps steps; with
     --eval_clips K it first scores K held-out clips (VideoTrainer.evaluate) and logs eval_psnr, eval_ssim and
-    eval_lpips."""
+    eval_lpips. With --ema_decay D it also saves the averaged weights as tvae_ema_step_<k>.pt (a TVAE state_dict) and,
+    with --eval_clips, logs eval_ema_psnr, eval_ema_ssim and eval_ema_lpips."""
     # arguments are checked before anything touches a device
+    if ema_decay is not None and not 0.0 < ema_decay < 1.0:
+        raise click.BadParameter(f"must satisfy 0 < D < 1, got {ema_decay}", param_hint="--ema_decay")
     if eval_clips < 0:
         raise click.BadParameter(f"must be >= 0, got {eval_clips}", param_hint="--eval_clips")
     if perceptual_frames is not None and not 1 <= perceptual_frames <= clip_frames:
@@ -360,7 +378,7 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
     if clip_frames % div or resolution % div:
         raise click.BadParameter(f"--clip_frames ({clip_frames}) and --resolution ({resolution}) must be multiples of "
                                  f"{div} for {len(ch_mult)} levels", param_hint="--vae_ch_mult")
-    extra = {}  # the clip discriminator's settings and eval_clips, passed only when used
+    extra = {}  # the clip discriminator's settings, eval_clips and ema_decay, passed only when used
     if do_clip_ganloss:
         if clip_disc_ch <= 0 or clip_disc_ch % 32 or clip_disc_ch > 256:
             raise click.BadParameter(f"must be a multiple of 32 up to 256, got {clip_disc_ch}",
@@ -375,6 +393,8 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
         extra["clip_disc"] = (clip_disc_ch, clip_disc_layers, lr)
     if eval_clips:
         extra["eval_clips"] = eval_clips
+    if ema_decay is not None:
+        extra["ema_decay"] = ema_decay
 
     assert torch.cuda.is_available(), "CUDA is required"
     rank = int(os.environ.get("RANK", "0"))
@@ -394,9 +414,10 @@ def train_video(batch_size, clip_frames, resolution, perceptual_frames, do_ganlo
 def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_frames, do_ganloss, disc_type, use_lecam,
                  no_lpips, recompute, learning_rate_vae, learning_rate_disc, vae_ch, ch_mult, vae_num_res_blocks,
                  vae_z_channels, max_steps, evaluate_every_n_steps, load_path, run_name, seed, clip_disc=None,
-                 eval_clips=0):
+                 eval_clips=0, ema_decay=None):
     """clip_disc: (ch, n_layers, learning rate) of a tae_disc.PatchDiscriminator3D to train against, or None.
-    eval_clips: the number of held-out clips rank 0 scores at every checkpoint."""
+    eval_clips: the number of held-out clips rank 0 scores at every checkpoint.
+    ema_decay: keep a weight EMA (VideoTrainer) and save it, and score it, at every checkpoint; None: no EMA."""
     import tae_disc
     import utils
 
@@ -415,7 +436,7 @@ def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_f
                        lr_clip_disc=lr)
     tr = VideoTrainer(vae.to(device), lpips, disc, disc_type=disc_type, use_lecam=use_lecam,
                       perceptual_frames=perceptual_frames, lr_vae=learning_rate_vae, lr_disc=learning_rate_disc,
-                      recompute=recompute, **clip_kw)
+                      recompute=recompute, ema_decay=ema_decay, **clip_kw)
     lr_scheduler = cosine_with_warmup(tr.optimizer_G, 200, max_steps)
     clips = iter(SyntheticLoader(batch_size, resolution, frames=clip_frames))  # seed 42 + rank
     held_out = []
@@ -458,10 +479,18 @@ def _train_video(rank, device, batch_size, clip_frames, resolution, perceptual_f
                 ev = tr.evaluate(c.to(device, non_blocking=True) for c in held_out)
                 logger.info(f"step {step + 1} - " + "\n\t".join(f"eval_{k}: {ev[k]:.4f}" for k in
                                                                   ("psnr", "ssim", "lpips") if k in ev))
+                if tr.vae_ema is not None:
+                    ev = tr.evaluate((c.to(device, non_blocking=True) for c in held_out), ema=True)
+                    logger.info(f"step {step + 1} - " + "\n\t".join(f"eval_ema_{k}: {ev[k]:.4f}" for k in
+                                                                      ("psnr", "ssim", "lpips") if k in ev))
             os.makedirs(f"./ckpt/{run_name}", exist_ok=True)
             ck = f"./ckpt/{run_name}/tvae_step_{step + 1}.pt"
             torch.save({k: v.detach().cpu() for k, v in tr.vae.state_dict().items()}, ck)
             logger.info(f"Saved checkpoint to {ck}")
+            if tr.vae_ema is not None:  # the averaged weights, loadable by --load_path and tae.TVAE.load_state_dict
+                ck = f"./ckpt/{run_name}/tvae_ema_step_{step + 1}.pt"
+                torch.save({k: v.detach().cpu() for k, v in tr.vae_ema.state_dict().items()}, ck)
+                logger.info(f"Saved checkpoint to {ck}")
 
 
 if __name__ == "__main__":

@@ -226,6 +226,7 @@ class FlatAllReduceDDP(nn.Module):
         self._flat = None
         self._store = None
         self._ranges = None
+        self.after_load = None  # load_vae_checkpoint calls this after the weights changed (a trainer's EMA restart)
 
     def forward(self, *a, **k):
         return self.module(*a, **k)
@@ -351,7 +352,8 @@ def latent_augment(z, z_s, real_images_hr, flip_invariance, crop_invariance, dow
 def load_vae_checkpoint(vae_ddp: nn.Module, path_or_state):
     """vae_trainer.py:505-513: strict load of a `module.`-prefixed VAE checkpoint (what the reference saves at :903-906);
     on failure the `_orig_mod.` infixes a torch.compile'd encoder/decoder leaves in the keys are stripped and the strict
-    load is retried. After loading, the cached bf16 GEMM operands are refreshed."""
+    load is retried. After loading, the cached bf16 GEMM operands are refreshed and, when the wrapper belongs to a
+    trainer that keeps a weight EMA, that average restarts from the loaded weights."""
     state_dict = torch.load(path_or_state, map_location="cpu") if isinstance(path_or_state, (str, os.PathLike)) \
         else path_or_state
     try:
@@ -365,6 +367,8 @@ def load_vae_checkpoint(vae_ddp: nn.Module, path_or_state):
         import ops
 
         ops.weights_updated(list(vae_ddp.parameters()))
+    if getattr(vae_ddp, "after_load", None) is not None:
+        vae_ddp.after_load()
     return status
 
 
@@ -381,6 +385,19 @@ def make_image_grid(images: torch.Tensor, D: int) -> torch.Tensor:
     return canvas
 
 
+@torch.no_grad()
+def restart_ema(optimizer, live: nn.Module, averaged: nn.Module):
+    """Restarts `optimizer`'s weight EMA from the current weights of `live` and copies `live`'s frozen parameters and
+    buffers into `averaged` (its FlatAdamW.averaged_copy)."""
+    optimizer.reset_ema()
+    trained = {id(p) for p in optimizer.store.plist}
+    for a, b in zip(averaged.parameters(), live.parameters()):
+        if id(b) not in trained:
+            a.copy_(b)
+    for a, b in zip(averaged.buffers(), live.buffers()):
+        a.copy_(b)
+
+
 class Trainer:
     """One object = the state of vae_trainer.py:422-522 (models, optimizers, scheduler, LeCam anchors); `.step(batch)`
     = one iteration of the loop body :530-708. bench.py and the tests drive this same public class."""
@@ -391,9 +408,16 @@ class Trainer:
                  do_clamp=False, clamp_th=8.0, crop_invariance=False, flip_invariance=False,
                  augment_before_perceptual_loss=False, downscale_factor=16, use_lecam=False, disc_type="bce",
                  lpips_eval=True, seed=42, use_vq=False, vq_codebook_size=8192, vq_beta=0.25, cuda_graph=None,
-                 recompute=False):
+                 recompute=False, ema_decay=None):
         """recompute=True: ae.enable_recompute on the VAE, so that every ResnetBlock keeps only its input for the
-        backward (larger batches or resolutions per GPU for one extra conv1 and two GroupNorm apply passes per block)."""
+        backward (larger batches or resolutions per GPU for one extra conv1 and two GroupNorm apply passes per block).
+        ema_decay (0 < d < 1): keep an exponential moving average of the VAE's weights (every parameter of optimizer_G,
+        the VQ codebook included) in the fused AdamW launch (flat.FlatAdamW); `vae_ema` is an ae.VAE over it. None: no
+        average (vae_ema is None)."""
+        if ema_decay is not None:
+            from flat import check_ema_decay
+
+            ema_decay = check_ema_decay(ema_decay)  # before any device work
         self.device = device
         # CUDA-graph the whole step (forward, backward, NCCL collectives, optimizers, weight re-pack): ~600-1100 launches
         # per step otherwise keep the host within ~10 % of being the limiter. Auto-enabled (None) when no host-side
@@ -448,11 +472,16 @@ class Trainer:
                   {"params": [p for n, p in named if "conv_in" in n], "lr": 1e-4}]
         if use_vq:
             groups.append({"params": [p for n, p in named if "reg.embedding" in n], "lr": learning_rate_vae})
-        self.optimizer_G = FlatAdamW(groups, weight_decay=1e-3, betas=(0.9, 0.95))
+        self.optimizer_G = FlatAdamW(groups, weight_decay=1e-3, betas=(0.9, 0.95), ema_decay=ema_decay)
         self.optimizer_D = FlatAdamW([{"params": list(self.discriminator.parameters()), "lr": learning_rate_disc}],
                                      weight_decay=1e-3, betas=(0.9, 0.95))
         self.vae.attach_store(self.optimizer_G.store)
         self.discriminator.attach_store(self.optimizer_D.store)
+        # [extension] the weight EMA (DESIGN.md section 7 row 26): the autoencoder only, started after the broadcast above
+        self.vae_ema = None
+        if ema_decay is not None:
+            self.vae_ema = self.optimizer_G.averaged_copy(vae)
+            self.vae.after_load = lambda: restart_ema(self.optimizer_G, self.vae.module, self.vae_ema)
         self.lpips = LPIPS().to(device)
         from utils import broadcast_module_state
 
@@ -625,25 +654,28 @@ class Trainer:
         return out
 
     @torch.no_grad()
-    def evaluate(self, test_batches, max_batches=2):
+    def evaluate(self, test_batches, max_batches=2, ema=False):
         """vae_trainer.py:811-893 (rank 0): encode the 256^2 area-resized test images, clamp, reg, [flip_invariance: decode
         the (-1,-2)-flipped latent with its last four channels negated and flip the image back, :837-861], decode,
-        un-normalise to [0,1]. -> (test grid, reconstruction grid) as (3, 4D, 4D) tensors + the raw tensors."""
-        vae = self.vae
+        un-normalise to [0,1]. -> (test grid, reconstruction grid) as (3, 4D, 4D) tensors + the raw tensors.
+        ema=True reconstructs with the averaged weights (vae_ema) instead of the trained ones."""
+        if ema and self.vae_ema is None:
+            raise ValueError("evaluate(ema=True): this trainer keeps no weight EMA (ema_decay=None)")
+        model = self.vae_ema if ema else self.vae.module
         all_test, all_rec = [], []
         for batch in test_batches:
             ori = (batch[0] if isinstance(batch, (tuple, list)) else batch).to(self.device)
             x = F.interpolate(ori, size=(256, 256), mode="area") if ori.shape[-2:] != (256, 256) else ori
-            z = vae.module.encoder(x)
+            z = model.encoder(x)
             if self.do_clamp:
                 z = z.clamp(-self.clamp_th, self.clamp_th)
-            z_s = vae.module.reg(z)
+            z_s = model.reg(z)
             if isinstance(z_s, tuple):
                 z_s = z_s[0]
             if self.flip_invariance:
                 z_s = torch.flip(z_s, [-1, -2]).clone()
                 z_s[:, -4:] = -z_s[:, -4:]
-            rec = vae.module.decoder(z_s.contiguous())
+            rec = model.decoder(z_s.contiguous())
             ori, rec = (ori * 0.5 + 0.5).clamp(0, 1), (rec * 0.5 + 0.5).clamp(0, 1)
             if self.flip_invariance:
                 rec = torch.flip(rec, [-1, -2])
