@@ -480,6 +480,22 @@ int vqb_pack_weights_multi(const VqbPackJob* jobs_dev, int njobs, int total_bloc
 int vqb_psnr_ssim(const void* x, const void* y, int bf16, int B, int C, int T, int H, int W, float lo, float hi,
                   float* psnr, float* ssim, float* work, int64_t work_elems, void* stream);
 
+/*
+ * Tiled encode / decode blend (DESIGN.md section 3.11, definition in section 7 row 27; the reference has none):
+ * accumulates one tile [N][C][Lt][Lh][Lw] (contiguous, fp32: tile_bf16 = 0, bf16: 1) into the fp32 grid acc
+ * [N][C][T][H][W] at window (t0, h0, w0). wt, wh, ww: the tile's fp32 weight tables of Lt, Lh, Lw entries. Per element,
+ * p = (wt[t] * wh[h]) * ww[w] rounded in that order; where every grid coordinate is >= its axis's prev_end (the end of
+ * the previous tile on that axis, or the window start) acc = p * v, otherwise acc = fmaf(p, v, acc). Where every grid
+ * coordinate is < its axis's next_start (the start of the next tile on that axis, or the extent) and out_bf16 is not
+ * null, out_bf16 [N][C][T][H][W] = bf16_rn(acc). Launched per tile in raster order, this writes every element without a
+ * memset or atomics, and rounds each bf16 output element once. Window inside the grid, t0 <= prev_end_t <= t0 + Lt,
+ * t0 <= next_start_t <= T (likewise h, w), pointers aligned to their element size; otherwise VQB_EINVAL. One launch.
+ */
+int vqb_tile_blend(const void* tile, int tile_bf16, float* acc, void* out_bf16, int N, int C, int T, int H, int W,
+                   int Lt, int Lh, int Lw, int t0, int h0, int w0, const float* wt, const float* wh, const float* ww,
+                   int prev_end_t, int prev_end_h, int prev_end_w, int next_start_t, int next_start_h,
+                   int next_start_w, void* stream);
+
 /* library / device info */
 const char* vqb_last_error(void);
 int vqb_version(void);

@@ -166,6 +166,7 @@ def load():
         "vqb_leaky_relu_fwd": (i32, [vp, vp, i64, vp]),
         "vqb_leaky_relu_bwd": (i32, [vp, vp, vp, i64, vp]),
         "vqb_psnr_ssim": (i32, [vp, vp] + [i32] * 6 + [f32, f32, vp, vp, vp, i64, vp]),
+        "vqb_tile_blend": (i32, [vp, i32, vp, vp] + [i32] * 11 + [vp, vp, vp] + [i32] * 6 + [vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name, None)
